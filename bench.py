@@ -1,17 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- frames/sec of the CLIP ViT-B/32 hot path (BASELINE.json configs[1]) on N B200s.
+"""bench.py -- frames/sec of the CLIP ViT-B/32 hot path (BASELINE.json configs[1]) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (uint8 frames -> transform -> ViT-B/32 tower -> (n,512) fp32 features)
 over one batch of 1000 synthetic 224x224x3 uint8 frames per GPU.  Prints ONE JSON line (rank 0):
   value     whole-job frames/s, inputs resident in HBM, CUDA-event timed, max over ranks
   e2e       same metric through the host-buffer C-ABI call (pinned host frames in, host features out; the H2D and
             D2H copies are inside the timed region)
-  roofline  tensor-pipe roofline of the dominant kernel (the tcgen05 GEMM), from per-launch CUDA events
+  roofline  tensor-pipe roofline of the dominant kernel (the wgmma GEMM), from per-launch CUDA events
   cpu_baseline  the oracle port (PIL transform + fp32 torch tower) timed on this box's host cores (N=1, rank 0)
 `--impl reference` times only that CPU path (the reference's `--cpu` path restated; see DESIGN.md) and prints the
 same line with "impl": "reference".
+`--dump-outputs DIR` writes the (1000, 512) fp32 features of the last timed step (rank 0) as DIR/clip_features.npy;
+inputs and weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -61,28 +63,10 @@ def base_config(n_gpus: int) -> dict:
         "frame": "224x224x3 uint8 HWC",
         "weights": "synthetic, seed 0, openai visual.* layout (real CLIP weights are not available offline)",
         "accumulate": "fp32",
-        "l2": "inputs are 150.5 MB per step per GPU > 126 MB L2 (no explicit flush needed)",
+        "l2": "inputs are 150.5 MB per step per GPU > 50 MB L2 (no explicit flush needed)",
         "parallelism": f"dp{n_gpus}: frame list sharded per rank, one NCCL all_gather of the (n,512) features per step "
                        "(side stream: overlaps the next step's tower)" if n_gpus > 1 else "dp1",
     }
-
-
-def ncu_traffic_per_launch():
-    """Mean DRAM bytes (read + write) per launch of the dominant kernel, from the committed ncu --set full capture
-    (profiles/r2_prof_gemm_raw.csv, else round 1's: consecutive GEMM launches of one 250-frame chunk); None if absent."""
-    import csv
-    p = os.path.join(ROOT, "profiles", "r2_prof_gemm_raw.csv")
-    if not os.path.exists(p):
-        p = os.path.join(ROOT, "profiles", "r1_prof_gemm_raw.csv")
-    try:
-        rows = list(csv.reader(open(p)))
-        hdr, units, data = rows[0], rows[1], rows[2:]
-        mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        ir, iw = hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-        tot = [float(d[ir]) * mult[units[ir]] + float(d[iw]) * mult[units[iw]] for d in data]
-        return sum(tot) / len(tot)
-    except Exception:
-        return None
 
 
 def load_peaks() -> dict:
@@ -92,8 +76,9 @@ def load_peaks() -> dict:
         return {"tflops_sustained": float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1400.0))),
                 "tflops_burst": float(d.get("bf16_tflops", 1590.0)), "hbm_gbs": float(d.get("hbm_gbs", 6650.0)),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_sustained": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W part): dense FP16 989 TFLOP/s, HBM3 3.35 TB/s -- a ceiling, not a measurement
+    return {"tflops_sustained": 989.0, "tflops_burst": 989.0, "hbm_gbs": 3350.0,
+            "source": "fallback (H100 SXM data sheet)"}
 
 
 # ----------------------------------------------------------------------------------------- clocks
@@ -229,7 +214,7 @@ def cpu_model_name() -> str:
 def run_reference(args, rank: int) -> None:
     if rank != 0:
         return
-    steps = min(max(args.steps, 1), 10)        # each step is a bounded sample; the whole arm stays within minutes
+    steps = max(args.steps, 1)                 # each step is a bounded sample: the budget below is shared by all steps
     ts, cores, sample = time_cpu(steps, min(max(args.warmup, 1), 3), budget_s=30.0)
     total = sum(ts)
     value = sample * len(ts) / total
@@ -292,10 +277,13 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
         y.record_stream(side)
         tick[0] += 1
 
+    last = {}
+
     def step_dev():
         y = eng.encode_frames_u8(frames_dev)
         if world > 1:
             gather_async(y)
+        last["y"] = y
         return y
 
     def step_host():
@@ -344,6 +332,10 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
     clocks = sampler.stop() if sampler else None
     launches = (eng.launch_count - launches0) // K
     value = world * n * K / (ms_total / 1e3)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "clip_features.npy"), last["y"].float().cpu().numpy())
 
     # end-to-end through the host-buffer entry point
     for _ in range(2):
@@ -352,7 +344,7 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
     ms_e2e = timed(step_host, K, drain_host)
     e2e_value = world * n * K / (ms_e2e / 1e3)
 
-    # roofline of the dominant kernel: per-launch CUDA events around every tcgen05 GEMM launch, separate pass over
+    # roofline of the dominant kernel: per-launch CUDA events around every wgmma GEMM launch, separate pass over
     # the same steps so the timed region above is not perturbed
     eng.profile(True)
     pk = min(K, 5)
@@ -364,7 +356,7 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
     peaks = load_peaks()
     # algorithmic FLOPs of the reference's GEMMs (SURVEY.md 8d) over the measured GEMM time; the engine executes
     # 5.9 % fewer (the last block's out-proj / MLP run on the CLS rows only), reported separately
-    # The dominant kernel is the plain tcgen05 GEMM (patch embedding, out-proj, fc1, fc2, final projection; plus QKV when
+    # The dominant kernel is the plain wgmma GEMM (patch embedding, out-proj, fc1, fc2, final projection; plus QKV when
     # VF_CLIP_ATTN=split).  With the default fused path the QKV projection runs inside vf::qkv_attention_kernel together
     # with the attention core: that kernel is timed as its own class ("attention") and reported under `qkv_attention`.
     fused = not os.environ.get("VF_CLIP_ATTN", "").startswith("s")
@@ -373,11 +365,11 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
     achieved = alg_flop * n * pk / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
     executed = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
     roofline = {
-        "bound": "tensor", "kernel": "vf::gemm_f16_pair_kernel + vf::qkv_attention_kernel (tcgen05.mma cta_group::2 kind::f16, fp32 "
-                                     "accumulate in TMEM)",
+        "bound": "tensor", "kernel": "vf::gemm_f16_kernel + vf::qkv_attention_kernel (wgmma m64nNk16 f16, fp32 "
+                                     "accumulate in registers)",
         "achieved": achieved, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
-        "frac": achieved / peaks["tflops_sustained"], "peak_source": peaks["source"] + ", bf16 dense sustained",
-        "traffic": ncu_traffic_per_launch(), "traffic_unit": "bytes/launch (ncu dram__bytes_read+write, mean of 4 launches)",
+        "frac": achieved / peaks["tflops_sustained"], "peak_source": peaks["source"] + ", fp16 dense",
+        "traffic": None,
         "executed_tflops": executed,
         "executed_over_algorithmic": gemm_flops / (alg_flop * n * pk),
         "algorithmic_gflop_per_frame": alg_flop / 1e9,
@@ -385,7 +377,7 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
         "algorithmic_flop_per_launch_avg": alg_flop * n * pk / max(gemm_launches, 1),
         "gemm_share_of_step": (gemm_ms / pk) / (ms_total / K),
         "eager_ms_per_step_by_kernel": cats,
-        "qkv_attention": ({"kernel": "vf::qkv_attention_kernel (QKV projection on tcgen05 + 50-token attention on mma.sync in the epilogue)",
+        "qkv_attention": ({"kernel": "vf::qkv_attention_kernel (QKV projection on wgmma + 50-token attention on mma.sync in the epilogue)",
                            "algorithmic_gflop_per_frame": (QKV_FLOP + ATT_CORE_FLOP) / 1e9, "ms_per_step": cats.get("attention", 0.0),
                            "achieved_tflops": (QKV_FLOP + ATT_CORE_FLOP) * n / (cats["attention"] / 1e3) / 1e12 if cats.get("attention") else None,
                            "frac": ((QKV_FLOP + ATT_CORE_FLOP) * n / (cats["attention"] / 1e3) / 1e12 / peaks["tflops_sustained"])
@@ -393,7 +385,7 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
         "whole_step_tflops": value / world * FLOP_PER_FRAME / 1e12,
         "whole_step_frac": value / world * FLOP_PER_FRAME / 1e12 / peaks["tflops_sustained"],
         # the memory-bound kernels against the HBM roofline: ALGORITHMIC bytes per frame (DESIGN.md 4) over their
-        # event-timed device time; the chunk's activations partly live in the 126 MB L2, so > 1 is possible
+        # event-timed device time; the chunk's activations partly live in the 50 MB L2, so > 1 is possible
         "hbm": {k: {"algorithmic_bytes_per_frame": b, "ms_per_step": cats.get(k, 0.0),
                     "achieved_gbs": (b * n / (cats[k] / 1e3) / 1e9) if cats.get(k) else None,
                     "frac_of_hbm_peak": (b * n / (cats[k] / 1e3) / 1e9 / peaks["hbm_gbs"]) if cats.get(k) else None}
@@ -510,20 +502,22 @@ def run_engine(args, rank: int, world: int, local_rank: int) -> None:
 
 # ----------------------------------------------------------------------------------------- secondary workloads
 # BASELINE.json configs[2] (I3D rgb, 64-frame 224x224 stacks) and configs[3] (RAFT on 480x270 pairs -> I3D flow).
-# They print the same kind of JSON line (metric stacks/s resp. pairs/s) for profiles/; the headline stays CLIP.
+# They print the same kind of JSON line (metric stacks/s resp. pairs/s); the headline stays CLIP.
 I3D_GFLOP = {"rgb": 222.30, "flow": 204.68}          # per 64-frame stack (SURVEY.md 8d / Appendix A)
 RAFT_GFLOP_272x480 = 309.82                          # per pair, 20 iterations, reference algorithm (SURVEY.md 8d)
 
 
 def _weights(kind: str):
-    """Reference checkpoint copy if present (checkpoints/), else seeded synthetic weights."""
+    """Reference checkpoint copy if present (oracle/_ref/checkpoints/, made by build()), else seeded weights: the I3D
+    synthetic state dict, and for RAFT the stand-in with the trained tensors' statistics (oracle/stand_in.py; RAFT with
+    plain random weights is not a meaningful dynamical system)."""
     import torch
-    p = os.path.join(ROOT, "checkpoints", {"rgb": "i3d_rgb.pt", "flow": "i3d_flow.pt", "raft": "raft-sintel.pth"}[kind])
+    p = os.path.join(ROOT, "oracle", "_ref", "checkpoints", {"rgb": "i3d_rgb.pt", "flow": "i3d_flow.pt", "raft": "raft-sintel.pth"}[kind])
     if os.path.exists(p):
         return torch.load(p, map_location="cpu"), "reference checkpoint"
-    from oracle import i3d_net
+    from oracle import i3d_net, stand_in
     if kind == "raft":
-        raise SystemExit("bench --workload raft needs checkpoints/raft-sintel.pth (scripts/fetch_checkpoints.py)")
+        return stand_in.state_dict("raft-sintel.pth"), "seeded stand-in of raft-sintel.pth (oracle/stand_in.py)"
     return i3d_net.synthetic_state_dict(kind, 0), "synthetic seed 0"
 
 
@@ -550,9 +544,9 @@ def _gemm_roofline(fn, reps, algorithmic_flops_per_step, step_ms):
     ops.gemm_profile(False)
     peaks = load_peaks()
     ach = algorithmic_flops_per_step * reps / (ms / 1e3) / 1e12 if ms > 0 else 0.0
-    return {"bound": "tensor", "kernel": "vf::gemm_f16_pair_kernel (tcgen05, shifted-row conv mode)",
+    return {"bound": "tensor", "kernel": "vf::gemm_f16_kernel (wgmma, shifted-row conv mode)",
             "achieved": ach, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s", "frac": ach / peaks["tflops_sustained"],
-            "peak_source": peaks["source"] + ", bf16 dense sustained", "traffic": None,
+            "peak_source": peaks["source"] + ", fp16 dense", "traffic": None,
             "executed_tflops": executed / (ms / 1e3) / 1e12 if ms > 0 else 0.0,
             "executed_over_algorithmic": executed / (algorithmic_flops_per_step * reps),
             "launches_per_step": launches // reps, "gemm_share_of_step": (ms / reps) / step_ms}
@@ -669,7 +663,7 @@ def smooth_frames(n: int, h: int, w: int, seed: int, shift=(1.7, -0.9)):
 
 def run_raft(args, rank: int = 0, world: int = 1, local_rank: int = 0, quick: bool = False):
     """BASELINE.json configs[3]: RAFT on 480x270 frame pairs -> I3D flow branch.  world = 2 is the configuration the
-    baseline names (2 x B200): stacks are sharded over the ranks (each runs RAFT -> I3D flow on its own 64 pairs, no
+    baseline names (2 GPUs): stacks are sharded over the ranks (each runs RAFT -> I3D flow on its own 64 pairs, no
     data-path collective) and the (1, 1024) features are all-gathered."""
     import torch
     import torch.distributed as dist
@@ -814,11 +808,11 @@ def run_b16(args, quick: bool = False):
             "e2e": {"value": n * K / (ms_e2e / 1e3), "unit": UNIT, "h2d_bytes_per_step": int(frames_host.numel()),
                     "d2h_bytes_per_step": n * 512 * 4},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "tensor", "kernel": "vf::gemm_f16_pair_kernel (QKV GEMM + attention_long_kernel: the fused kernel is 50-token only)",
+            "roofline": {"bound": "tensor", "kernel": "vf::gemm_f16_kernel (QKV GEMM + attention_long_kernel: the fused kernel is 50-token only)",
                          "achieved": gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0,
                          "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
                          "frac": (gemm_flops / (gemm_ms / 1e3) / 1e12 / peaks["tflops_sustained"]) if gemm_ms > 0 else 0.0,
-                         "peak_source": peaks["source"] + ", bf16 dense sustained", "traffic": None,
+                         "peak_source": peaks["source"] + ", fp16 dense", "traffic": None,
                          "eager_ms_per_step_by_kernel": cats}}
     eng.close()
     torch.cuda.empty_cache()
@@ -983,12 +977,17 @@ def main() -> None:
     ap.add_argument("--workload", default="clip", choices=["clip", "i3d", "raft", "c5", "b16"],
                     help="clip = the headline (BASELINE.json configs[1], with the other configs as `secondary`); i3d / raft "
                          "/ c5 = configs[2] / configs[3] / configs[4] alone")
+    ap.add_argument("--dump-outputs", default=None, dest="dump_outputs", metavar="DIR",
+                    help="write the features of the last timed headline step as DIR/clip_features.npy (fp32)")
     ap.add_argument("--no-secondary", action="store_true", dest="no_secondary",
                     help="headline only: skip the secondary workloads (c5 video list, I3D, RAFT -> I3D flow)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.dump_outputs and (args.impl == "reference" or args.workload != "clip"):
+        print("bench.py: --dump-outputs writes the CLIP headline's features only; this run dumps nothing",
+              file=sys.stderr, flush=True)
     if args.impl == "reference":
         run_reference(args, rank)
         return

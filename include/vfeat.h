@@ -1,4 +1,4 @@
-/* libvfeat.so -- C ABI of the B200-native video-feature engine.
+/* libvfeat.so -- C ABI of the H100-native video-feature engine.
  *
  * Every entry point is `extern "C"`, takes plain pointers and sizes, returns an int status
  * (VF_OK == 0) and never throws.  Device buffers are raw CUDA device pointers owned by the
@@ -66,7 +66,7 @@ int vf_clip_normalize_u8(const uint8_t* src, int n, int src_h, int src_w, float*
  * D: fp16 or fp32 (out_f32, row pitch ldd elements, 16-byte aligned rows), bias/scale: fp32 [N] or NULL. */
 int vf_gemm_f16(const void* A, int lda, const void* B, int ldb, int M, int N, int K, void* D, int ldd, int out_f32,
                 const float* bias, const float* scale, int act, void* stream);
-/* D += act(A . B^T * scale + bias), D fp32: the add happens in the L2 (TMA reduction), each element exactly once -- the
+/* D += act(A . B^T * scale + bias), D fp32: added by fp32 global reductions from the GEMM epilogue, each element exactly once -- the
  * residual-stream update `x = x + attn(...)` / `x = x + mlp(...)` of clip/model.py ResidualAttentionBlock.forward. */
 int vf_gemm_f16_accumulate(const void* A, int lda, const void* B, int ldb, int M, int N, int K, float* D, int ldd,
                            const float* bias, const float* scale, int act, void* stream);
@@ -76,7 +76,7 @@ int vf_gemm_f16_accumulate(const void* A, int lda, const void* B, int ldb, int M
 int vf_gemm_f16_split(const void* A, int lda, const void* B, int ldb, int M, int N, int K, void* D, int ldd, int split_off,
                       const float* bias, const float* scale, int act, void* stream);
 
-/* Roofline instrumentation (bench.py): while enabled on the calling thread, every tcgen05 GEMM launch of any handle
+/* Roofline instrumentation (bench.py): while enabled on the calling thread, every wgmma GEMM launch of any handle
  * is bracketed by CUDA events on its stream.  _read synchronises the device and returns the summed device time (ms),
  * the launch count and the EXECUTED flops (2*M*N*K including zero-padded K blocks and hi/lo weight passes). */
 int vf_gemm_profile(int enable);

@@ -1,4 +1,4 @@
-"""CLI of the B200-native video-feature engine: the flags of the reference's main.py (main.py:93-149), same names,
+"""CLI of the H100-native video-feature engine: the flags of the reference's main.py (main.py:93-149), same names,
 defaults and choices.  ``--device_ids`` starts one process per GPU (reference: one thread per GPU); ``--cpu`` is
 refused -- the reference's CPU path is what ``bench.py --impl reference`` times, the engine itself has no CPU path.
 """
@@ -95,7 +95,7 @@ _FLAGS = [
 
 
 def make_parser():
-    parser = argparse.ArgumentParser(description='B200-native video feature extraction')
+    parser = argparse.ArgumentParser(description='H100-native video feature extraction')
     for flag, kw in _FLAGS:
         parser.add_argument(flag, **kw)
     return parser

@@ -14,6 +14,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF = "/root/reference"
 OUT = os.path.join(ROOT, "tests", "golden")
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from helpers import stand_in_state_dict  # noqa: E402
 
 
 def install_mmcv_shim():
@@ -143,7 +145,8 @@ def main():
 
 
 def i3d_golden():
-    """Reference I3D module + vendored checkpoints vs the restated oracle, seeded inputs; stores only the outputs."""
+    """Reference I3D module + the seeded stand-ins of its checkpoints (oracle/stand_in.py) vs the restated oracle, seeded
+    inputs; stores only the outputs."""
     import torch
     sys.path.insert(0, REF)
     cwd = os.getcwd()
@@ -153,7 +156,7 @@ def i3d_golden():
         from oracle import i3d_net
         d = {}
         for mod, cin in (("rgb", 3), ("flow", 2)):
-            sd = torch.load(f"models/i3d/checkpoints/i3d_{mod}.pt", map_location="cpu")
+            sd = stand_in_state_dict(f"i3d_{mod}.pt")
             net = I3D(num_classes=400, modality=mod).eval()
             net.load_state_dict(sd)
             for T in (16, 11):
@@ -193,7 +196,8 @@ if __name__ == "__main__" and len(sys.argv) == 1:
 
 
 def raft_golden():
-    """Reference RAFT module + vendored raft-sintel.pth vs the restated oracle on synthetic moving frames."""
+    """Reference RAFT module + the seeded stand-in of raft-sintel.pth (oracle/stand_in.py) vs the restated oracle on
+    synthetic moving frames."""
     import torch
     sys.path.insert(0, REF)
     cwd = os.getcwd()
@@ -201,7 +205,7 @@ def raft_golden():
     try:
         from models.raft.raft_src.raft import RAFT, InputPadder
         from oracle import raft_net
-        sd = torch.load("models/raft/checkpoints/raft-sintel.pth", map_location="cpu")
+        sd = stand_in_state_dict("raft-sintel.pth")
         net = torch.nn.DataParallel(RAFT(), device_ids=None)
         net.load_state_dict(sd)
         net = net.module.eval()

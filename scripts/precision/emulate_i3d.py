@@ -1,5 +1,5 @@
 """CPU emulation behind DESIGN.md §2 (I3D): which fp16-rounded tensors make up the feature error of the trained rgb
-checkpoint on a uniform-noise clip (T = 16).  Needs checkpoints/i3d_rgb.pt.
+checkpoint on a uniform-noise clip (T = 16).  Needs oracle/_ref/checkpoints/i3d_rgb.pt.
 
 Measured in the build container (rel-L2 / max-abs relative to max |feature|, weights fp32, seed 1 / seed 116):
     every conv input rounded to fp16                       8.1e-04 / 8.6e-04      8.0e-04 / 7.4e-04
@@ -19,7 +19,7 @@ from oracle import i3d_net as N
 
 def main(seed=116):
     torch.set_num_threads(os.cpu_count() or 1)
-    sd = torch.load(os.path.join(ROOT, "checkpoints", "i3d_rgb.pt"), map_location="cpu")
+    sd = torch.load(os.path.join(ROOT, "oracle", "_ref", "checkpoints", "i3d_rgb.pt"), map_location="cpu")
     x = torch.rand(1, 3, 16, 224, 224, generator=torch.Generator().manual_seed(seed)) * 2 - 1
     ref = N.forward_features(sd, x)
     orig = N._unit

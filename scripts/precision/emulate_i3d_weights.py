@@ -11,7 +11,7 @@ from oracle import i3d_net as N
 
 def main(mod="rgb", seed=116):
     torch.set_num_threads(os.cpu_count() or 1)
-    sd = torch.load(os.path.join(ROOT, "checkpoints", f"i3d_{mod}.pt"), map_location="cpu")
+    sd = torch.load(os.path.join(ROOT, "oracle", "_ref", "checkpoints", f"i3d_{mod}.pt"), map_location="cpu")
     cin = 3 if mod == "rgb" else 2
     x = torch.rand(1, cin, 16, 224, 224, generator=torch.Generator().manual_seed(seed)) * 2 - 1
     ref = N.forward_features(sd, x)

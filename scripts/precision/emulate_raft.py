@@ -1,6 +1,6 @@
 """CPU emulation behind DESIGN.md §2 (RAFT): how much of the flow error on block-compressed frames comes from rounding
 which operand to fp16.  Runs the oracle (fp32 torch, CPU) on 6 decoded frames of a synthetic 128x160 mp4 and perturbs
-one operand group at a time.  Needs checkpoints/raft-sintel.pth (scripts/fetch_checkpoints.py) and cv2.
+one operand group at a time.  Needs oracle/_ref/checkpoints/raft-sintel.pth (oracle/fetch_ref.py) and cv2.
 
 Measured in the build container (rel-L2 / max-abs relative to max |flow|, 20 iterations):
     fp32, 16 threads vs 1 thread (summation order only)          2.6e-05 / 2.8e-04
@@ -38,7 +38,7 @@ def compressed_frames(path="/tmp/_raft_emul.mp4"):
 
 def main():
     torch.set_num_threads(os.cpu_count() or 1)
-    sd = torch.load(os.path.join(ROOT, "checkpoints", "raft-sintel.pth"), map_location="cpu")
+    sd = torch.load(os.path.join(ROOT, "oracle", "_ref", "checkpoints", "raft-sintel.pth"), map_location="cpu")
     x = compressed_frames()
     ref = R.forward(sd, x[:-1], x[1:], 20)
     err = lambda y: (float((y - ref).norm() / ref.norm()), float((y - ref).abs().max() / ref.abs().max()))

@@ -7,9 +7,9 @@ little motion (few grey levels in use, small input norm) that is a large relativ
 
 This script runs the fp32 oracle (CPU) on the two clips the -m gpu composite tests use and reports, for Gaussian flow
 perturbations of sigma px (seeded, 3 draws each), the relative L2 change of the oracle's own 1024-d feature:
-    python scripts/precision/flow_quantiser_sensitivity.py            # prints a table, writes profiles/r2_flow_sensitivity.json
+    python scripts/precision/flow_quantiser_sensitivity.py            # prints a table and the JSON report
 `feature_sensitivity()` is what tests/test_extract_i3d_raft_gpu.py imports to derive its bar from the engine's measured
-flow error.  Needs checkpoints/{raft-sintel.pth,i3d_flow.pt} (scripts/fetch_checkpoints.py) and cv2.
+flow error.  Needs oracle/_ref/checkpoints/{raft-sintel.pth,i3d_flow.pt} (oracle/fetch_ref.py) and cv2.
 """
 import json
 import os
@@ -61,8 +61,8 @@ def main():
     from PIL import Image
     import cv2
     torch.set_num_threads(os.cpu_count() or 1)
-    sd_raft = torch.load(os.path.join(ROOT, "checkpoints", "raft-sintel.pth"), map_location="cpu")
-    sd_flow = torch.load(os.path.join(ROOT, "checkpoints", "i3d_flow.pt"), map_location="cpu")
+    sd_raft = torch.load(os.path.join(ROOT, "oracle", "_ref", "checkpoints", "raft-sintel.pth"), map_location="cpu")
+    sd_flow = torch.load(os.path.join(ROOT, "oracle", "_ref", "checkpoints", "i3d_flow.pt"), map_location="cpu")
     report = {}
     for name, shift in CLIPS.items():
         path = f"/tmp/_flow_sens_{name}.mp4"
@@ -100,8 +100,7 @@ def main():
               f"-> feature rel-L2 {self_noise['feature_rel']:.3e}")
         for k, v in sens.items():
             print(f"   sigma {k:g} px -> feature rel-L2 {v['feature_rel']:.3e}   ({100 * v['levels_changed_frac']:.3f} % of levels changed)")
-    os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
-    json.dump(report, open(os.path.join(ROOT, "profiles", "r2_flow_sensitivity.json"), "w"), indent=1)
+    print(json.dumps(report, indent=1))
 
 
 if __name__ == "__main__":

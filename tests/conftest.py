@@ -9,22 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
     try:
         import torch
         torch.backends.cuda.matmul.allow_tf32 = False
         torch.backends.cudnn.allow_tf32 = False
     except Exception:
         pass
-
-
-def pytest_sessionstart(session):
-    """The real-checkpoint parity tests never skip: in the build container the reference's vendored weights are copied
-    into ./checkpoints/ on demand (the GPU box receives that folder with the snapshot)."""
-    need = [os.path.join(ROOT, "checkpoints", n) for n in ("i3d_rgb.pt", "i3d_flow.pt", "raft-sintel.pth")]
-    if not all(os.path.exists(n) for n in need) and os.path.isdir("/root/reference/models"):
-        import subprocess
-        subprocess.call([sys.executable, os.path.join(ROOT, "scripts", "fetch_checkpoints.py")])
 
 
 @pytest.fixture(scope="session")

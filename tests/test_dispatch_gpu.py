@@ -1,6 +1,6 @@
 """--device_ids dispatch on real GPUs: one process per GPU, NCCL group, ExtractCLIP over a shard each, ONE all-gather of
 every video's (T, 512) block (reference: main.py:11-55 -- threads, no gather).  Needs >= 2 GPUs on the box
-(`gpurun --gpus 2 -- python -m pytest tests/test_dispatch_gpu.py -m gpu`); on a 1-GPU box only the single-device form
+(`python -m pytest tests/test_dispatch_gpu.py -m gpu`); on a 1-GPU machine only the single-device form
 (no process group) runs."""
 import argparse
 import functools
@@ -42,7 +42,7 @@ def _save(target, blocks):
 @pytest.mark.parametrize("n_dev", [1, 2])
 def test_parallel_feature_extraction_nccl(cuda_device, tmp_path, n_dev):
     if torch.cuda.device_count() < n_dev:
-        pytest.skip(f"needs {n_dev} GPUs, this box has {torch.cuda.device_count()} (run under `gpurun --gpus 2`)")
+        pytest.skip(f"needs {n_dev} GPUs, this box has {torch.cuda.device_count()} (run it on a machine with two GPUs)")
     from video_features_b200.dispatch import parallel_feature_extraction
     vids = []
     for i in range(7):

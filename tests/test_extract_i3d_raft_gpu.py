@@ -11,7 +11,14 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 import sys
 sys.path.insert(0, os.path.join(ROOT, "scripts", "precision"))
-from helpers import checkpoint  # noqa: E402  (a missing checkpoint copy FAILS these tests, it never skips them)
+from helpers import checkpoint, checkpoint_dir  # noqa: E402  (seeded stand-ins of the reference checkpoints)
+
+
+@pytest.fixture(autouse=True)
+def _reference_weights(monkeypatch):
+    """The extractors look their weights up in $VF_CKPT_DIR / ./checkpoints: point them at the stand-in files."""
+    from video_features_b200.extract import extract_i3d
+    monkeypatch.setattr(extract_i3d, "_CKPT_DIRS", [checkpoint_dir()])
 
 
 def _write_video(path, n, h=120, w=160, fps=25.0, shift=(0.8, 0.5)):
@@ -76,7 +83,7 @@ def test_extract_i3d_two_streams_vs_oracle(cuda_device, tmp_path, clip, shift):
     # The flow stream passes through the reference's 8-bit quantiser `round(128 + 255/40 f)` (transforms.py:43-51), a
     # staircase: a flow perturbation of 1e-5 px already moves the oracle's OWN feature by 3e-3 .. 4e-3 on these clips, and
     # the fp32 oracle with a different thread count differs from itself by more than that
-    # (scripts/precision/flow_quantiser_sensitivity.py -> profiles/r2_flow_sensitivity.json).  No implementation whose
+    # (scripts/precision/flow_quantiser_sensitivity.py).  No implementation whose
     # flow differs from the oracle's at all can therefore be held to 1e-3 on the composite.  The bar is derived, not
     # guessed: (1) the engine's flow must meet the 1e-3 RAFT bar on this very clip, (2) quantiser + I3D on identical flow
     # is asserted elsewhere (test_i3d_gpu.py, 2e-4), and (3) the composite may not exceed 2x the oracle's own
@@ -89,7 +96,7 @@ def test_extract_i3d_two_streams_vs_oracle(cuda_device, tmp_path, clip, shift):
     flow_max = float(d.abs().max()) / float(flow.abs().max())
     # rel-L2 at the RAFT bar; the max-abs half is asserted on the RAFT tests proper (test_raft_gpu.py, ExtractRAFT below).
     # Here every third "pair" is the SAME decoded frame twice (a 20-frame video resampled to 65 indices): RAFT on identical
-    # frames is a badly conditioned iteration and single pixels move by a few 1e-3 px (measured 3.2e-3 of max |flow|).
+    # frames is a badly conditioned iteration and single pixels move by a few 1e-3 px.
     assert flow_rel <= 1e-3 and flow_max <= 5e-3, (flow_rel, flow_max)
     sens = feature_sensitivity(sd_flow, flow, [flow_rms], draws=5)[flow_rms]["feature_rel"]
     bar = max(1e-3, 2.0 * sens)

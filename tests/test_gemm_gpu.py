@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (vf_gemm_f16 through the C ABI) against a plain fp32 torch reference of the same op."""
+"""wgmma GEMM (vf_gemm_f16 through the C ABI) against a plain fp32 torch reference of the same op."""
 import pytest
 import torch
 
@@ -134,7 +134,7 @@ def test_gemm_rejects_bad_arguments(cuda_device):
 
 @pytest.mark.parametrize("M,N,K", [(300, 256, 768), (6000, 768, 768), (6000, 768, 3072), (77, 96, 200), (250, 768, 768)])
 def test_gemm_accumulate_adds_into_fp32_output(cuda_device, M, N, K):
-    """out += a @ b.T + bias (TMA reduction in the L2): twice in a row, against the fp32 reference of the same op; rows /
+    """out += a @ b.T + bias (fp32 global reductions from the epilogue): twice in a row, against the fp32 reference of the same op; rows /
     columns outside M x N of a larger buffer stay untouched."""
     g = torch.Generator(device="cpu").manual_seed(M + N + K)
     a = (torch.randn(M, K, generator=g) * 0.5).half().to(cuda_device)

@@ -1,5 +1,5 @@
 """The split-fp16 ("pair") arithmetic the conv engines rely on, emulated on the CPU: fp16 operands, exact products, fp32
-accumulation -- what a tcgen05 kind::f16 MMA computes.  Pins the claims of DESIGN.md §2:
+accumulation -- what a wgmma f16 MMA computes.  Pins the claims of DESIGN.md §2:
   * x = hi + lo with hi = fp16(x), lo = fp16(x - hi) carries ~22 mantissa bits;
   * hi.W_hi + lo.W_hi + hi.W_lo reproduces the fp32 product to ~1e-6 (the dropped lo.W_lo term is ~2^-22);
   * max() over pairs may compare hi + lo in fp32 (exact) and re-split (the pool kernels)."""

@@ -1,4 +1,4 @@
-"""video_features_b200 -- B200-native (sm_100a) engine for the per-frame / per-clip inference hot path of
+"""video_features_b200 -- H100-native (sm_90a) engine for the per-frame / per-clip inference hot path of
 Kamino666/video_features.  Host side mirrors the reference's Extract* classes; the compute lives in
 libvfeat.so (hand-written CUDA behind a C ABI, see include/vfeat.h)."""
 __version__ = "0.1.0"

@@ -39,7 +39,7 @@ class ClipEngine:
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, chunk_frames: int = 0):
         if not torch.cuda.is_available():
-            raise RuntimeError("ClipEngine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("ClipEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         keep = []     # keep numpy arrays alive across the create call
         if "visual.conv1.weight" not in state_dict:

@@ -1,28 +1,21 @@
-// QKV projection fused with the 50-token self-attention of the ViT blocks, for sm_100a.
+// QKV projection fused with the 50-token self-attention of the ViT blocks, for sm_90a.
 //
 //   att[frame, token, head*64 .. +64] = softmax(q k^T / 8) v      with  [q | k | v] = h . W_qkv^T + b   (per head)
 //
 // Replaces, per block, the QKV GEMM + `attention50_kernel` pair (reference: third-party clip `ResidualAttentionBlock
-// .attention` = nn.MultiheadAttention, called from models/CLIP/extract_clip.py:128).  Why fuse: the K = 768 GEMMs are
-// bound by the bytes their epilogues write (profiles/r2_gemm_notes.md: 64 KB of stores per tile stretch the main loop's
-// tile period from 6144 to 9200 cycles).  The QKV GEMM writes 3 x 768 columns only for the attention kernel to read them
-// back and emit 768: here q, k, v never leave the SM -- the epilogue stages them in shared memory, runs the attention of
-// the tile's frames on mma.sync and writes the 768-wide result.
+// .attention` = nn.MultiheadAttention, called from models/CLIP/extract_clip.py:128).  Why fuse: the QKV GEMM would write
+// 3 x 768 columns only for the attention kernel to read them back and emit 768: here q, k, v never leave the SM -- the
+// epilogue stages them in shared memory, runs the attention of the tile's frames on mma.sync and writes the 768-wide
+// result.
 //
 // Tiling: the weight rows are permuted so that the 192 rows [q_h | k_h | v_h] of head h are contiguous; an output tile
-// is (5 frames = 250 token rows) x (one head = 192 columns).  A CTA pair computes it with M = 256 UMMAs: CTA 0 holds tile
-// rows 0..127 (frames 0, 1 and tokens 0..27 of frame 2), CTA 1 rows 128..255 (tokens 28..49 of frame 2, frames 3, 4,
-// 6 rows of the next group that are computed and ignored).  Frame 2 straddles the pair: each CTA pushes its k / v rows of
-// that frame into the peer's staging buffer through distributed shared memory, and each handles the queries it owns.
-//
-// Warp roles per CTA (16 warps).  The epilogue is a two-stage pipeline over two staging buffers, so that the attention of
-// tile i, the staging of tile i+1 and the main loop of tile i+2 run at the same time (in-kernel timeline, profiles/r2:
-// with one set of warps doing both phases in turn a tile cost 13.4 k cycles against 4.6 k of main loop):
-//   0      TMA producer                      1   MMA issuer (leader CTA) + TMEM allocation
-//   4..7   loaders, one per TMEM lane quarter: tcgen05.ld of their 32 rows x 192 columns -> + bias -> fp16 -> staging row
-//          (and the peer's halo for the straddling frame), then release the accumulator stage
-//   2, 3, 8..15   attention warps: one 16-query m-tile of one frame per warp (10 per CTA): S = Q K^T on mma.sync m16n8k16,
-//          softmax in the accumulator fragments (fp32), O = P V, O through the unit's own Q rows, 16-byte global stores.
+// is (2 frames = 100 token rows) x (one head = 192 columns), computed as a 128-row wgmma tile (the 28 rows behind the
+// two frames belong to the next tile: they are computed and ignored).  Three warpgroups per CTA:
+//   warpgroup 0      TMA producer (one lane), a ring of STAGES stages; it runs ahead into the next tile
+//   warpgroups 1, 2  rows 0..63 / 64..127: wgmma m64n192k16 main loop, then accumulator + bias -> fp16 -> staging
+//                    rows; after a named barrier each of the 8 warps runs one attention unit (16 queries of one frame:
+//                    S = Q K^T on mma.sync m16n8k16, softmax in the accumulator fragments (fp32), O = P V) and stores its
+//                    rows with 16-byte global stores.
 // Numerics are those of attention50_kernel (fp16 q / k / v / P, fp32 scores and accumulation).
 #include <string.h>
 
@@ -30,27 +23,21 @@
 
 #include "common.cuh"
 #include "internal.h"
+#include "wgmma.cuh"
 
 namespace vf {
 
 namespace {
 
-constexpr int BM = 128, BK = 64, BN = 192, STAGES = 3;
-constexpr int FRAMES_PER_TILE = 5, TOK = 50, TILE_ROWS = FRAMES_PER_TILE * TOK;   // 250
-constexpr int LOADERS = 4, ATT_WARPS = 10, THREADS = 16 * 32;
-#ifndef VF_ATTN_LOADER_WARP0
-#define VF_ATTN_LOADER_WARP0 4       // loaders = warps 4..7 (2..5 also satisfies warp % 4 == TMEM lane quarter)
-#endif
-constexpr int LOADER_WARP0 = VF_ATTN_LOADER_WARP0;
-constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = (BN / 2) * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int BM = 128, BK = 64, BN = 192, STAGES = 4;
+constexpr int FRAMES_PER_TILE = 2, TOK = 50, TILE_ROWS = FRAMES_PER_TILE * TOK;   // 100
+constexpr int THREADS = 384, CONSUMER_THREADS = 256, CONSUMER_WARPS = 8;
+constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int PITCH = 200;                        // halfs per staging row: 192 + 8 (16-byte shift per row: conflict-free ldmatrix)
-constexpr int ROW0 = 28;                          // staging row of the CTA's local row 0 (rows 0..27: halo of CTA 1)
-constexpr int STG_ROWS = 178;                     // 28 + 128 + 22 halo rows of CTA 0
-constexpr uint32_t STG_BYTES = STG_ROWS * PITCH * 2;          // one staging buffer (there are two)
-constexpr uint32_t ZERO_BYTES = 128, BIAS_BYTES = 2 * BN * 4;     // bias of the tile's head: one copy per tile parity
-constexpr uint32_t BAR_BYTES = (2 * STAGES + 4 + 4) * 8 + 16;
-constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STG_BYTES + ZERO_BYTES + BIAS_BYTES + BAR_BYTES + 1024;
-constexpr uint32_t TMEM_COLS = 512, ACC_STRIDE = 256;
+constexpr uint32_t STG_BYTES = BM * PITCH * 2;
+constexpr uint32_t ZERO_BYTES = 128;
+constexpr uint32_t BAR_BYTES = 2 * STAGES * 8;
+constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + ZERO_BYTES + BAR_BYTES + 1024;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 
 __device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
@@ -67,27 +54,6 @@ __device__ __forceinline__ void ldsm_x4_trans(uint32_t* r, const void* p) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
 }
-// 16-byte store into the shared memory of CTA `cta` of this cluster (distributed shared memory)
-__device__ __forceinline__ void st_cluster_v4(uint32_t local_addr, uint32_t cta, uint4 v) {
-    asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(mapa_u32(local_addr, cta)), "r"(v.x), "r"(v.y),
-                 "r"(v.z), "r"(v.w)
-                 : "memory");
-}
-// wait on a barrier whose arrivals come from the peer CTA (its distributed-shared-memory writes must be visible after)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
 // one attention unit: 16 query rows (staging rows qrow0..qrow0+15) against the 50 keys at staging rows krow0..krow0+49
 // S: [row][q 0..63 | k 64..127 | v 128..191] fp16.  The result replaces the q columns of the unit's first `nvalid` rows (the
 // rows behind them belong to the next frame: they are read, their results discarded, and they are never written).
@@ -177,245 +143,120 @@ __device__ __forceinline__ void attention_unit(__half* S, const __half* zero, in
     __syncwarp();
 }
 
-#ifdef VF_DBG_TRACE
-// SM-clock stamps of the leader CTA's attention warp 8 per tile (scripts/attn_trace.py): [pair][tile iteration][slot]
-//   3 tile staged (stg_full passed)   4 attention unit done   5 output stored / tile done
-// and of its loader warp 4:   0 accumulator ready   1 staging buffer free   2 rows staged, accumulator released
-__device__ long long g_attn_trace[74][64][8];
-#define ATR(slot) do { if (cta == 0 && warp == 9 && lane == 0 && titer < 63) g_attn_trace[pair][titer][slot] = clock64(); } while (0)
-#define LTR(slot) do { if (cta == 0 && warp == LOADER_WARP0 && lane == 0 && titer < 63) g_attn_trace[pair][titer][slot] = clock64(); } while (0)
-#else
-#define ATR(slot) do { } while (0)
-#define LTR(slot) do { } while (0)
-#endif
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 qkv_attention_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const float* __restrict__ bias, __half* __restrict__ att, const int n_frames, const int heads) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;
     uint8_t* sB = smem + STAGES * A_BYTES;
-    uint8_t* stg = smem + STAGES * STAGE_BYTES;                         // two staging buffers, then 128 B of zeros
-    __half* zero = reinterpret_cast<__half*>(stg + 2 * STG_BYTES);
-    float* sbias = reinterpret_cast<float*>(stg + 2 * STG_BYTES + ZERO_BYTES);      // [tile parity][192]
-    uint64_t* full = reinterpret_cast<uint64_t*>(stg + 2 * STG_BYTES + ZERO_BYTES + BIAS_BYTES);
+    __half* S = reinterpret_cast<__half*>(smem + STAGES * STAGE_BYTES);        // staging rows [128][PITCH]
+    __half* zero = reinterpret_cast<__half*>(smem + STAGES * STAGE_BYTES + STG_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + STG_BYTES + ZERO_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;
-    uint64_t* tempty = tfull + 2;
-    uint64_t* stg_full = tempty + 2;      // [2] q/k/v of the tile are staged in buffer b, the peer's halo rows included
-    uint64_t* stg_free = stg_full + 2;    // [2] nobody reads buffer b any more: neither this CTA nor (its halo) the peer
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stg_free + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t cta = cluster_ctarank();
-    const uint32_t peer = cta ^ 1u;
-    const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
     const int num_m = (n_frames + FRAMES_PER_TILE - 1) / FRAMES_PER_TILE;
     const int num_tiles = num_m * heads;
     const int width = heads * 64;
     constexpr int num_k = 768 / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull[i], 1);
-            mbar_init(&tempty[i], 2 * LOADERS);          // the loader warps of both CTAs arrive on the LEADER's copy
-            mbar_init(&stg_full[i], LOADERS + 32);       // 4 local loader warps + every lane of the peer's halo-writing loader
-            mbar_init(&stg_free[i], 2 * ATT_WARPS);      // the attention warps of both CTAs
+            mbar_init(&empty[i], CONSUMER_WARPS);
         }
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc_2sm(tmem_slot, TMEM_COLS);
-    // staging rows a tile never writes are read (masked) by neighbouring units: no uninitialised bit patterns anywhere
-    for (uint32_t i = threadIdx.x; i < (2 * STG_BYTES + ZERO_BYTES) / 16; i += THREADS)
-        reinterpret_cast<uint4*>(stg)[i] = make_uint4(0, 0, 0, 0);
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (threadIdx.x < ZERO_BYTES / 16) reinterpret_cast<uint4*>(zero)[threadIdx.x] = make_uint4(0, 0, 0, 0);
+    __syncthreads();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-                const int m_blk = tile % num_m, head = tile / num_m;
-                const int m0 = m_blk * TILE_ROWS + int(cta) * BM;          // rows past the matrix are zero-filled by TMA
-                const int n0 = head * BN + int(cta) * (BN / 2);
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int m0 = (tile % num_m) * TILE_ROWS;      // rows past the matrix are zero-filled by TMA
+                const int n0 = (tile / num_m) * BN;
                 for (int kk = 0; kk < num_k; ++kk) {
                     mbar_wait(&empty[stage], phase ^ 1);
-                    if (cta == 0) mbar_expect_tx(&full[stage], 2 * STAGE_BYTES);
-                    const uint32_t bar = mapa_u32(smem_u32(&full[stage]), 0);
-                    tma_load_2d_2sm(sA + stage * A_BYTES, &tmA, bar, kk * BK, m0);
-                    tma_load_2d_2sm(sB + stage * B_BYTES, &tmB, bar, kk * BK, n0);
+                    mbar_expect_tx(&full[stage], STAGE_BYTES);
+                    tma_load_2d(sA + stage * A_BYTES, &tmA, &full[stage], kk * BK, m0);
+                    tma_load_2d(sB + stage * B_BYTES, &tmB, &full[stage], kk * BK, n0);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (cta == 0 && lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(2 * BM, BN, 0);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-                mbar_wait(&tempty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * ACC_STRIDE;
-                for (int kb = 0; kb < num_k; ++kb) {
-                    mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-                    const uint64_t adesc = umma_desc_sw128(sA + stage * A_BYTES);
-                    const uint64_t bdesc = umma_desc_sw128(sB + stage * B_BYTES);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k)
-                        umma_f16_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                    umma_commit_2sm(&empty[stage], 3);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                umma_commit_2sm(&tfull[acc], 3);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= LOADER_WARP0 && warp < LOADER_WARP0 + 4) {
-        // ------------------------------------------------------------ loaders: accumulator -> (+ bias) -> fp16 -> staging
-        const int q = warp & 3;                // TMEM lane quarter (== warp id % 4)
-        const int lrow = q * 32 + lane;        // row inside this CTA's 128-row block == TMEM lane
-        // the straddling frame (index 2 of the tile): CTA 0 owns its tokens 0..27 (local rows 100..127), CTA 1 its tokens
-        // 28..49 (local rows 0..21).  k / v of those rows are ALSO written into the peer's staging buffer:
-        //   CTA 0 -> peer rows 0..27   (the peer's frame-2 keys start at staging row 0)
-        //   CTA 1 -> peer rows 156..177 (CTA 0's frame-2 keys start at staging row 128 = ROW0 + 100)
-        const bool halo_row = cta == 0 ? (lrow >= 100) : (lrow < 22);
-        const int halo_dst = cta == 0 ? (lrow - 100) : (ROW0 + 128 + lrow);
-        const bool halo_writer = cta == 0 ? q == 3 : q == 0;       // the one loader of this CTA that owns such rows
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int tile = pair, titer = 0; tile < num_tiles; tile += num_pairs, ++titer) {
-            const int head = tile / num_m;
-            const int b = titer & 1;
-            const uint32_t bpar = uint32_t(titer >> 1) & 1u;
-            __half* S = reinterpret_cast<__half*>(stg + b * STG_BYTES);
-            // this tile's 192 bias values into shared memory (then read as broadcasts).  Every loader writes the same values
-            // into the copy of this tile's parity and reads after its own __syncwarp; loaders are never more than one tile
-            // apart (a buffer is re-staged only after all four staged it two tiles ago), so two copies suffice.  The global
-            // loads are in flight while the warp waits for the accumulator.
-            float* mybias = sbias + b * BN;
-#pragma unroll
-            for (int j = 0; j < BN / 32; ++j) mybias[lane + 32 * j] = __ldg(bias + head * BN + lane + 32 * j);
-            __syncwarp();
-            mbar_wait(&tfull[acc], acc_phase);
-            LTR(0);
-            tc_fence_after();
-            // buffer b: the attention warps of BOTH CTAs are done with what was staged there two tiles ago
-            mbar_wait_cluster(&stg_free[b], bpar ^ 1);
-            LTR(1);
-            const uint32_t t_row = tmem_base + acc * ACC_STRIDE + (uint32_t(q * 32) << 16);
-            __half* srow = S + (ROW0 + lrow) * PITCH;
-            // q: columns 0..63, k: 64..127, v: 128..191.  Three 32-column TMEM loads are in flight per wait: under a busy
-            // tensor pipe a single tcgen05.ld takes ~1000 cycles to come back (timeline, profiles/r2), and the four loader
-            // warps are the stage that bounds the tile period.
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 96) {
-                uint32_t raw[3][32];
-#pragma unroll
-                for (int u = 0; u < 3; ++u) tmem_ld_32x32(t_row + c0 + 32 * u, raw[u]);
-                tmem_ld_wait();
-#pragma unroll
-                for (int u = 0; u < 3; ++u) {
-                    const int c = c0 + 32 * u;
-                    uint4 pk[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float4 b0 = *reinterpret_cast<const float4*>(mybias + c + 8 * j);
-                        const float4 b1 = *reinterpret_cast<const float4*>(mybias + c + 8 * j + 4);
-                        pk[j] = make_uint4(pack_half2(__uint_as_float(raw[u][8 * j]) + b0.x, __uint_as_float(raw[u][8 * j + 1]) + b0.y),
-                                           pack_half2(__uint_as_float(raw[u][8 * j + 2]) + b0.z, __uint_as_float(raw[u][8 * j + 3]) + b0.w),
-                                           pack_half2(__uint_as_float(raw[u][8 * j + 4]) + b1.x, __uint_as_float(raw[u][8 * j + 5]) + b1.y),
-                                           pack_half2(__uint_as_float(raw[u][8 * j + 6]) + b1.z, __uint_as_float(raw[u][8 * j + 7]) + b1.w));
-                        *reinterpret_cast<uint4*>(srow + c + 8 * j) = pk[j];
-                    }
-                    if (halo_writer && halo_row && c >= 64) {
-                        const uint32_t dst = smem_u32(S + halo_dst * PITCH + c);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) st_cluster_v4(dst + 16 * j, peer, pk[j]);
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive_remote(&tempty[acc], 0);      // this accumulator stage is drained
-                mbar_arrive(&stg_full[b]);                // this warp's 32 rows are staged (release: the warp's writes)
-            }
-            if (halo_writer) mbar_arrive_remote(&stg_full[b], peer);   // every lane releases its own remote rows
-            LTR(2);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    } else if (warp >= 2) {
-        // ------------------------------------------------------------ attention: one 16-query m-tile of one frame per warp
-        const int e = warp < LOADER_WARP0 ? warp - 2 : warp - 6;      // unit 0..9 (the 10 warps that are not loaders)
-        // CTA 0: frames 0, 1 + tokens 0..27 of frame 2;  CTA 1: tokens 28..49 of frame 2 + frames 3, 4
-        int f, tok0, krow0;       // frame in tile, first query token, staging row of the frame's token 0
-        if (cta == 0) {
-            if (e < 8) { f = e >> 2; tok0 = (e & 3) * 16; krow0 = ROW0 + 50 * f; }
-            else       { f = 2; tok0 = (e - 8) * 16; krow0 = ROW0 + 100; }
-        } else {
-            if (e < 2) { f = 2; tok0 = 28 + e * 16; krow0 = 0; }
-            else       { f = 3 + ((e - 2) >> 2); tok0 = ((e - 2) & 3) * 16; krow0 = 50 * (f - 2); }
-        }
-        const int qrow0 = krow0 + tok0;
-        const int tok_end = (cta == 0 && f == 2) ? 28 : TOK;       // queries this CTA owns in that frame
-        for (int tile = pair, titer = 0; tile < num_tiles; tile += num_pairs, ++titer) {
-            const int m_blk = tile % num_m, head = tile / num_m;
-            const int b = titer & 1;
-            const uint32_t bpar = uint32_t(titer >> 1) & 1u;
-            __half* S = reinterpret_cast<__half*>(stg + b * STG_BYTES);
-            mbar_wait_cluster(&stg_full[b], bpar);                  // own rows staged + the peer's rows of the straddling frame
-            ATR(3);
-            attention_unit(S, zero, qrow0, krow0, tok_end - tok0, lane);
-            ATR(4);
-            const int frame = m_blk * FRAMES_PER_TILE + f;
-            if (frame < n_frames) {
-                __half* orow = att + (int64_t(frame) * TOK) * width + head * 64;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = i * 4 + (lane >> 3), seg = lane & 7;
-                    const int tok = tok0 + r;
-                    if (tok < tok_end)
-                        *reinterpret_cast<uint4*>(orow + int64_t(tok) * width + seg * 8) =
-                            *reinterpret_cast<const uint4*>(S + (qrow0 + r) * PITCH + seg * 8);
-                }
-            }
-            __syncwarp();
-            ATR(5);
-            if (lane == 0) {                      // buffer b is free as far as this warp is concerned: tell both loaders' CTAs
-                mbar_arrive(&stg_free[b]);
-                mbar_arrive_remote(&stg_free[b], peer);
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm(tmem_base, TMEM_COLS);
+    const int wg = (warp >> 2) - 1, wq = warp & 3;
+    const int e = warp - 4;                              // attention unit 0..7: frame e / 4, queries 16 (e % 4) ..
+    const int f = e >> 2, tok0 = (e & 3) * 16;
+    const int krow0 = TOK * f, qrow0 = krow0 + tok0;
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile % num_m, head = tile / num_m;
+        int prev = -1;
+        for (int kb = 0; kb < num_k; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint64_t adesc = wgmma_desc_sw128(sA + stage * A_BYTES + wg * (64 * 128));
+            const uint64_t bdesc = wgmma_desc_sw128(sB + stage * B_BYTES);
+            wgmma_fence_regs<BN / 2>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) Wgmma<BN>::mma(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();
+            wgmma_fence_regs<BN / 2>(acc);
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs<BN / 2>(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+
+        // every unit is done with the previous tile's staging rows before they are overwritten
+        named_bar_sync(1, CONSUMER_THREADS);
+        // accumulator register 4j + 2h + c: row (lane / 4) + 8h of this warp's 16, column 8j + 2 (lane % 4) + c
+        const float* hb = bias + head * BN;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const float2 b = __ldg(reinterpret_cast<const float2*>(hb + c));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+                *reinterpret_cast<uint32_t*>(S + r * PITCH + c) = pack_half2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
+            }
+        }
+        named_bar_sync(1, CONSUMER_THREADS);
+        attention_unit(S, zero, qrow0, krow0, tok0 + 16 <= TOK ? 16 : TOK - tok0, lane);
+        const int frame = m_blk * FRAMES_PER_TILE + f;
+        if (frame < n_frames) {
+            __half* orow = att + (int64_t(frame) * TOK) * width + head * 64;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int r = i * 4 + (lane >> 3), seg = lane & 7;
+                const int tok = tok0 + r;
+                if (tok < TOK)
+                    *reinterpret_cast<uint4*>(orow + int64_t(tok) * width + seg * 8) =
+                        *reinterpret_cast<const uint4*>(S + (qrow0 + r) * PITCH + seg * 8);
+            }
+        }
     }
 }
 
 }  // namespace
-
-#ifdef VF_DBG_TRACE
-extern "C" int vf_dbg_attn_trace(long long* host_out) {
-    cudaDeviceSynchronize();
-    return int(cudaMemcpyFromSymbol(host_out, g_attn_trace, sizeof(g_attn_trace)));
-}
-#endif
 
 // h: [n_frames*50, 768] fp16 (row pitch lda); w_perm: [heads*192, 768] fp16, row h*192 + part*64 + d = in_proj row
 // part*768 + h*64 + d; bias_perm likewise (fp32); att: [n_frames*50, heads*64] fp16
@@ -433,10 +274,10 @@ int qkv_attention(const __half* h, int lda, const __half* w_perm, const float* b
     const int M = n_frames * TOK;
     CUtensorMap tmA, tmB;
     VF_TRY(make_tmap_2d(&tmA, h, 2, uint64_t(M), 768, uint64_t(lda) * 2, BM, BK));
-    VF_TRY(make_tmap_2d(&tmB, w_perm, 2, uint64_t(heads) * BN, 768, 768 * 2, BN / 2, BK));
+    VF_TRY(make_tmap_2d(&tmB, w_perm, 2, uint64_t(heads) * BN, 768, 768 * 2, BN, BK));
     const int tiles = ((n_frames + FRAMES_PER_TILE - 1) / FRAMES_PER_TILE) * heads;
-    const int pairs = device_sm_count() / 2;
-    const int grid = 2 * (tiles < pairs ? tiles : pairs);
+    const int sms = device_sm_count();
+    const int grid = tiles < sms ? tiles : sms;
     qkv_attention_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(tmA, tmB, bias_perm, att, n_frames, heads);
     VF_CUDA(cudaGetLastError());
     return VF_OK;

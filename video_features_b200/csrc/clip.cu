@@ -1,11 +1,11 @@
 // CLIP ViT-B image tower (patch 32: the north-star model; patch 16: the reference's 'CLIP-ViT-B/16' feature type, same
-// width / depth, 197 tokens) on the tcgen05 GEMM + memory-bound kernels.
+// width / depth, 197 tokens) on the wgmma GEMM + memory-bound kernels.
 // Replaces `clip.load("ViT-B/32")` + `model.encode_image(frames)` (reference: models/CLIP/extract_clip.py:47,128;
 // algorithm: third-party openai/CLIP clip/model.py VisionTransformer.forward, restated in oracle/clip_tower.py).
 //
-// Numerics: GEMM operands fp16, accumulation fp32 (TMEM), residual stream / LayerNorm / softmax fp32.
-// Frames are packed along M (row = frame*tokens + token), processed in chunks sized so that one chunk's
-// activations stay L2-resident between kernels.
+// Numerics: GEMM operands fp16, accumulation fp32 (wgmma registers), residual stream / LayerNorm / softmax fp32.
+// Frames are packed along M (row = frame*tokens + token) and processed in chunks (default 256 frames, chosen by
+// measurement: vf_clip_create_vit).
 #include <stdlib.h>
 #include <string.h>
 
@@ -80,7 +80,7 @@ struct vf_clip {
     cudaStream_t cs = nullptr;                // stream of the active lane
     cudaEvent_t ev_in = nullptr;
     bool use_graph = true;
-    bool acc_o = true, acc_m = true;          // residual adds in the GEMM epilogue (TMA reduction) instead of an fp16 y
+    bool acc_o = true, acc_m = true;          // residual adds in the GEMM epilogue (fp32 reductions) instead of an fp16 y
     bool fused_attn = true;                   // QKV projection + attention in one kernel (VF_CLIP_ATTN=split: GEMM + kernel)
     float* feat = nullptr;                    // [chunk, 512] tower output of the active lane
     cudaStream_t copy_stream = nullptr;
@@ -190,8 +190,8 @@ static int tower_attention(vf_clip* h, int c, cudaStream_t s) {
 }
 
 // The tower on one chunk whose patch matrix is already in h->patches; writes c x 512 fp32 to out.
-// GEMM epilogues never read global memory: bias / QuickGELU in registers, then TMA stores -- or, for the two GEMMs that
-// end a residual branch, a TMA reduction that adds the tile into the fp32 residual stream x.
+// GEMM epilogues never read global memory: bias / QuickGELU in registers, then global stores -- or, for the two GEMMs
+// that end a residual branch, fp32 reductions that add the tile into the fp32 residual stream x.
 static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
     const int T = h->T, P = h->P, PK = h->PK;
     const int M = c * T;
@@ -201,7 +201,7 @@ static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
     VF_TRY(tower_embed_ln(h, c, s));
     h->launches += 2;
     // The residual stream x stays fp32 in HBM.  A GEMM that ends a residual branch either ADDS its result into x from the
-    // epilogue (TMA reduction in the L2; the LayerNorm pass that follows then only reads x and writes h: 6 bytes per
+    // epilogue (fp32 global reductions; the LayerNorm pass that follows then only reads x and writes h: 6 bytes per
     // element), or writes an fp16 increment y that the LayerNorm kernel adds ("x += y; h = LN(x)": 12 bytes per element).
     // acc_o / acc_m select the form for the attention out-projection / the MLP's second GEMM (VF_CLIP_RESID=acc|y|mix).
     const bool acc_o = h->acc_o, acc_m = h->acc_m;
@@ -363,16 +363,18 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
     *out = nullptr;
     if (patch_size != 32 && patch_size != 16)
         return fail(VF_ERR_UNSUPPORTED, "clip_create: patch size %d (ViT-B/32 and ViT-B/16 are built)", patch_size);
-    // default chunk: ~12.5 k token rows per GEMM launch (49 M-tiles of 256 rows: one wave of 74 CTA pairs is too few,
-    // the activations of one chunk still sit in the L2)
+    // default chunk: 256 frames (a 1000-frame call runs as 4 balanced chunks of 250 = 12.5 k token rows, 98 M-tiles of
+    // 128 rows: 9 waves of the fc1 GEMM over 132 SMs, 1500 fused QKV + attention tiles).  Measured on one H100 at a 400 W
+    // power limit (bench.py --chunk, 20 steps): 128 / 250 / 500 / 1000 frames per chunk give 21.5 / 23.0 / 22.3 / 21.9 k
+    // frames/s -- larger chunks gain no GEMM efficiency and lose overlap of the copies with the tower.
     if (chunk_frames <= 0) chunk_frames = patch_size == 32 ? 256 : 126;
     if (chunk_frames > 4096) return fail(VF_ERR_INVALID, "clip_create: chunk_frames %d too large", chunk_frames);
     VF_CUDA(cudaSetDevice(device));
     int major = 0, minor = 0;
     VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
     VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 10)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only", device, major, minor);
+    if (major != 9 || minor != 0)
+        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
     vf_clip* h = new vf_clip();
     h->device = device;
     h->chunk = chunk_frames;
@@ -427,8 +429,8 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
         }
         const size_t C = size_t(chunk_frames);
         {
-            // measured: two lanes give no gain on B200 (87.1 k vs 88.4 k frames/s; the persistent GEMM leaves no room
-            // for co-resident blocks), so one lane is the default and the second is opt-in for experiments
+            // the persistent GEMM leaves no room for co-resident blocks, so one lane is the default and the second is
+            // opt-in for experiments
             const char* e = getenv("VF_CLIP_LANES");
             h->n_lanes = (e && e[0] == '2') ? 2 : 1;
         }

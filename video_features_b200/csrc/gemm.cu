@@ -1,25 +1,20 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a, CTA pairs (cta_group::2).
+// Persistent warp-specialised wgmma GEMM for sm_90a.
 //
-//   D[M,N] = act( A[M,K] . B[N,K]^T * scale[n] + bias[n] )     A, B fp16 K-major; fp32 accumulate in TMEM;
+//   D[M,N] = act( A[M,K] . B[N,K]^T * scale[n] + bias[n] )     A, B fp16 K-major; fp32 accumulate in registers;
 //                                                              D fp16 or fp32
 //
-// A cluster of two CTAs (one TPC) owns a 256 x BN output tile.  Each CTA stages its own 128 rows of A and HALF of
-// the B tile (BN/2 rows) through a 128B-swizzled TMA ring; the leader CTA issues one UMMA of M=256 per 16-wide K
-// step that reads both halves, and each CTA's TMEM receives the 128 x BN block of its rows (two accumulator stages,
-// so the epilogue of tile i overlaps the main loop of tile i+1).  4 + 4*NGRP warps per CTA:
-//   warp 0      TMA producer (one lane, both CTAs)          warp 1   MMA issuer (one lane, leader CTA only)
-//   warp 2      TMEM allocator                              warp 3   idle
-//   warps 4..   epilogue, NGRP groups of 4 warps (one warp per TMEM lane quarter = 32 rows of this CTA's 128); groups
-//               take column slices of 128 bytes in turn.  Per slice a warp does tcgen05.ld (thread = row) -> scale / bias /
-//               activation -> its [32 rows x 128 B] of a 128B-swizzled staging slice -> fence.proxy.async + __syncwarp ->
-//               its elected lane issues a TMA store (or TMA reduce-add) of that box.  No barrier between warps; M/N tails
-//               are clipped by the TMA unit; no per-thread global stores.
-// How it got here (profiles/r1_gemm_notes.md, profiles/r2_gemm_notes.md): per-thread stores from registers are bound by
-// the LSU (32 sectors per warp instruction); one elected thread per 128-row slice serialises four warps on a named
-// barrier; with 8 epilogue warps the fc1 + QuickGELU epilogue (2 MUFU ops per element) was the critical path.
+// A CTA owns a 128 x BN output tile at a time (tiles are strided over a grid of at most one CTA per SM).  Three
+// warpgroups:
+//   warpgroup 0    TMA producer (one lane): A and B tiles through a 128B-swizzled ring of STAGES stages, one mbarrier
+//                  pair (full / empty) per stage.  It runs ahead into the next tile while the consumers store this one.
+//   warpgroups 1,2 consumers: rows 0..63 and 64..127 of the tile.  Per 64-wide K block, four wgmma m64nBNk16 (eight with
+//                  split weights), one commit group; the stage is released as soon as the group behind it has retired.
+//                  Epilogue straight from the accumulator registers: scale / bias / activation, row mask, then fp16x2 or
+//                  fp32x2 global stores (fp32x2 reductions for `accumulate`), M / N tails clipped per element.
 //
 // Used for every dense contraction of the hot path: ViT patch-embed / QKV / out-proj / FFN GEMMs (reference:
-// third-party clip `VisionTransformer.forward`, called at models/CLIP/extract_clip.py:128).
+// third-party clip `VisionTransformer.forward`, called at models/CLIP/extract_clip.py:128) and the I3D / RAFT
+// convolutions in the shifted-row mode below.
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
@@ -29,66 +24,32 @@
 
 #include "common.cuh"
 #include "internal.h"
+#include "wgmma.cuh"
 
-// epilogue warp groups (4 warps = the 4 TMEM lane quarters each) of the plain 256-wide configuration -- the ViT GEMMs.
-// Measured (profiles/r2_gemm_notes.md): 2 -> 4 groups takes the fc1 + QuickGELU epilogue off the critical path.
-#ifndef VF_EPI_GROUPS
-#define VF_EPI_GROUPS 4
-#endif
-#ifndef VF_STAGES_256
-#define VF_STAGES_256 5       // TMA ring depth of the plain 256-wide configuration
-#endif
-// measurement aid (scripts/build_variants.sh, scripts/gemm_trace.py): which parts of the epilogue run.
-//   0 all (product)   1 no TMA store   2 TMEM load + math only   3 TMEM load only   4 everything but the TMEM load
-//   9 nothing: accumulators are released unread (main loop only)
-#ifndef VF_DBG_EPI
-#define VF_DBG_EPI 0
-#endif
 namespace vf {
 
 namespace {
 
-#ifdef VF_DBG_TRACE
-// per-tile SM-clock timestamps of the leader CTA of every pair (scripts/gemm_trace.py): [pair][tile iteration][slot]
-//   0 MMA: accumulator stage granted      1 MMA: last MMA of the tile issued      2 epilogue warp 4: accumulator ready
-//   3 epilogue warp 4: its slices done    4 producer: first load of the tile issued   5 producer: last load issued
-__device__ long long g_trace[74][64][8];
-#define VF_TRACE(slot, iter) do { if ((iter) < 63) g_trace[pair][iter][slot] = clock64(); } while (0)
-#else
-#define VF_TRACE(slot, iter) do { } while (0)
-#endif
-constexpr int BM = 128;          // rows per CTA (256 per pair)
-constexpr int STORE_ROWS = 32;   // rows of one TMA store box: every epilogue warp stores its own 32 rows
+constexpr int BM = 128;          // rows per CTA tile (64 per consumer warpgroup)
 constexpr int BK = 64;           // 64 fp16 = one 128-byte swizzle row
-// epilogue warp groups (4 warps = the 4 TMEM lane quarters each) of the plain 256-wide configuration -- the ViT GEMMs, whose
-// K = 768 shapes are bounded by the epilogue's latency chain (TMEM load -> math -> shared -> store), not by its bandwidth
-#ifndef VF_EPI_GROUPS
-#define VF_EPI_GROUPS 4
-#endif
-#ifndef VF_STAGES_256
-#define VF_STAGES_256 5       // TMA ring depth of the plain 256-wide configuration
-#endif
-constexpr uint32_t SLICE_BYTES = 128 * 128;   // 128 rows x 128 B (32 fp32 or 64 fp16 columns)
+constexpr int THREADS = 384;     // producer warpgroup + two consumer warpgroups
+constexpr int CONSUMER_WARPS = 8;
+constexpr uint32_t SMEM_BUDGET = 200 * 1024;   // operand ring; the rest of the 227 KB stays free
 
-// NSPLIT = 2: the B stage holds the hi and the lo half-tile of a split-fp16 weight matrix and every K step issues two
-// MMAs against the same A tile; the epilogue then keeps ONE slice buffer per group to make room for the wider stages.
-template <int BN, int STAGES, int NSPLIT = 1>
+// NSPLIT = 2: the B stage holds the hi and the lo tile of a split-fp16 weight matrix and every K step issues two
+// MMAs against the same A tile.
+template <int BN, int NSPLIT>
 struct GemmCfg {
-    static constexpr uint32_t A_BYTES = BM * BK * 2;          // 128 rows of A per CTA
-    static constexpr uint32_t B_HALF = (BN / 2) * BK * 2;     // half of the B tile per CTA (one of hi / lo)
-    static constexpr uint32_t B_BYTES = NSPLIT * B_HALF;
+    static constexpr uint32_t A_BYTES = BM * BK * 2;
+    static constexpr uint32_t B_TILE = BN * BK * 2;           // one of hi / lo
+    static constexpr uint32_t B_BYTES = NSPLIT * B_TILE;
     static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr uint32_t TMEM_COLS = BN == 192 ? 512 : 2 * BN;   // two accumulator stages BN columns apart (power of 2)
-    static constexpr int NGRP = (NSPLIT == 1 && BN == 256) ? VF_EPI_GROUPS : 2;   // epilogue groups of 4 warps
-    static constexpr int EPI_WARPS = 4 * NGRP;
-    static constexpr int THREADS = (4 + EPI_WARPS) * 32;
-    static constexpr uint32_t EPI_BUFS = (NSPLIT == 2 || NGRP > 2) ? 1 : 2;
-    static constexpr uint32_t STG_BYTES = NGRP * EPI_BUFS * SLICE_BYTES;   // NGRP groups x EPI_BUFS slice buffers
-    static constexpr uint32_t BAR_BYTES = (2 * STAGES + 4) * 8 + 16;
-    static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + STG_BYTES + BAR_BYTES + 1024;   // + align slack
-    static_assert(TMEM_COLS == 128 || TMEM_COLS == 256 || TMEM_COLS == 512, "TMEM columns");
+    static constexpr int STAGES = int(SMEM_BUDGET / STAGE_BYTES) > 8 ? 8 : int(SMEM_BUDGET / STAGE_BYTES);
+    static constexpr uint32_t BAR_BYTES = 2 * STAGES * 8;
+    static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;   // + align slack
+    static_assert(STAGES >= 2, "at least two pipeline stages");
     static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-    static_assert(A_BYTES % 1024 == 0 && B_BYTES % 1024 == 0, "swizzle-128B tiles must stay 1024-byte aligned");
+    static_assert(A_BYTES % 1024 == 0 && B_TILE % 1024 == 0, "swizzle-128B tiles must stay 1024-byte aligned");
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -104,297 +65,150 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     return v;
 }
 
-// scale/bias/activation on 32 consecutive columns starting at global column n (same for every lane of the warp)
-__device__ __forceinline__ void epi_math32(float* v, const GemmEpi& ep, int n, int N) {
-    if (ep.scale) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-            if (n + j < N) {
-                const float4 s = __ldg(reinterpret_cast<const float4*>(ep.scale + n + j));
-                v[j] *= s.x; v[j + 1] *= s.y; v[j + 2] *= s.z; v[j + 3] *= s.w;
-            }
-        }
-    }
-    if (ep.bias) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-            if (n + j < N) {
-                const float4 b = __ldg(reinterpret_cast<const float4*>(ep.bias + n + j));
-                v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
-            }
-        }
-    }
-    if (ep.act != VF_ACT_NONE) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = apply_act(v[j], ep.act);
-    }
-}
-
-// 32 consecutive fp32 accumulator columns of this thread's row: TMEM -> registers -> scale / bias / activation (zeroed
-// for rows outside the valid conv region)
-__device__ __forceinline__ void epi_load32(float* v, uint32_t taddr, const GemmEpi& ep, int n, int N, bool keep) {
-#if VF_DBG_EPI == 4
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = float(n + j);        // measurement aid: the accumulator is never read
-    (void)taddr;
-#else
-    uint32_t raw[32];
-    tmem_ld_32x32(taddr, raw);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(raw[j]);
-#endif
-#if VF_DBG_EPI != 3
-    epi_math32(v, ep, n, N);
-#endif
-    if (!keep) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-    }
-}
-__device__ __forceinline__ void epi_sink(const float* v) {      // measurement aid: keep the values alive without storing them
-#pragma unroll
-    for (int j = 0; j < 32; ++j) asm volatile("" ::"f"(v[j]));
-}
-
-// SPLIT: split-fp16 output (GemmEpi::split_off) -- every fp16 slice is emitted twice, hi then lo, through tmO / tmO2.  A
-// compile-time switch: as a run-time loop it cost the plain epilogue 20 % on K = 768 shapes.
-template <int BN, int STAGES, int NSPLIT, bool SPLIT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GemmCfg<BN, STAGES, NSPLIT>::THREADS, 1)
-gemm_f16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                     const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmO2, const GemmEpi ep,
-                     const int M, const int N, const __grid_constant__ ConvGeom cg) {
-    using Cfg = GemmCfg<BN, STAGES, NSPLIT>;
+// SPLIT: split-fp16 output (GemmEpi::split_off) -- every fp16 pair is written twice, hi at column n and lo at
+// split_off + n.  A compile-time switch keeps the plain epilogue free of it.
+template <int BN, int NSPLIT, bool SPLIT>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmEpi ep,
+                const int M, const int N, const __grid_constant__ ConvGeom cg) {
+    using Cfg = GemmCfg<BN, NSPLIT>;
+    constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;
     uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
-    uint8_t* stg = smem + STAGES * Cfg::STAGE_BYTES;                 // 1024-byte aligned (stage sizes are)
-    uint64_t* full = reinterpret_cast<uint64_t*>(stg + Cfg::STG_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t cta = cluster_ctarank();        // 0 = leader (issues the MMAs), 1 = peer
-    const int pair = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-    const int num_m = (M + 2 * BM - 1) / (2 * BM);
+    const int num_m = (M + BM - 1) / BM;
     const int num_n = (N + BN - 1) / BN;
     const int num_tiles = num_m * num_n;
     const int kpt = (cg.k_per_tap + BK - 1) / BK;    // K blocks per filter tap (a plain GEMM is one "tap")
     const int num_k = cg.ntaps * kpt;
 
-#ifdef VF_DBG_TRACE
-    if (cta == 0 && threadIdx.x == 0) {
-        g_trace[pair][63][6] = clock64();
-        long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        g_trace[pair][63][4] = gt;
-    }
-#endif
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-        tma_prefetch_desc(&tmO);
-        tma_prefetch_desc(&tmO2);
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full[i], 1);      // the leader's arrive.expect_tx; the bytes of BOTH CTAs are credited here
-            mbar_init(&empty[i], 1);     // multicast tcgen05.commit from the leader
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull[i], 1);               // multicast tcgen05.commit
-            mbar_init(&tempty[i], 2 * Cfg::EPI_WARPS);  // every epilogue warp of both CTAs arrives on the LEADER's copy
+            mbar_init(&full[i], 1);                  // the producer's arrive.expect_tx
+            mbar_init(&empty[i], CONSUMER_WARPS);    // one arrive per consumer warp
         }
         fence_mbar_init();
     }
-    if (warp == 2) tmem_alloc_2sm(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    cluster_sync_all();      // barriers of both CTAs initialised before any remote arrive / TMA credit
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
-    if (warp == 0) {
-        // ------------------------------------------------------------ TMA producer (both CTAs)
-        if (lane == 0) {
+    if (warp < 4) {
+        // ------------------------------------------------------------ TMA producer
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = pair, titer = 0; tile < num_tiles; tile += num_pairs, ++titer) {
-                const int m_blk = tile % num_m, n_blk = tile / num_m;
-                const int m0 = m_blk * 2 * BM + int(cta) * BM;
-                const int n0 = n_blk * BN + int(cta) * (BN / 2);
-                bool first_load = true;
-                (void)first_load; (void)titer;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
                 for (int tap = 0; tap < cg.ntaps; ++tap) {
                     const int arow = m0 + cg.tap_off[tap];       // may be negative / past the end: TMA zero-fills
                     const int bcol = tap * cg.k_per_tap;
                     for (int kk = 0; kk < kpt; ++kk) {
                         mbar_wait(&empty[stage], phase ^ 1);
-                        if (cta == 0 && first_load) { VF_TRACE(4, titer); first_load = false; }
                         const bool lo_blk = NSPLIT == 2 && ((cg.lo_mask >> kk) & 1ull);    // W_lo not needed
-                        if (cta == 0)
-                            mbar_expect_tx(&full[stage], 2 * (Cfg::A_BYTES + (lo_blk ? Cfg::B_HALF : Cfg::B_BYTES)));
-                        const uint32_t bar = mapa_u32(smem_u32(&full[stage]), 0);
-                        tma_load_2d_2sm(sA + stage * Cfg::A_BYTES, &tmA, bar, kk * BK, arow);
-                        tma_load_2d_2sm(sB + stage * Cfg::B_BYTES, &tmB, bar, bcol + kk * BK, n0);
+                        mbar_expect_tx(&full[stage], Cfg::A_BYTES + (lo_blk ? Cfg::B_TILE : Cfg::B_BYTES));
+                        tma_load_2d(sA + stage * Cfg::A_BYTES, &tmA, &full[stage], kk * BK, arow);
+                        tma_load_2d(sB + stage * Cfg::B_BYTES, &tmB, &full[stage], bcol + kk * BK, n0);
                         if (NSPLIT == 2 && !lo_blk)   // the lo half of the weights lives ntaps*k_per_tap columns to the right
-                            tma_load_2d_2sm(sB + stage * Cfg::B_BYTES + Cfg::B_HALF, &tmB, bar,
-                                            cg.ntaps * cg.k_per_tap + bcol + kk * BK, n0);
+                            tma_load_2d(sB + stage * Cfg::B_BYTES + Cfg::B_TILE, &tmB, &full[stage],
+                                        cg.ntaps * cg.k_per_tap + bcol + kk * BK, n0);
                         if (++stage == STAGES) { stage = 0; phase ^= 1; }
                     }
                 }
-                if (cta == 0) VF_TRACE(5, titer);
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer (leader CTA, one lane)
-        if (cta == 0 && lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(2 * BM, BN, 0);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            for (int tile = pair, titer = 0; tile < num_tiles; tile += num_pairs, ++titer) {
-                (void)titer;
-                mbar_wait(&tempty[acc], acc_phase ^ 1);
-                VF_TRACE(0, titer);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                for (int kb = 0, kk = 0; kb < num_k; ++kb) {
-                    mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-                    const uint64_t adesc = umma_desc_sw128(sA + stage * Cfg::A_BYTES);
-                    const uint64_t bdesc = umma_desc_sw128(sB + stage * Cfg::B_BYTES);
-                    const bool lo_blk = NSPLIT == 2 && ((cg.lo_mask >> kk) & 1ull);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {   // +32 B (encoded 2) per K step inside the swizzle row
-                        umma_f16_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                        if (NSPLIT == 2 && !lo_blk)
-                            umma_f16_2sm(d_tmem, adesc + 2 * k, bdesc + (Cfg::B_HALF >> 4) + 2 * k, idesc, 1u);
-                    }
-                    umma_commit_2sm(&empty[stage], 3);    // free this smem slot in both CTAs
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                    if (++kk == kpt) kk = 0;              // K block index inside the current tap
-                }
-                umma_commit_2sm(&tfull[acc], 3);           // accumulators of both CTAs complete
-                VF_TRACE(1, titer);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ------------------------------------------------------------ epilogue: 2 groups x 4 warps per CTA
-        const int e = warp - 4;
-        const int q = e & 3;                   // TMEM lane quarter (== warp id % 4)
-        const int grp = e >> 2;
-        const int row = q * 32 + lane;         // row inside this CTA's 128-row block == TMEM lane
-        uint8_t* bufs = stg + grp * Cfg::EPI_BUFS * SLICE_BYTES;
-        const int slice_cols = ep.out_f32 ? 32 : 64;
-        constexpr int NSP = SPLIT ? 2 : 1;
-        const uint32_t sw = uint32_t(row & 7);
-        int acc = 0, it = 0;
-        uint32_t acc_phase = 0;
-        for (int tile = pair, titer = 0; tile < num_tiles; tile += num_pairs, ++titer) {
-            (void)titer;
-            const int m_blk = tile % num_m, n_blk = tile / num_m;
-            const int m0 = m_blk * 2 * BM + int(cta) * BM;
-            mbar_wait(&tfull[acc], acc_phase);
-            if (cta == 0 && warp == 4 && lane == 0) VF_TRACE(2, titer);
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + acc * BN + (uint32_t(q * 32) << 16);
-#if VF_DBG_EPI != 9
-            bool keep = true;     // rows outside the valid conv region become the next layer's zero padding
-            if (cg.mask) {
-                const int m = m0 + row - cg.row0;
-                const int w = m % cg.Wp, r1 = m / cg.Wp;
-                const int hh = r1 % cg.Hp, r2 = r1 / cg.Hp;
-                const int tt = r2 % cg.Tp;
-                keep = (m >= 0) && (w >= cg.w0) && (w < cg.w1) && (hh >= cg.h0) && (hh < cg.h1) && (tt >= cg.t0) && (tt < cg.t1);
-            }
-#pragma unroll 1
-            for (int c = grp * slice_cols; c < BN; c += Cfg::NGRP * slice_cols)
-#pragma unroll
-            for (int sp = 0; sp < NSP; ++sp) {     // split output: the slice is produced twice, hi then lo
-                // this warp's 32 rows x 128 B of the group's slice buffer: its own TMA store of two slices ago (one slice ago
-                // with a single buffer) must have finished READING them before they are overwritten
-                uint8_t* buf = bufs + (Cfg::EPI_BUFS == 2 ? (it & 1) : 0) * SLICE_BYTES + q * 4096;
-                uint8_t* myrow = buf + lane * 128;
-                if (lane == 0) {
-                    if (Cfg::EPI_BUFS == 2) bulk_wait_read<1>(); else bulk_wait_read<0>();
-                }
-                __syncwarp();
-                const int n = n_blk * BN + c;
-                if (ep.out_f32) {
-                    float v[32];
-                    epi_load32(v, t_row + c, ep, n, N, keep);
-                    if (VF_DBG_EPI >= 2 && VF_DBG_EPI <= 3) {
-                        epi_sink(v);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<float4*>(myrow + ((uint32_t(j) ^ sw) << 4)) =
-                                make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    }
-                } else {
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        float v[32];
-                        epi_load32(v, t_row + c + hh * 32, ep, n + hh * 32, N, keep);
-                        if (SPLIT && sp) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] -= __half2float(__float2half_rn(v[j]));
-                        }
-                        if (VF_DBG_EPI >= 2 && VF_DBG_EPI <= 3) {
-                            epi_sink(v);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                *reinterpret_cast<uint4*>(myrow + ((uint32_t(hh * 4 + j) ^ sw) << 4)) =
-                                    make_uint4(pack_half2(v[8 * j], v[8 * j + 1]), pack_half2(v[8 * j + 2], v[8 * j + 3]),
-                                               pack_half2(v[8 * j + 4], v[8 * j + 5]), pack_half2(v[8 * j + 6], v[8 * j + 7]));
-                        }
-                    }
-                }
-                if (VF_DBG_EPI >= 2 && VF_DBG_EPI <= 3) {
-                    __syncwarp();
-                } else {
-                    // generic-proxy writes -> visible to the async proxy; then the warp's elected lane hands its
-                    // [32 x 128 B] box to the TMA unit.  Rows >= M and columns >= N are clipped by the TMA unit.  A group is
-                    // committed for EVERY slice, also for the (empty) ones right of N: uniform wait_group.read accounting.
-                    fence_proxy_async();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if ((VF_DBG_EPI == 0 || VF_DBG_EPI == 4) && n < N) {
-                            if (ep.accumulate) tma_reduce_add_2d(&tmO, buf, n, m0 + q * 32);
-                            else tma_store_2d((SPLIT && sp) ? &tmO2 : &tmO, buf, n, m0 + q * 32);
-                        }
-                        bulk_commit();
-                    }
-                }
-                ++it;
-            }
-#endif  // VF_DBG_EPI != 9
-            tc_fence_before();
-            __syncwarp();
-            if (cta == 0 && warp == 4 && lane == 0) VF_TRACE(3, titer);
-            if (lane == 0) mbar_arrive_remote(&tempty[acc], 0);   // this accumulator stage is drained
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-        if (lane == 0) bulk_wait<0>();   // all global writes of this warp are complete before the CTA retires
+        return;
     }
 
-    tc_fence_before();
-    cluster_sync_all();      // the peer's smem / barriers stay alive until the leader's MMAs and commits are done
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS);
+    // ---------------------------------------------------------------- consumers
+    const int wg = (warp >> 2) - 1;              // 0: tile rows 0..63, 1: rows 64..127
+    const int wq = warp & 3;                     // warp inside the warpgroup: 16 rows each
+    constexpr int R = BN / 2;                    // accumulator registers per thread
+    float acc[R];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
+        int prev = -1;
+        for (int kb = 0, kk = 0; kb < num_k; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint64_t adesc = wgmma_desc_sw128(sA + stage * Cfg::A_BYTES + wg * (64 * 128));
+            const uint64_t bdesc = wgmma_desc_sw128(sB + stage * Cfg::B_BYTES);
+            const bool lo_blk = NSPLIT == 2 && ((cg.lo_mask >> kk) & 1ull);
+            wgmma_fence_regs<R>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) {
+                Wgmma<BN>::mma(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0 ? 1u : 0u);
+                if (NSPLIT == 2 && !lo_blk) Wgmma<BN>::mma(acc, adesc + 2 * k, bdesc + (Cfg::B_TILE >> 4) + 2 * k, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                     // the group of the previous K block has retired: its stage is free
+            wgmma_fence_regs<R>(acc);
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            if (++kk == kpt) kk = 0;              // K block index inside the current tap
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs<R>(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+
+        // ------------------------------------------------------------ epilogue from registers
+        // accumulator register 4j + 2h + e: row (lane / 4) + 8h of this warp's 16, column 8j + 2 (lane % 4) + e
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            if (m >= M) continue;
+            bool keep = true;     // rows outside the valid conv region become the next layer's zero padding
+            if (cg.mask) {
+                const int mm = m - cg.row0;
+                const int w = mm % cg.Wp, r1 = mm / cg.Wp;
+                const int hh = r1 % cg.Hp, r2 = r1 / cg.Hp;
+                const int tt = r2 % cg.Tp;
+                keep = (mm >= 0) && (w >= cg.w0) && (w < cg.w1) && (hh >= cg.h0) && (hh < cg.h1) && (tt >= cg.t0) && (tt < cg.t1);
+            }
+            char* orow = static_cast<char*>(ep.out) + int64_t(m) * ep.ldo * (ep.out_f32 ? 4 : 2);
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = n0 + 8 * j + 2 * (lane & 3);
+                if (n >= N) continue;            // N % 8 == 0: n < N implies n + 1 < N
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (ep.scale) {
+                    const float2 s = __ldg(reinterpret_cast<const float2*>(ep.scale + n));
+                    v0 *= s.x; v1 *= s.y;
+                }
+                if (ep.bias) {
+                    const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + n));
+                    v0 += b.x; v1 += b.y;
+                }
+                if (ep.act != VF_ACT_NONE) { v0 = apply_act(v0, ep.act); v1 = apply_act(v1, ep.act); }
+                if (!keep) { v0 = 0.f; v1 = 0.f; }
+                if (ep.out_f32) {
+                    float* p = reinterpret_cast<float*>(orow) + n;
+                    if (ep.accumulate) atomicAdd(reinterpret_cast<float2*>(p), make_float2(v0, v1));   // one add per element: deterministic
+                    else *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
+                } else {
+                    __half* p = reinterpret_cast<__half*>(orow) + n;
+                    const __half2 hi = __floats2half2_rn(v0, v1);
+                    *reinterpret_cast<__half2*>(p) = hi;
+                    if (SPLIT)
+                        *reinterpret_cast<__half2*>(p + ep.split_off) =
+                            __floats2half2_rn(v0 - __low2float(hi), v1 - __high2float(hi));
+                }
+            }
+        }
     }
-#ifdef VF_DBG_TRACE
-    if (cta == 0 && threadIdx.x == 0) {
-        g_trace[pair][63][7] = clock64();
-        long long gt; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        g_trace[pair][63][5] = gt;
-    }
-#endif
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -413,25 +227,24 @@ EncodeTiledFn get_encode_tiled() {
     return fn;
 }
 
-template <int BN, int STAGES, int NSPLIT, bool SPLIT = false>
-int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmO2,
-                     const GemmEpi& ep, int M,
-                     int N, const ConvGeom& cg, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, STAGES, NSPLIT>;
+template <int BN, int NSPLIT, bool SPLIT = false>
+int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmEpi& ep, int M, int N, const ConvGeom& cg,
+                cudaStream_t stream) {
+    using Cfg = GemmCfg<BN, NSPLIT>;
     // one handle per thread, but several threads (one per handle) may reach the same instantiation at once: the attribute
     // call is idempotent, the flag that remembers it is an atomic (acquire / release), so there is no data race
     static std::atomic<bool> attr_set[64];
     int dev = 0;
     VF_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-        VF_CUDA(cudaFuncSetAttribute(gemm_f16_pair_kernel<BN, STAGES, NSPLIT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        VF_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BN, NSPLIT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      Cfg::SMEM_BYTES));
         if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
     }
-    const int tiles = ((M + 2 * BM - 1) / (2 * BM)) * ((N + BN - 1) / BN);
-    const int pairs = device_sm_count() / 2;
-    const int grid = 2 * (tiles < pairs ? tiles : pairs);
-    gemm_f16_pair_kernel<BN, STAGES, NSPLIT, SPLIT><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmO2, ep, M, N, cg);
+    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+    const int sms = device_sm_count();
+    const int grid = tiles < sms ? tiles : sms;
+    gemm_f16_kernel<BN, NSPLIT, SPLIT><<<grid, THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, ep, M, N, cg);
     VF_CUDA(cudaGetLastError());
     return VF_OK;
 }
@@ -441,10 +254,10 @@ int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUten
 int device_sm_count() {
     static std::atomic<int> sms[64];
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     int v = sms[dev].load(std::memory_order_relaxed);
     if (v == 0) {
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         sms[dev].store(v, std::memory_order_relaxed);
     }
     return v;
@@ -478,40 +291,42 @@ struct GemmProf {
 };
 static thread_local GemmProf g_prof;
 
-static int run_gemm_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmO2,
-                           int bn, const GemmEpi& ep,
-                           int M, int N, const ConvGeom& cg, cudaStream_t stream) {
+static int run_gemm_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, const GemmEpi& ep, int M, int N,
+                           const ConvGeom& cg, cudaStream_t stream) {
     if (ep.split_off > 0 && !ep.out_f32) {
         if (cg.nsplit == 2) {
-            if (bn == 256) return launch_gemm_pair<256, 4, 2, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-            if (bn == 192) return launch_gemm_pair<192, 4, 2, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-            if (bn == 128) return launch_gemm_pair<128, 6, 2, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-            return launch_gemm_pair<64, 8, 2, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
+            if (bn == 256) return launch_gemm<256, 2, true>(tmA, tmB, ep, M, N, cg, stream);
+            if (bn == 192) return launch_gemm<192, 2, true>(tmA, tmB, ep, M, N, cg, stream);
+            if (bn == 128) return launch_gemm<128, 2, true>(tmA, tmB, ep, M, N, cg, stream);
+            return launch_gemm<64, 2, true>(tmA, tmB, ep, M, N, cg, stream);
         }
-        if (bn == 256) return launch_gemm_pair<256, 5, 1, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-        if (bn == 192) return launch_gemm_pair<192, 5, 1, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-        if (bn == 128) return launch_gemm_pair<128, 6, 1, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-        return launch_gemm_pair<64, 8, 1, true>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
+        if (bn == 256) return launch_gemm<256, 1, true>(tmA, tmB, ep, M, N, cg, stream);
+        if (bn == 192) return launch_gemm<192, 1, true>(tmA, tmB, ep, M, N, cg, stream);
+        if (bn == 128) return launch_gemm<128, 1, true>(tmA, tmB, ep, M, N, cg, stream);
+        return launch_gemm<64, 1, true>(tmA, tmB, ep, M, N, cg, stream);
     }
     if (cg.nsplit == 2) {
-        if (bn == 256) return launch_gemm_pair<256, 4, 2>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-        if (bn == 192) return launch_gemm_pair<192, 4, 2>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-        if (bn == 128) return launch_gemm_pair<128, 6, 2>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-        return launch_gemm_pair<64, 8, 2>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
+        if (bn == 256) return launch_gemm<256, 2>(tmA, tmB, ep, M, N, cg, stream);
+        if (bn == 192) return launch_gemm<192, 2>(tmA, tmB, ep, M, N, cg, stream);
+        if (bn == 128) return launch_gemm<128, 2>(tmA, tmB, ep, M, N, cg, stream);
+        return launch_gemm<64, 2>(tmA, tmB, ep, M, N, cg, stream);
     }
-    if (bn == 256) return launch_gemm_pair<256, VF_STAGES_256, 1>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-    if (bn == 192) return launch_gemm_pair<192, 5, 1>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-    if (bn == 128) return launch_gemm_pair<128, 6, 1>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
-    return launch_gemm_pair<64, 8, 1>(tmA, tmB, tmO, tmO2, ep, M, N, cg, stream);
+    if (bn == 256) return launch_gemm<256, 1>(tmA, tmB, ep, M, N, cg, stream);
+    if (bn == 192) return launch_gemm<192, 1>(tmA, tmB, ep, M, N, cg, stream);
+    if (bn == 128) return launch_gemm<128, 1>(tmA, tmB, ep, M, N, cg, stream);
+    return launch_gemm<64, 1>(tmA, tmB, ep, M, N, cg, stream);
 }
 
 static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Ktot, int M, int N, const ConvGeom& cg,
                     const GemmEpi& ep, cudaStream_t stream) {
     if (!ep.out) return fail(VF_ERR_INVALID, "gemm: null output");
+    if (reinterpret_cast<uintptr_t>(ep.out) & 15) return fail(VF_ERR_INVALID, "gemm: output must be 16-byte aligned");
     if (ep.accumulate && !ep.out_f32) return fail(VF_ERR_INVALID, "gemm: accumulate needs fp32 output");
     if (N % 8) return fail(VF_ERR_INVALID, "gemm: N=%d must be a multiple of 8", N);
     if (ep.out_f32 ? (ep.ldo % 4) : (ep.ldo % 8)) return fail(VF_ERR_INVALID, "gemm: ldo breaks 16-byte rows");
-    // pair-tile width (the B box is half of it): the candidate that pads N least, the widest on a tie
+    if (ep.split_off && (ep.out_f32 || ep.split_off < N || ep.split_off % 8))
+        return fail(VF_ERR_INVALID, "gemm: split output needs fp16 out and split_off >= N, multiple of 8");
+    // tile width: the candidate that pads N least, the widest on a tie
     int bn = 64;
     if (N > 64) {
         int best = 0x7fffffff;
@@ -520,19 +335,9 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
             if (padded < best) { best = padded; bn = cand; }
         }
     }
-    CUtensorMap tmB, tmO, tmO2;
-    VF_TRY(make_tmap_2d(&tmB, B, 2, uint64_t(N), uint64_t(Ktot), uint64_t(ldb) * 2, uint32_t(bn / 2), BK));
-    const uint64_t ncols = uint64_t(N);     // (N % 8 == 0: a store view narrower than a 16-byte multiple corrupts its neighbours)
-    if (ep.out_f32) VF_TRY(make_tmap_2d(&tmO, ep.out, 4, uint64_t(M), ncols, uint64_t(ep.ldo) * 4, STORE_ROWS, 32));
-    else            VF_TRY(make_tmap_2d(&tmO, ep.out, 2, uint64_t(M), ncols, uint64_t(ep.ldo) * 2, STORE_ROWS, 64));
-    tmO2 = tmO;
-    if (ep.split_off) {     // second view of the output rows: the lo halves, both views clip at N columns
-        if (ep.out_f32 || ep.split_off < N || ep.split_off % 8)
-            return fail(VF_ERR_INVALID, "gemm: split output needs fp16 out and split_off >= N, multiple of 8");
-        VF_TRY(make_tmap_2d(&tmO2, static_cast<__half*>(ep.out) + ep.split_off, 2, uint64_t(M), ncols,
-                            uint64_t(ep.ldo) * 2, STORE_ROWS, 64));
-    }
-    if (!g_prof.on) return run_gemm_launch(tmA, tmB, tmO, tmO2, bn, ep, M, N, cg, stream);
+    CUtensorMap tmB;
+    VF_TRY(make_tmap_2d(&tmB, B, 2, uint64_t(N), uint64_t(Ktot), uint64_t(ldb) * 2, uint32_t(bn), BK));
+    if (!g_prof.on) return run_gemm_launch(tmA, tmB, bn, ep, M, N, cg, stream);
     if (g_prof.used + 2 > g_prof.ev.size())
         for (int i = 0; i < 2; ++i) {
             cudaEvent_t e;
@@ -540,7 +345,7 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
             g_prof.ev.push_back(e);
         }
     VF_CUDA(cudaEventRecord(g_prof.ev[g_prof.used], stream));
-    const int st = run_gemm_launch(tmA, tmB, tmO, tmO2, bn, ep, M, N, cg, stream);
+    const int st = run_gemm_launch(tmA, tmB, bn, ep, M, N, cg, stream);
     VF_CUDA(cudaEventRecord(g_prof.ev[g_prof.used + 1], stream));
     g_prof.used += 2;
     double kexec = double(Ktot);
@@ -554,16 +359,6 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
     return st;
 }
 
-#ifdef VF_DBG_TRACE
-extern "C" int vf_dbg_gemm_trace(long long* host_out) {     // 74 x 64 x 8 timestamps, after a device synchronise
-    cudaDeviceSynchronize();
-    return int(cudaMemcpyFromSymbol(host_out, g_trace, sizeof(g_trace)));
-}
-extern "C" int vf_dbg_gemm_trace_clear() {
-    static long long zeros[74 * 64 * 8];
-    return int(cudaMemcpyToSymbol(g_trace, zeros, sizeof(zeros)));
-}
-#endif
 bool gemm_profile_on() { return g_prof.on; }
 int gemm_profile(int enable) {
     g_prof.on = enable != 0;

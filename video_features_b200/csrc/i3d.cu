@@ -1,4 +1,4 @@
-// Inception-3D (I3D) feature extractor on the tcgen05 conv-GEMM.
+// Inception-3D (I3D) feature extractor on the wgmma conv-GEMM.
 // Replaces `I3D(num_classes=400, modality).forward(x, features=True)` (reference: models/i3d/i3d_src/i3d_net.py:238-264,
 // called at models/i3d/extract_i3d.py:186) and the stream transforms around it (extract_i3d.py:62-73).
 //
@@ -12,7 +12,7 @@
 //     [n][T/2+3][115][115][4 x 8*C] carries the 4 h-taps inside each row, so the GEMM walks 4 t-taps of 4*32*C contiguous
 //     elements (i3d_kernels.cu).
 // BatchNorm (eval) is folded into the epilogue's per-channel scale/bias (fp32), ReLU fused; branch outputs of a Mixed
-// block are written straight into their channel slice of the concat buffer (TMA store with the concat row pitch).
+// block are written straight into their channel slice of the concat buffer (stored with the concat row pitch).
 //
 // Numerics: accumulate fp32.  With single-fp16 weights the 1024-d feature is 1.7e-3 off the fp32 reference (trained
 // weights; CPU emulation in DESIGN.md); weights are therefore carried as a hi+lo fp16 pair and every K block is issued
@@ -264,9 +264,11 @@ int vf_i3d_create(vf_i3d_t** out, const vf_i3d_weights* w, int in_channels, int 
     if (max_stacks <= 0) max_stacks = 4;
     if (max_T <= 0) max_T = 64;
     VF_CUDA(cudaSetDevice(device));
-    int major = 0;
+    int major = 0, minor = 0;
     VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(VF_ERR_UNSUPPORTED, "device %d is not sm_100; this library is built for sm_100a only", device);
+    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+    if (major != 9 || minor != 0)
+        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
     vf_i3d* h = new vf_i3d();
     h->device = device; h->cin = in_channels; h->max_stacks = max_stacks; h->max_T = max_T;
     {

@@ -18,8 +18,7 @@ inline unsigned nblocks(int64_t total, int threads) { return unsigned((total + t
 // rows hq-1 .. hq+2 (slot sb = source row hq + sb - 1), each 8*C channels:
 //   out[tq][hq][wq][sb*8C + ((pt*2+ph)*2+pw)*C + c] = x[c][2(tq-1)+pt][2(hq+sb-2)+ph][2(wq-1)+pw]   (zero outside the clip)
 // i.e. the 4 h-taps are pre-gathered into the row, so the GEMM needs only the 4 t-taps (each a run of 4 w-positions x
-// 32*C channels): 3 KB of A operand per output row instead of 16 unaligned 192-byte runs -- the stem was bound by L2
-// operand traffic (ncu: 22.5 GB through L2, tensor pipe 31 %).
+// 32*C channels): 3 KB of A operand per output row instead of 16 unaligned 192-byte runs.
 //
 // x: [n][C][T][224][224] fp32 (already cropped + scaled to [-1,1], what the reference feeds I3D)
 __global__ void i3d_phase_pack_f32_kernel(const float* __restrict__ x, int n, int C, int T, __half* __restrict__ out,

@@ -33,7 +33,7 @@ int fail(int code, const char* fmt, ...);
 int make_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint64_t rows, uint64_t cols,
                  uint64_t row_pitch_bytes, uint32_t box_rows, uint32_t box_cols);
 
-// ---- GEMM: D[M,N] = act(A[M,K] . B[N,K]^T * scale[n] + bias[n]), fp16 operands, fp32 accumulate (tcgen05)
+// ---- GEMM: D[M,N] = act(A[M,K] . B[N,K]^T * scale[n] + bias[n]), fp16 operands, fp32 accumulate (wgmma)
 struct GemmEpi {
     void* out;              // fp16 or fp32, row pitch ldo elements, 16-byte aligned rows
     const float* bias;      // [N] or null
@@ -43,8 +43,8 @@ struct GemmEpi {
     int act;                // VF_ACT_*
     int split_off;          // fp16 out only: > 0 writes the result as a split-fp16 pair, hi at column n and
                             // lo = fp16(v - hi) at column split_off + n of the same row (0: plain fp16)
-    int accumulate;         // fp32 out only: 1 = out += result (a TMA reduction in the L2; every element is added exactly
-                            // once, so the sum is deterministic) -- the residual-stream update of the ViT blocks
+    int accumulate;         // fp32 out only: 1 = out += result (fp32x2 global reductions from the epilogue; every element
+                            // is added exactly once, so the sum is deterministic) -- the residual-stream update of the ViT blocks
 };
 int gemm_f16(const __half* A, int lda, const __half* B, int ldb, int M, int N, int K, const GemmEpi& ep,
              cudaStream_t stream);

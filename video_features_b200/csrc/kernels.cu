@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(256, 6) embed_layernorm768_kernel(const float*
 // Self-attention for one (frame, head): S = 50 tokens, head_dim 64, no mask.  q is scaled by 1/8 after the
 // in-projection (torch nn.MultiheadAttention semantics; applied here to the fp32 scores, which is the same
 // arithmetic since 1/8 is a power of two).  The two contractions are 64x64x64 after padding -- far too small for a
-// tcgen05 tile, so they run on warp-level mma.sync (m16n8k16, fp16 in / fp32 accumulate): one block of 4 warps
+// wgmma tile, so they run on warp-level mma.sync (m16n8k16, fp16 in / fp32 accumulate): one block of 4 warps
 // per (frame, head), warp w owns query rows 16w..16w+15.  Q, K, V are staged once in shared memory with 16-byte
 // cp.async (row pitch 144 B: conflict-free ldmatrix), fragments come from ldmatrix (.trans for V), the softmax
 // lives in the accumulator fragments (fp32) with quad shuffles, and O goes back through shared memory so that the

@@ -1,4 +1,4 @@
-// RAFT optical flow (full model, 20 refinement iterations) on the tcgen05 conv-GEMM.
+// RAFT optical flow (full model, 20 refinement iterations) on the wgmma conv-GEMM.
 // Replaces `RAFT()(image1, image2, iters=20, test_mode=True)` (reference: models/raft/raft_src/raft.py:115-174, called at
 // models/raft/extract_raft.py:99 and models/i3d/extract_i3d.py:172) together with InputPadder (raft.py:27-44).
 //
@@ -399,9 +399,11 @@ int vf_raft_create(vf_raft_t** out, const vf_named_tensor* tensors, int n_tensor
     if (max_frames < 2) max_frames = 2;
     if (max_h <= 0 || max_w <= 0) return fail(VF_ERR_INVALID, "raft_create: max frame size required");
     VF_CUDA(cudaSetDevice(device));
-    int major = 0;
+    int major = 0, minor = 0;
     VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(VF_ERR_UNSUPPORTED, "device %d is not sm_100; this library is built for sm_100a only", device);
+    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+    if (major != 9 || minor != 0)
+        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
     vf_raft* h = new vf_raft();
     h->device = device; h->max_frames = max_frames;
     h->max_h = (max_h + 7) / 8 * 8; h->max_w = (max_w + 7) / 8 * 8;

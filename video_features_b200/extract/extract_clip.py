@@ -1,4 +1,4 @@
-"""``ExtractCLIP`` -- drop-in for the reference's models/CLIP/extract_clip.py on the B200 engine.
+"""``ExtractCLIP`` -- drop-in for the reference's models/CLIP/extract_clip.py on the H100 engine.
 
 Same constructor, attributes, ``forward(indices)`` / ``extract(...)`` signatures, dict keys and file naming.  What
 changes underneath: ``clip.load`` is replaced by a ``ClipEngine`` (device weights + workspace), and ``preprocess`` +
@@ -139,7 +139,7 @@ class ExtractCLIP(torch.nn.Module):
 
     def _engine(self, device: torch.device) -> ClipEngine:
         if device.type != 'cuda':
-            raise RuntimeError("the B200 engine has no CPU path: pass indices on a CUDA device "
+            raise RuntimeError("the H100 engine has no CPU path: pass indices on a CUDA device "
                                "(the reference's --cpu flow is timed by bench.py --impl reference)")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if idx not in self._engines:

@@ -1,4 +1,4 @@
-"""``ExtractI3D`` -- drop-in for the reference's models/i3d/extract_i3d.py on the B200 engine.
+"""``ExtractI3D`` -- drop-in for the reference's models/i3d/extract_i3d.py on the H100 engine.
 
 Same constructor / attributes / ``forward(indices)`` / ``extract(...)`` surface, dict keys ('rgb', 'flow', 'fps',
 'timestamps_ms'), stack / step logic (stack_size+1 frames per stack, one overlap frame when step == stack) and
@@ -89,7 +89,7 @@ class ExtractI3D(torch.nn.Module):
             self.output_path = args.output_path if self.output_direct is True else os.path.join(args.output_path, self.feature_type)
         if 'flow' in self.streams and self.flow_type not in ('raft', 'flow'):
             raise NotImplementedError(f"flow_type '{self.flow_type}': the RAFT and pre-computed flow branches are built "
-                                      "on the B200 engine (pass --flow_type raft / flow, or --streams rgb)")
+                                      "on the H100 engine (pass --flow_type raft / flow, or --streams rgb)")
         self.progress = tqdm(total=len(self.path_list))
         self.group_stacks = max(1, int(os.environ.get("VF_I3D_STACKS", "8")))     # stacks per engine call
         self.keep_features = False
@@ -97,7 +97,7 @@ class ExtractI3D(torch.nn.Module):
 
     def _load(self, device: torch.device) -> dict:
         if device.type != 'cuda':
-            raise RuntimeError("the B200 engine has no CPU path: pass indices on a CUDA device")
+            raise RuntimeError("the H100 engine has no CPU path: pass indices on a CUDA device")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if idx not in self._models:
             m = {s: I3DEngine(load_checkpoint(s), s, idx, max_stacks=self.group_stacks, max_T=max(self.stack_size, 16))

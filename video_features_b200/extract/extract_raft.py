@@ -1,4 +1,4 @@
-"""``ExtractRAFT`` -- drop-in for the reference's models/raft/extract_raft.py on the B200 engine.
+"""``ExtractRAFT`` -- drop-in for the reference's models/raft/extract_raft.py on the H100 engine.
 
 Same constructor / attributes / ``forward`` (returns None) / ``extract`` surface; output key 'raft' is a float64
 ``(T-1, 2, H, W)`` array (the reference builds it with ``.tolist()``), saved under ``{output_path}/raft``.  Frames are
@@ -47,7 +47,7 @@ class ExtractRAFT(torch.nn.Module):
     def forward(self, indices: torch.LongTensor):
         device = indices.device
         if device.type != 'cuda':
-            raise RuntimeError("the B200 engine has no CPU path: pass indices on a CUDA device")
+            raise RuntimeError("the H100 engine has no CPU path: pass indices on a CUDA device")
         sink = AsyncSink() if os.environ.get("VF_ASYNC_SINK") == "1" else None     # opt-in extras, see ExtractCLIP.forward
         resume = os.environ.get("VF_RESUME") == "1"
         try:

@@ -29,7 +29,7 @@ class I3DEngine:
     def __init__(self, state_dict: Dict[str, torch.Tensor], modality: str = "rgb", device: int = 0,
                  max_stacks: int = 4, max_T: int = 64):
         if not torch.cuda.is_available():
-            raise RuntimeError("I3DEngine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("I3DEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.modality = modality
         self.cin = 3 if modality == "rgb" else 2
         self.device = torch.device("cuda", device)

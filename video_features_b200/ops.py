@@ -35,7 +35,7 @@ def _need_cuda(*ts: torch.Tensor) -> None:
 @torch.library.custom_op("vfeat::gemm_f16", mutates_args=())
 def gemm_f16(a: torch.Tensor, b: torch.Tensor, bias: Optional[torch.Tensor], scale: Optional[torch.Tensor],
              act: int, out_f32: bool) -> torch.Tensor:
-    """act(a @ b.T * scale + bias); a (M,K) fp16, b (N,K) fp16; fp32 accumulate on tcgen05."""
+    """act(a @ b.T * scale + bias); a (M,K) fp16, b (N,K) fp16; fp32 accumulate on wgmma."""
     _need_cuda(a, b, bias, scale)
     assert a.dtype == torch.float16 and b.dtype == torch.float16 and a.shape[1] == b.shape[1]
     M, K = a.shape
@@ -54,7 +54,7 @@ def _(a, b, bias, scale, act, out_f32):
 
 @torch.library.custom_op("vfeat::gemm_f16_accumulate", mutates_args=("out",))
 def gemm_f16_accumulate(out: torch.Tensor, a: torch.Tensor, b: torch.Tensor, bias: Optional[torch.Tensor], act: int) -> None:
-    """out (M,N) fp32 += act(a @ b.T + bias): the residual-stream update, added in the L2 by a TMA reduction."""
+    """out (M,N) fp32 += act(a @ b.T + bias): the residual-stream update, added by global fp32 reductions from the GEMM epilogue."""
     _need_cuda(out, a, b, bias)
     assert out.dtype == torch.float32 and a.dtype == torch.float16 and b.dtype == torch.float16
     M, K = a.shape

@@ -17,7 +17,7 @@ class RAFTEngine:
     def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, max_frames: int = 65, max_h: int = 272,
                  max_w: int = 480):
         if not torch.cuda.is_available():
-            raise RuntimeError("RAFTEngine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("RAFTEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         keep, names = [], []
         items = [(k[7:] if k.startswith("module.") else k, v) for k, v in state_dict.items()
