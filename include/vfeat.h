@@ -75,6 +75,19 @@ int vf_gemm_f16_accumulate(const void* A, int lda, const void* B, int ldb, int M
  * consumer's weights are duplicated over both halves, which restores ~22 mantissa bits on the activation operand. */
 int vf_gemm_f16_split(const void* A, int lda, const void* B, int ldb, int M, int N, int K, void* D, int ldd, int split_off,
                       const float* bias, const float* scale, int act, void* stream);
+/* The same GEMM in its shifted-row convolution mode, the one every I3D / RAFT convolution runs (exported for the parity
+ * tests).  X holds channels-last rows of C elements (fp16, row pitch C); row p of the A operand of tap j is the
+ * k_per_tap contiguous elements starting at element (p + tap_off[j]) * C, so X must be readable for (P-1)*C + k_per_tap
+ * elements, and rows that fall before 0 or at / past P read as zeros.  Wt: N x (nsplit*ntaps*k_per_tap) fp16, row-major,
+ * tap j at columns j*k_per_tap; nsplit = 2 appends the lo halves of a hi+lo weight pair after all the hi columns.
+ * lo_mask (nsplit = 2): bit kk skips the W_lo pass on K block kk (64 columns) of every tap; bits must name existing
+ * blocks of a tap of at most 64 blocks.  region: NULL (no mask) or {Tp, Hp, Wp, t0, t1, h0, h1, w0, w1}: output row m
+ * is volume position m - row0 of [n][Tp][Hp][Wp] and is written as 0 outside [t0,t1) x [h0,h1) x [w0,w1) and for
+ * m < row0.  D: P rows of pitch ldd, fp16 or fp32 (out_f32); split_off > 0 writes a split-fp16 pair as vf_gemm_f16_split
+ * does.  1 <= ntaps <= 64, C and k_per_tap multiples of 8, N a multiple of 8. */
+int vf_conv_gemm_f16(const void* X, int C, int64_t P, const void* Wt, int N, int ntaps, int k_per_tap, const int* tap_off,
+                     int nsplit, uint64_t lo_mask, int row0, const int* region, void* D, int ldd, int out_f32, int split_off,
+                     const float* bias, const float* scale, int act, void* stream);
 
 /* Roofline instrumentation (bench.py): while enabled on the calling thread, every wgmma GEMM launch of any handle
  * is bracketed by CUDA events on its stream.  _read synchronises the device and returns the summed device time (ms),

@@ -105,12 +105,13 @@ def test_encode_with_outlier_channel_weights(cuda_device):
         eng.close()
 
 
-@pytest.mark.parametrize("n_frames", [1, 4, 5, 7, 23, 250])
+@pytest.mark.parametrize("n_frames", [1, 2, 4, 5, 7, 22, 23, 250])
 def test_fused_qkv_attention_vs_fp32_reference_and_split_path(tower, cuda_device, n_frames):
-    """The QKV-projection + attention kernel (one tile = 5 frames x 1 head on a CTA pair, the third frame straddling the
-    pair through distributed shared memory) against nn.MultiheadAttention's math in fp32, and against the split path (QKV
-    GEMM + stand-alone attention kernel).  Frame counts: single frame, below / at / above one 5-frame group, a ragged
-    last group, a full chunk."""
+    """The QKV-projection + attention kernel (one tile = 2 frames x 1 head: the 100 token rows of a 128-row wgmma tile,
+    whose last 28 rows are computed and dropped) against nn.MultiheadAttention's math in fp32, and against the split
+    path (QKV GEMM + stand-alone attention kernel).  Frame counts: a single frame (half-empty tile), exactly one tile,
+    even and odd counts (a ragged last tile), 22 frames = 11 x 12 = 132 tiles (exactly one wave on 132 SMs), 23 frames
+    (one tile past the wave), a full chunk (several tiles per CTA)."""
     sd, eng = tower
     g = torch.Generator().manual_seed(40 + n_frames)
     x = torch.randn(n_frames * 50, 768, generator=g).half().to(cuda_device)

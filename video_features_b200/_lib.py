@@ -72,6 +72,9 @@ SIGNATURES = {
                                          C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "vf_gemm_f16_split": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                     C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "vf_conv_gemm_f16": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                   C.POINTER(C.c_int), C.c_int, C.c_uint64, C.c_int, C.POINTER(C.c_int), C.c_void_p,
+                                   C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "vf_gemm_profile": (C.c_int, [C.c_int]),
     "vf_gemm_profile_read": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
     "vf_clip_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(ClipWeights), C.c_int, C.c_int]),

@@ -400,10 +400,17 @@ int conv_gemm_f16(const __half* X, int C, int64_t P, const __half* Wt, int N, co
     if (C % 8) return fail(VF_ERR_INVALID, "conv_gemm: C=%d must be a multiple of 8", C);
     if (g.ntaps < 1 || g.ntaps > 64 || g.k_per_tap < 8 || g.k_per_tap % 8)
         return fail(VF_ERR_INVALID, "conv_gemm: bad tap geometry (%d taps x %d)", g.ntaps, g.k_per_tap);
+    if (g.nsplit != 1 && g.nsplit != 2) return fail(VF_ERR_INVALID, "conv_gemm: nsplit must be 1 or 2");
+    // lo_mask bit kk names K block kk of a tap; the kernel tests it with lo_mask >> kk, so a tap of more than 64 blocks
+    // cannot carry a mask, and a bit at or above the tap's block count would name a block that does not exist
+    const int kpt = (g.k_per_tap + BK - 1) / BK;
+    if (g.lo_mask && (kpt > 64 || (kpt < 64 && (g.lo_mask >> kpt) != 0)))
+        return fail(VF_ERR_INVALID, "conv_gemm: lo_mask 0x%llx names K blocks beyond the %d of a tap", g.lo_mask, kpt);
+    if (g.mask && (g.Tp < 1 || g.Hp < 1 || g.Wp < 1 || g.row0 < 0))
+        return fail(VF_ERR_INVALID, "conv_gemm: bad mask volume %dx%dx%d, row0 %d", g.Tp, g.Hp, g.Wp, g.row0);
     // overlapping-row view: row p = k_per_tap contiguous elements starting at element p*C
     CUtensorMap tmA;
     VF_TRY(make_tmap_2d(&tmA, X, 2, uint64_t(P), uint64_t(g.k_per_tap), uint64_t(C) * 2, BM, BK));
-    if (g.nsplit != 1 && g.nsplit != 2) return fail(VF_ERR_INVALID, "conv_gemm: nsplit must be 1 or 2");
     const int64_t Ktot = int64_t(g.ntaps) * g.k_per_tap * g.nsplit;
     if (Ktot % 8) return fail(VF_ERR_INVALID, "conv_gemm: K must be a multiple of 8");
     return run_gemm(tmA, Wt, int(Ktot), Ktot, int(P), N, g, ep, stream);

@@ -266,4 +266,27 @@ int vf_gemm_f16_split(const void* A, int lda, const void* B, int ldb, int M, int
                     static_cast<cudaStream_t>(stream));
 }
 
+int vf_conv_gemm_f16(const void* X, int C, int64_t P, const void* Wt, int N, int ntaps, int k_per_tap, const int* tap_off,
+                     int nsplit, uint64_t lo_mask, int row0, const int* region, void* D, int ldd, int out_f32, int split_off,
+                     const float* bias, const float* scale, int act, void* stream) {
+    if (!X || !Wt || !D || !tap_off) return fail(VF_ERR_INVALID, "conv_gemm: null buffer");
+    if (ntaps < 1 || ntaps > 64) return fail(VF_ERR_INVALID, "conv_gemm: %d taps (1..64)", ntaps);
+    if (split_off > 0 && ldd < split_off + N)
+        return fail(VF_ERR_INVALID, "conv_gemm: split output needs ldd >= split_off + N");
+    ConvGeom g;
+    memset(&g, 0, sizeof(g));
+    g.ntaps = ntaps; g.k_per_tap = k_per_tap; g.nsplit = nsplit; g.lo_mask = lo_mask; g.row0 = row0;
+    memcpy(g.tap_off, tap_off, sizeof(int) * size_t(ntaps));
+    if (region) {
+        g.mask = 1;
+        g.Tp = region[0]; g.Hp = region[1]; g.Wp = region[2];
+        g.t0 = region[3]; g.t1 = region[4]; g.h0 = region[5]; g.h1 = region[6]; g.w0 = region[7]; g.w1 = region[8];
+    }
+    GemmEpi ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.out = D; ep.ldo = ldd; ep.out_f32 = out_f32; ep.bias = bias; ep.scale = scale; ep.act = act; ep.split_off = split_off;
+    return conv_gemm_f16(static_cast<const __half*>(X), C, P, static_cast<const __half*>(Wt), N, g, ep,
+                         static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
