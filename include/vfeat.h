@@ -229,6 +229,26 @@ int vf_raft_padded_size(int Hs, int Ws, int* H, int* W);
 int vf_raft_debug_read(vf_raft_t* h, int what, float* out, int64_t capacity, int* dims4, void* stream);
 int64_t vf_raft_launch_count(const vf_raft_t* h);
 
+/* ---- ResNet-18/34/50/101/152 frame features: replaces torchvision `models.resnetXX(pretrained=True)` with
+ * `fc = Identity()` in eval mode, and its per-frame transform Resize(256) -> CenterCrop(224) -> ToTensor -> Normalize
+ * (models/resnet/extract_resnet.py:32-38,52-72,108).  Weights: the torchvision state_dict by key (optionally with the
+ * "module." prefix), HOST fp32; fc.* is ignored.  An unknown depth, or a missing / mis-sized tensor, is VF_ERR_INVALID. */
+typedef struct vf_resnet vf_resnet_t;
+
+/* depth: 18, 34, 50, 101 or 152.  Workspace holds max_frames frames (0 = 64); larger calls run in chunks of that size. */
+int vf_resnet_create(vf_resnet_t** out, const vf_named_tensor* tensors, int n_tensors, int depth, int device, int max_frames);
+int vf_resnet_destroy(vf_resnet_t* h);
+/* frames: n x 3 x 224 x 224 fp32 on the device, already transformed (the tensor the reference passes to the model)
+ * -> out: n x D fp32 (D = 512 for depths 18 / 34, 2048 otherwise). */
+int vf_resnet_forward_f32(vf_resnet_t* h, const float* frames, int n, float* out, void* stream);
+/* transform fused: frames n x Hr x Wr x 3 uint8 BGR on the device (the decoder's order), already resized to short side
+ * 256 (vf_resize_u8, bilinear) -> BGR->RGB, CenterCrop(224), ToTensor, Normalize -> network.  Hr, Wr >= 224. */
+int vf_resnet_forward_u8(vf_resnet_t* h, const uint8_t* frames, int n, int Hr, int Wr, float* out, void* stream);
+/* Diagnostics: an activation of the last chunk of the last call as fp32 NCHW: stage 0 stem (conv1 + bn1 + relu),
+ * 1 maxpool, 2..5 layer1..layer4.  dims4 receives (n, C, H, W); out == NULL only queries the shape. */
+int vf_resnet_read_stage(vf_resnet_t* h, int stage, float* out, int64_t capacity, int* dims4, void* stream);
+int64_t vf_resnet_launch_count(const vf_resnet_t* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,7 +10,8 @@ import torch  # noqa: F401
 
 from video_features_b200.utils import form_list_from_user_input, sanity_check
 
-SUPPORTED = ['i3d', 'raft', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32']
+SUPPORTED = ['i3d', 'raft', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
+             'resnet101', 'resnet152']
 
 
 def build_extractor(args):
@@ -24,8 +25,10 @@ def build_extractor(args):
     if args.feature_type == 'raft':
         from video_features_b200.extract.extract_raft import ExtractRAFT
         return ExtractRAFT(args)
-    if args.feature_type in ['vggish', 'r21d_rgb', 'resnet18', 'resnet34', 'resnet50', 'resnet101', 'resnet152', 'pwc',
-                             'vggish_torch']:
+    if args.feature_type in ['resnet18', 'resnet34', 'resnet50', 'resnet101', 'resnet152']:
+        from video_features_b200.extract.extract_resnet import ExtractResNet
+        return ExtractResNet(args)
+    if args.feature_type in ['vggish', 'r21d_rgb', 'pwc', 'vggish_torch']:
         raise NotImplementedError(f'{args.feature_type}: outside the hot path this engine rebuilds (SURVEY.md §2)')
     raise NotADirectoryError                      # main.py:41
 

@@ -230,3 +230,63 @@ def raft_golden():
 
 if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "raft":
     raft_golden()
+
+
+def resnet_golden():
+    """The reference's own ExtractResNet.extract on the sample video, with torchvision's resnet constructors patched to
+    return the calibrated stand-in (oracle/resnet_net.py); stores fps, timestamps, a sha1 per frame of the transform
+    output, and the feature rows of every 16th frame plus the last, for resnet18 and resnet50."""
+    import argparse
+    import torch
+    from oracle import resnet_net
+    install_mmcv_shim()
+    sys.path.insert(0, REF)
+    cwd = os.getcwd()
+    os.chdir(REF)
+    try:
+        from models.resnet import extract_resnet
+        video = os.path.join(REF, "sample", "v_GGSY1Qvo990.mp4")
+        d = {}
+        for depth in (18, 50):
+            name = f"resnet{depth}"
+            tv = extract_resnet.models
+
+            sd = resnet_net.stand_in_state_dict(depth)       # built before the constructor is patched
+            orig = getattr(tv, name)
+
+            def patched(pretrained=False, _sd=sd, _orig=orig):
+                net = _orig(weights=None)
+                net.load_state_dict(_sd)
+                return net
+            args = argparse.Namespace(feature_type=name, video_paths=[video], file_with_video_paths=None, batch_size=16,
+                                      extraction_fps=None, show_pred=False, keep_tmp_files=False, on_extraction="print",
+                                      tmp_path="./tmp", output_path="./output", video_dir=None,
+                                      flow_paths=None, flow_dir=None)
+            ex = extract_resnet.ExtractResNet(args)
+            hashes = []
+            tf = ex.transforms
+
+            def hashing(img, _tf=tf, _h=hashes):
+                t = _tf(img)
+                _h.append(resnet_net.tensor_hash(t))
+                return t
+            ex.transforms = hashing
+            setattr(tv, name, patched)
+            model = getattr(tv, name)(pretrained=True).eval()
+            model.fc = torch.nn.Identity()
+            out = ex.extract(torch.device("cpu"), model, None, video)
+            setattr(tv, name, orig)
+            feats = out[name]
+            n = feats.shape[0]
+            rows = np.array(sorted(set(range(0, n, 16)) | {n - 1}), np.int64)
+            d[name] = feats[rows]
+            d["rows"], d["fps"], d["timestamps_ms"] = rows, out["fps"], out["timestamps_ms"]
+            d["transform_sha1"] = np.array(hashes)
+            print(f"{name}: {n} frames, fps {out['fps']}, kept rows {len(rows)}")
+        np.savez_compressed(os.path.join(OUT, "resnet_outputs.npz"), **d)
+    finally:
+        os.chdir(cwd)
+
+
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "resnet":
+    resnet_golden()
