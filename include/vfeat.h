@@ -249,6 +249,30 @@ int vf_resnet_forward_u8(vf_resnet_t* h, const uint8_t* frames, int n, int Hr, i
 int vf_resnet_read_stage(vf_resnet_t* h, int stage, float* out, int64_t capacity, int* dims4, void* stream);
 int64_t vf_resnet_launch_count(const vf_resnet_t* h);
 
+/* ---- R(2+1)D-18 clip features: replaces torchvision `r2plus1d_18(pretrained=True)` with `fc = Identity()` in eval mode,
+ * and its clip transform ToFloatTensorInZeroOne -> Resize((128, 171)) -> Normalize -> CenterCrop(112)
+ * (models/r21d/extract_r21d.py).  Weights: the torchvision state_dict by key (optionally with the "module." prefix),
+ * HOST fp32; fc.* is ignored.  A missing / mis-sized tensor is VF_ERR_INVALID. */
+typedef struct vf_r21d vf_r21d_t;
+
+/* Workspace holds max_clips clips of max_T frames (0 = 4 and 16); a call of T-frame clips runs in chunks of
+ * max_clips * (max_T + 2) / (T + 2) clips (at most 256), so any T up to that holds with bounded device memory. */
+int vf_r21d_create(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips, int max_T);
+int vf_r21d_destroy(vf_r21d_t* h);
+/* clips: n x 3 x T x 112 x 112 fp32 on the device, already transformed (the tensor the reference passes to the model)
+ * -> out: n x 512 fp32. */
+int vf_r21d_forward_f32(vf_r21d_t* h, const float* clips, int n, int T, float* out, void* stream);
+/* transform fused: frames n_frames x H x W x 3 uint8 BGR on the device (the decoder's order, any size); clip i is
+ * frames starts[i] .. starts[i] + T - 1 (starts: HOST array of n ints) -> BGR->RGB, /255, bilinear Resize((128, 171))
+ * of the 112 x 112 CenterCrop window, Normalize -> network -> out: n x 512 fp32.  A frame that several clips of one
+ * chunk share is transformed once. */
+int vf_r21d_forward_u8(vf_r21d_t* h, const uint8_t* frames, int n_frames, int H, int W, const int* starts, int n, int T,
+                       float* out, void* stream);
+/* Diagnostics: an activation of the last chunk of the last call as fp32 NCTHW: stage 0 stem (after the temporal
+ * conv), 1..4 layer1..layer4.  dims5 receives (n, C, T, H, W); out == NULL only queries the shape. */
+int vf_r21d_read_stage(vf_r21d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream);
+int64_t vf_r21d_launch_count(const vf_r21d_t* h);
+
 #ifdef __cplusplus
 }
 #endif

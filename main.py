@@ -11,7 +11,7 @@ import torch  # noqa: F401
 from video_features_b200.utils import form_list_from_user_input, sanity_check
 
 SUPPORTED = ['i3d', 'raft', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
-             'resnet101', 'resnet152']
+             'resnet101', 'resnet152', 'r21d_rgb']
 
 
 def build_extractor(args):
@@ -28,7 +28,10 @@ def build_extractor(args):
     if args.feature_type in ['resnet18', 'resnet34', 'resnet50', 'resnet101', 'resnet152']:
         from video_features_b200.extract.extract_resnet import ExtractResNet
         return ExtractResNet(args)
-    if args.feature_type in ['vggish', 'r21d_rgb', 'pwc', 'vggish_torch']:
+    if args.feature_type == 'r21d_rgb':
+        from video_features_b200.extract.extract_r21d import ExtractR21D
+        return ExtractR21D(args)
+    if args.feature_type in ['vggish', 'pwc', 'vggish_torch']:
         raise NotImplementedError(f'{args.feature_type}: outside the hot path this engine rebuilds (SURVEY.md §2)')
     raise NotADirectoryError                      # main.py:41
 
@@ -82,8 +85,8 @@ _FLAGS = [
     ('--output_direct', dict(action='store_true', help='save as <output_path>/<video stem>.npy')),
     ('--extraction_fps', dict(type=float, help='resample to this frame rate first (I3D)')),
     ('--extract_method', dict(type=str, help='frame sampler: uni_N or fix_N')),
-    ('--stack_size', dict(type=int, help='frames per I3D stack')),
-    ('--step_size', dict(type=int, help='frames between I3D stacks')),
+    ('--stack_size', dict(type=int, help='frames per I3D / R(2+1)D stack')),
+    ('--step_size', dict(type=int, help='frames between I3D / R(2+1)D stacks')),
     ('--streams', dict(nargs='+', choices=['flow', 'rgb'], help='I3D streams (default: both)')),
     ('--flow_type', dict(choices=['raft', 'pwc', 'flow'], default='pwc', help='optical flow feeding the I3D flow stream')),
     ('--batch_size', dict(type=int, default=1, help='frame pairs per RAFT call')),

@@ -290,3 +290,48 @@ def resnet_golden():
 
 if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "resnet":
     resnet_golden()
+
+
+def r21d_golden():
+    """The reference's own R(2+1)D pieces on the sample video, with the calibrated stand-in (oracle/r21d_net.py):
+    frames decoded with OpenCV and swapped BGR->RGB (the reference's torchvision.io.read_video needs PyAV), the
+    reference's rgb_transforms Compose, its form_slices, and torchvision r2plus1d_18 with fc = Identity.  Stores the
+    sha1 of every transformed stack and all feature rows (355 frames -> 22 stacks of 16)."""
+    import cv2
+    import torch
+    import torchvision
+    from torchvision.transforms import Compose
+    from oracle import r21d_net
+    install_mmcv_shim()
+    sys.path.insert(0, REF)
+    import models.r21d.transforms.rgb_transforms as T
+    from utils.utils import form_slices
+    cap = cv2.VideoCapture(os.path.join(REF, "sample", "v_GGSY1Qvo990.mp4"))
+    frames = []
+    while True:
+        ok, bgr = cap.read()
+        if not ok:
+            break
+        frames.append(bgr[:, :, ::-1].copy())
+    rgb = torch.from_numpy(np.stack(frames))                                 # (T, H, W, 3), read_video's layout
+    tf = Compose([T.ToFloatTensorInZeroOne(), T.Resize((128, 171)),
+                  T.Normalize(mean=[0.43216, 0.394666, 0.37645], std=[0.22803, 0.22145, 0.216989]),
+                  T.CenterCrop((112, 112))])                                 # extract_r21d.py's Compose
+    x = tf(rgb).unsqueeze(0)
+    net = torchvision.models.video.r2plus1d_18(weights=None)
+    net.load_state_dict(r21d_net.stand_in_state_dict())
+    net.fc = torch.nn.Identity()
+    net.eval()
+    feats, hashes = [], []
+    with torch.no_grad():
+        for s, e in form_slices(x.size(2), 16, 16):
+            hashes.append(r21d_net.tensor_hash(x[0, :, s:e]))
+            feats.extend(net(x[:, :, s:e]).tolist())
+    feats = np.array(feats)
+    print(f"r21d: {len(frames)} frames -> {feats.shape}")
+    np.savez_compressed(os.path.join(OUT, "r21d_outputs.npz"), r21d_rgb=feats, transform_sha1=np.array(hashes),
+                        n_frames=np.array(len(frames)))
+
+
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "r21d":
+    r21d_golden()

@@ -112,6 +112,13 @@ SIGNATURES = {
     "vf_resnet_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_resnet_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
     "vf_resnet_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_r21d_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vf_r21d_destroy": (C.c_int, [C.c_void_p]),
+    "vf_r21d_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_r21d_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int,
+                                     C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_r21d_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_r21d_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_clip_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "vf_clip_profile_categories": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
     "vf_clip_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
