@@ -94,6 +94,12 @@ template <int N>
 __device__ __forceinline__ void bulk_wait() {        // <= N groups not yet complete
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
 // make generic-proxy shared-memory writes visible to the async proxy (TMA) before it reads them
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {

@@ -9,8 +9,10 @@
 //                  pair (full / empty) per stage.  It runs ahead into the next tile while the consumers store this one.
 //   warpgroups 1,2 consumers: rows 0..63 and 64..127 of the tile.  Per 64-wide K block, four wgmma m64nBNk16 (eight with
 //                  split weights), one commit group; the stage is released as soon as the group behind it has retired.
-//                  Epilogue straight from the accumulator registers: scale / bias / activation, row mask, then fp16x2 or
-//                  fp32x2 global stores (fp32x2 reductions for `accumulate`), M / N tails clipped per element.
+//                  Epilogue: scale / bias / activation and row mask in registers, then 64-row x 128-byte subtiles
+//                  through two swizzled shared-memory buffers per warpgroup, each handed to a TMA store (TMA reduce-add
+//                  for `accumulate`) that TMA clips at N and M.  The consumers go on to the next tile's main loop while
+//                  the stores drain.
 //
 // Used for every dense contraction of the hot path: ViT patch-embed / QKV / out-proj / FFN GEMMs (reference:
 // third-party clip `VisionTransformer.forward`, called at models/CLIP/extract_clip.py:128) and the I3D / RAFT
@@ -34,7 +36,14 @@ constexpr int BM = 128;          // rows per CTA tile (64 per consumer warpgroup
 constexpr int BK = 64;           // 64 fp16 = one 128-byte swizzle row
 constexpr int THREADS = 384;     // producer warpgroup + two consumer warpgroups
 constexpr int CONSUMER_WARPS = 8;
-constexpr uint32_t SMEM_BUDGET = 200 * 1024;   // operand ring; the rest of the 227 KB stays free
+constexpr int EPI_ROWS = 64;                   // output rows per consumer warpgroup = rows of one TMA store box
+constexpr uint32_t STG_BYTES = EPI_ROWS * 128; // one staging subtile: 64 rows x 128 bytes (64 fp16 / 32 fp32 columns)
+constexpr uint32_t STAGING_BYTES = 2 * 2 * STG_BYTES;   // two warpgroups x two buffers
+constexpr uint32_t SMEM_LIMIT = 227 * 1024;    // opt-in dynamic shared memory per block on sm_90
+constexpr uint32_t MAX_STAGES = 8;
+// operand ring = what is left after the staging buffers, the barriers of MAX_STAGES stages and the alignment slack:
+// 194 KB, i.e. stages (plain / split weights) 4 / 2 at BN = 256, 4 / 3 at 192, 6 / 4 at 128, 8 / 6 at 64.
+constexpr uint32_t RING_BUDGET = SMEM_LIMIT - STAGING_BYTES - 2 * MAX_STAGES * 8 - 1024;
 
 // NSPLIT = 2: the B stage holds the hi and the lo tile of a split-fp16 weight matrix and every K step issues two
 // MMAs against the same A tile.
@@ -44,11 +53,12 @@ struct GemmCfg {
     static constexpr uint32_t B_TILE = BN * BK * 2;           // one of hi / lo
     static constexpr uint32_t B_BYTES = NSPLIT * B_TILE;
     static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = int(SMEM_BUDGET / STAGE_BYTES) > 8 ? 8 : int(SMEM_BUDGET / STAGE_BYTES);
+    static constexpr int STAGES = RING_BUDGET / STAGE_BYTES > MAX_STAGES ? MAX_STAGES : int(RING_BUDGET / STAGE_BYTES);
     static constexpr uint32_t BAR_BYTES = 2 * STAGES * 8;
-    static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;   // + align slack
+    // ring | staging | barriers, + align slack
+    static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;
     static_assert(STAGES >= 2, "at least two pipeline stages");
-    static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+    static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget");
     static_assert(A_BYTES % 1024 == 0 && B_TILE % 1024 == 0, "swizzle-128B tiles must stay 1024-byte aligned");
 };
 
@@ -65,11 +75,13 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     return v;
 }
 
-// SPLIT: split-fp16 output (GemmEpi::split_off) -- every fp16 pair is written twice, hi at column n and lo at
-// split_off + n.  A compile-time switch keeps the plain epilogue free of it.
+// SPLIT: split-fp16 output (GemmEpi::split_off) -- every fp16 pair is written twice, hi at column n (tmD) and lo at
+// split_off + n (tmD2).  A compile-time switch keeps the plain epilogue free of it.
+// tmD / tmD2: the output as dims (N, M), row pitch ldo, 64-row x 128-byte boxes; TMA clips every store at N and M.
 template <int BN, int NSPLIT, bool SPLIT>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmEpi ep,
+gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2, const GemmEpi ep,
                 const int M, const int N, const __grid_constant__ ConvGeom cg) {
     using Cfg = GemmCfg<BN, NSPLIT>;
     constexpr int STAGES = Cfg::STAGES;
@@ -77,7 +89,8 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;
     uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint8_t* sD = smem + STAGES * Cfg::STAGE_BYTES;      // staging: [warpgroup][buffer] subtiles, 1024-byte aligned
+    uint64_t* full = reinterpret_cast<uint64_t*>(sD + STAGING_BYTES);
     uint64_t* empty = full + STAGES;
 
     const int warp = threadIdx.x >> 5;
@@ -91,6 +104,8 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
+        tma_prefetch_desc(&tmD);
+        if (SPLIT) tma_prefetch_desc(&tmD2);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full[i], 1);                  // the producer's arrive.expect_tx
             mbar_init(&empty[i], CONSUMER_WARPS);    // one arrive per consumer warp
@@ -133,6 +148,29 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     float acc[R];
     int stage = 0;
     uint32_t phase = 0;
+    // Staging: two buffers per warpgroup.  Row r of a subtile is 128 bytes at r * 128 with its 16-byte chunk c at
+    // position c ^ (r % 8) (CU_TENSOR_MAP_SWIZZLE_128B).  A thread's rows are wq * 16 + lane / 4 + 8h, so r % 8 = lane / 4.
+    // Thread 0 of the warpgroup issues the stores and waits for them.
+    const bool issuer = (threadIdx.x & 127) == 0;
+    uint32_t buf = 0;                            // plain output: subtiles alternate between the buffers, across tiles too
+    auto wg_sync = [&] {                         // literal ids: ptxas counts only the barriers used
+        if (wg == 0) named_bar_sync(1, 128);
+        else named_bar_sync(2, 128);
+    };
+    // Hand the subtile just written to buffer `buf` to the TMA unit.  Before the barrier the issuer waits until the
+    // store issued before it has read its buffer, so once the barrier is passed the other buffer may be refilled.
+    auto store_subtile = [&](int col, int row) {
+        fence_proxy_async();                     // this thread's shared-memory writes -> visible to the async proxy
+        if (issuer) bulk_wait_read<0>();
+        wg_sync();
+        if (issuer) {
+            const uint8_t* src = sD + (wg * 2 + buf) * STG_BYTES;
+            if (ep.accumulate) tma_reduce_add_2d(&tmD, src, col, row);   // one add per element: deterministic
+            else tma_store_2d(&tmD, src, col, row);
+            bulk_commit();
+        }
+        buf ^= 1;
+    };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
         int prev = -1;
@@ -164,25 +202,26 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[prev]);
 
-        // ------------------------------------------------------------ epilogue from registers
-        // accumulator register 4j + 2h + e: row (lane / 4) + 8h of this warp's 16, column 8j + 2 (lane % 4) + e
+        // ------------------------------------------------------------ epilogue through shared memory
+        // accumulator register 4j + 2h + e: row (lane / 4) + 8h of this warp's 16, column 8j + 2 (lane % 4) + e.
+        bool keep[2] = {true, true};   // rows outside the valid conv region become the next layer's zero padding
+        if (cg.mask) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int m = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
-            if (m >= M) continue;
-            bool keep = true;     // rows outside the valid conv region become the next layer's zero padding
-            if (cg.mask) {
-                const int mm = m - cg.row0;
+            for (int h = 0; h < 2; ++h) {
+                const int mm = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h - cg.row0;
                 const int w = mm % cg.Wp, r1 = mm / cg.Wp;
                 const int hh = r1 % cg.Hp, r2 = r1 / cg.Hp;
                 const int tt = r2 % cg.Tp;
-                keep = (mm >= 0) && (w >= cg.w0) && (w < cg.w1) && (hh >= cg.h0) && (hh < cg.h1) && (tt >= cg.t0) && (tt < cg.t1);
+                keep[h] = (mm >= 0) && (w >= cg.w0) && (w < cg.w1) && (hh >= cg.h0) && (hh < cg.h1) && (tt >= cg.t0) && (tt < cg.t1);
             }
-            char* orow = static_cast<char*>(ep.out) + int64_t(m) * ep.ldo * (ep.out_f32 ? 4 : 2);
+        }
+        // scale / bias / activation / row mask of accumulator column group j, in place; columns at or past N are left
+        // as they are (TMA clips them)
+        auto finish = [&](int j) {
+            const int n = n0 + 8 * j + 2 * (lane & 3);
+            if (n >= N) return;                  // N % 8 == 0: n < N implies n + 1 < N
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int n = n0 + 8 * j + 2 * (lane & 3);
-                if (n >= N) continue;            // N % 8 == 0: n < N implies n + 1 < N
+            for (int h = 0; h < 2; ++h) {
                 float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
                 if (ep.scale) {
                     const float2 s = __ldg(reinterpret_cast<const float2*>(ep.scale + n));
@@ -193,22 +232,78 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     v0 += b.x; v1 += b.y;
                 }
                 if (ep.act != VF_ACT_NONE) { v0 = apply_act(v0, ep.act); v1 = apply_act(v1, ep.act); }
-                if (!keep) { v0 = 0.f; v1 = 0.f; }
-                if (ep.out_f32) {
-                    float* p = reinterpret_cast<float*>(orow) + n;
-                    if (ep.accumulate) atomicAdd(reinterpret_cast<float2*>(p), make_float2(v0, v1));   // one add per element: deterministic
-                    else *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
+                if (!keep[h]) { v0 = 0.f; v1 = 0.f; }
+                acc[4 * j + 2 * h] = v0;
+                acc[4 * j + 2 * h + 1] = v1;
+            }
+        };
+        // Subtiles of 128-byte rows, left to right; those wholly at or past N are skipped.
+        const int row = m0 + wg * EPI_ROWS;
+        const uint32_t stg = smem_u32(sD) + wg * 2 * STG_BYTES + (wq * 16 + (lane >> 2)) * 128;
+        const int swz = lane >> 2;
+        if (!SPLIT && ep.out_f32) {              // (run_gemm refuses a split fp32 output)
+#pragma unroll
+            for (int s = 0; s < BN / 32; ++s) {  // 32 columns: j = 4s .. 4s + 3
+                if (n0 + 32 * s >= N) break;
+                const uint32_t d = stg + buf * STG_BYTES;
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const int j = 4 * s + c;
+                    finish(j);
+                    const int chunk = 2 * c + ((lane & 3) >> 1);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                        st_shared_v2_f32(d + h * 8 * 128 + ((chunk ^ swz) << 4) + 8 * (lane & 1), acc[4 * j + 2 * h],
+                                         acc[4 * j + 2 * h + 1]);
+                }
+                store_subtile(n0 + 32 * s, row);
+            }
+        } else {
+#pragma unroll
+            for (int s = 0; s < BN / 64; ++s) {  // 64 columns: j = 8s .. 8s + 7
+                if (n0 + 64 * s >= N) break;
+                if (SPLIT) {
+                    // hi into buffer 0, lo = fp16(v - hi) into buffer 1, in one pass: finish the values first, then
+                    // wait until both stores of the previous subtile have read their buffers
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) finish(8 * s + c);
+                    if (issuer) bulk_wait_read<0>();
+                    wg_sync();
+#pragma unroll
+                    for (int c = 0; c < 8; ++c)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int j = 8 * s + c;
+                            const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                            const __half2 hi = __floats2half2_rn(v0, v1);
+                            const uint32_t off = h * 8 * 128 + ((c ^ swz) << 4) + 4 * (lane & 3);
+                            st_shared_b32(stg + off, *reinterpret_cast<const uint32_t*>(&hi));
+                            st_shared_b32(stg + STG_BYTES + off, pack_half2(v0 - __low2float(hi), v1 - __high2float(hi)));
+                        }
+                    fence_proxy_async();
+                    wg_sync();
+                    if (issuer) {
+                        tma_store_2d(&tmD, sD + wg * 2 * STG_BYTES, n0 + 64 * s, row);
+                        tma_store_2d(&tmD2, sD + (wg * 2 + 1) * STG_BYTES, n0 + 64 * s, row);
+                        bulk_commit();
+                    }
                 } else {
-                    __half* p = reinterpret_cast<__half*>(orow) + n;
-                    const __half2 hi = __floats2half2_rn(v0, v1);
-                    *reinterpret_cast<__half2*>(p) = hi;
-                    if (SPLIT)
-                        *reinterpret_cast<__half2*>(p + ep.split_off) =
-                            __floats2half2_rn(v0 - __low2float(hi), v1 - __high2float(hi));
+                    const uint32_t d = stg + buf * STG_BYTES;
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) {
+                        const int j = 8 * s + c;
+                        finish(j);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            st_shared_b32(d + h * 8 * 128 + ((c ^ swz) << 4) + 4 * (lane & 3),
+                                          pack_half2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+                    }
+                    store_subtile(n0 + 64 * s, row);
                 }
             }
         }
     }
+    if (issuer) bulk_wait<0>();                  // the last stores have landed before the CTA exits
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -228,8 +323,8 @@ EncodeTiledFn get_encode_tiled() {
 }
 
 template <int BN, int NSPLIT, bool SPLIT = false>
-int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmEpi& ep, int M, int N, const ConvGeom& cg,
-                cudaStream_t stream) {
+int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmD2,
+                const GemmEpi& ep, int M, int N, const ConvGeom& cg, cudaStream_t stream) {
     using Cfg = GemmCfg<BN, NSPLIT>;
     // one handle per thread, but several threads (one per handle) may reach the same instantiation at once: the attribute
     // call is idempotent, the flag that remembers it is an atomic (acquire / release), so there is no data race
@@ -244,7 +339,7 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmEpi& e
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
     const int sms = device_sm_count();
     const int grid = tiles < sms ? tiles : sms;
-    gemm_f16_kernel<BN, NSPLIT, SPLIT><<<grid, THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, ep, M, N, cg);
+    gemm_f16_kernel<BN, NSPLIT, SPLIT><<<grid, THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, ep, M, N, cg);
     VF_CUDA(cudaGetLastError());
     return VF_OK;
 }
@@ -291,30 +386,31 @@ struct GemmProf {
 };
 static thread_local GemmProf g_prof;
 
-static int run_gemm_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, int bn, const GemmEpi& ep, int M, int N,
-                           const ConvGeom& cg, cudaStream_t stream) {
+static int run_gemm_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
+                           const CUtensorMap& tmD2, int bn, const GemmEpi& ep, int M, int N, const ConvGeom& cg,
+                           cudaStream_t stream) {
     if (ep.split_off > 0 && !ep.out_f32) {
         if (cg.nsplit == 2) {
-            if (bn == 256) return launch_gemm<256, 2, true>(tmA, tmB, ep, M, N, cg, stream);
-            if (bn == 192) return launch_gemm<192, 2, true>(tmA, tmB, ep, M, N, cg, stream);
-            if (bn == 128) return launch_gemm<128, 2, true>(tmA, tmB, ep, M, N, cg, stream);
-            return launch_gemm<64, 2, true>(tmA, tmB, ep, M, N, cg, stream);
+            if (bn == 256) return launch_gemm<256, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            if (bn == 192) return launch_gemm<192, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            if (bn == 128) return launch_gemm<128, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            return launch_gemm<64, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
         }
-        if (bn == 256) return launch_gemm<256, 1, true>(tmA, tmB, ep, M, N, cg, stream);
-        if (bn == 192) return launch_gemm<192, 1, true>(tmA, tmB, ep, M, N, cg, stream);
-        if (bn == 128) return launch_gemm<128, 1, true>(tmA, tmB, ep, M, N, cg, stream);
-        return launch_gemm<64, 1, true>(tmA, tmB, ep, M, N, cg, stream);
+        if (bn == 256) return launch_gemm<256, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 192) return launch_gemm<192, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 128) return launch_gemm<128, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        return launch_gemm<64, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
     }
     if (cg.nsplit == 2) {
-        if (bn == 256) return launch_gemm<256, 2>(tmA, tmB, ep, M, N, cg, stream);
-        if (bn == 192) return launch_gemm<192, 2>(tmA, tmB, ep, M, N, cg, stream);
-        if (bn == 128) return launch_gemm<128, 2>(tmA, tmB, ep, M, N, cg, stream);
-        return launch_gemm<64, 2>(tmA, tmB, ep, M, N, cg, stream);
+        if (bn == 256) return launch_gemm<256, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 192) return launch_gemm<192, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 128) return launch_gemm<128, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        return launch_gemm<64, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
     }
-    if (bn == 256) return launch_gemm<256, 1>(tmA, tmB, ep, M, N, cg, stream);
-    if (bn == 192) return launch_gemm<192, 1>(tmA, tmB, ep, M, N, cg, stream);
-    if (bn == 128) return launch_gemm<128, 1>(tmA, tmB, ep, M, N, cg, stream);
-    return launch_gemm<64, 1>(tmA, tmB, ep, M, N, cg, stream);
+    if (bn == 256) return launch_gemm<256, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    if (bn == 192) return launch_gemm<192, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    if (bn == 128) return launch_gemm<128, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    return launch_gemm<64, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
 }
 
 static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Ktot, int M, int N, const ConvGeom& cg,
@@ -326,18 +422,25 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
     if (ep.out_f32 ? (ep.ldo % 4) : (ep.ldo % 8)) return fail(VF_ERR_INVALID, "gemm: ldo breaks 16-byte rows");
     if (ep.split_off && (ep.out_f32 || ep.split_off < N || ep.split_off % 8))
         return fail(VF_ERR_INVALID, "gemm: split output needs fp16 out and split_off >= N, multiple of 8");
-    // tile width: the candidate that pads N least, the widest on a tie
-    int bn = 64;
-    if (N > 64) {
-        int best = 0x7fffffff;
-        for (int cand : {256, 192, 128}) {
-            const int padded = (N + cand - 1) / cand * cand;
-            if (padded < best) { best = padded; bn = cand; }
-        }
+    // Tile width: the one whose busiest SM computes the fewest columns, i.e. rounds of tiles over the SMs x width.  This
+    // counts both the padding of N and the idle SMs of a last partial wave; the widest wins a tie.
+    const int64_t num_m = (M + BM - 1) / BM, sms = device_sm_count();
+    int bn = 256;
+    int64_t best = INT64_MAX;
+    for (int cand : {256, 192, 128, 64}) {
+        const int64_t cost = (num_m * ((N + cand - 1) / cand) + sms - 1) / sms * cand;
+        if (cost < best) { best = cost; bn = cand; }
     }
-    CUtensorMap tmB;
+    CUtensorMap tmB, tmD, tmD2;
     VF_TRY(make_tmap_2d(&tmB, B, 2, uint64_t(N), uint64_t(Ktot), uint64_t(ldb) * 2, uint32_t(bn), BK));
-    if (!g_prof.on) return run_gemm_launch(tmA, tmB, bn, ep, M, N, cg, stream);
+    const int eb = ep.out_f32 ? 4 : 2;
+    VF_TRY(make_tmap_2d(&tmD, ep.out, eb, uint64_t(M), uint64_t(N), uint64_t(ep.ldo) * eb, EPI_ROWS, 128 / eb));
+    if (ep.split_off)
+        VF_TRY(make_tmap_2d(&tmD2, static_cast<__half*>(ep.out) + ep.split_off, eb, uint64_t(M), uint64_t(N),
+                            uint64_t(ep.ldo) * eb, EPI_ROWS, 128 / eb));
+    else
+        tmD2 = tmD;
+    if (!g_prof.on) return run_gemm_launch(tmA, tmB, tmD, tmD2, bn, ep, M, N, cg, stream);
     if (g_prof.used + 2 > g_prof.ev.size())
         for (int i = 0; i < 2; ++i) {
             cudaEvent_t e;
@@ -345,7 +448,7 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
             g_prof.ev.push_back(e);
         }
     VF_CUDA(cudaEventRecord(g_prof.ev[g_prof.used], stream));
-    const int st = run_gemm_launch(tmA, tmB, bn, ep, M, N, cg, stream);
+    const int st = run_gemm_launch(tmA, tmB, tmD, tmD2, bn, ep, M, N, cg, stream);
     VF_CUDA(cudaEventRecord(g_prof.ev[g_prof.used + 1], stream));
     g_prof.used += 2;
     double kexec = double(Ktot);

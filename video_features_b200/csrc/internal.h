@@ -43,7 +43,7 @@ struct GemmEpi {
     int act;                // VF_ACT_*
     int split_off;          // fp16 out only: > 0 writes the result as a split-fp16 pair, hi at column n and
                             // lo = fp16(v - hi) at column split_off + n of the same row (0: plain fp16)
-    int accumulate;         // fp32 out only: 1 = out += result (fp32x2 global reductions from the epilogue; every element
+    int accumulate;         // fp32 out only: 1 = out += result (fp32 TMA reduce-adds from the epilogue; every element
                             // is added exactly once, so the sum is deterministic) -- the residual-stream update of the ViT blocks
 };
 int gemm_f16(const __half* A, int lda, const __half* B, int ldb, int M, int N, int K, const GemmEpi& ep,
