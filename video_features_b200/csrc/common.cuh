@@ -105,6 +105,20 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// count this thread towards named barrier `id` without waiting for it (the waiting side uses named_bar_sync)
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// Register reallocation between warpgroups (sm_90a): every warp of a warpgroup executes the same one.  dec hands
+// registers back to the CTA's pool; inc waits until the pool holds the ones it asks for.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // Shared-memory matrix descriptor for a K-major operand tile whose rows are 128 bytes (64 x 16-bit) laid out by TMA

@@ -3,16 +3,19 @@
 //   D[M,N] = act( A[M,K] . B[N,K]^T * scale[n] + bias[n] )     A, B fp16 K-major; fp32 accumulate in registers;
 //                                                              D fp16 or fp32
 //
-// A CTA owns a 128 x BN output tile at a time (tiles are strided over a grid of at most one CTA per SM).  Three
-// warpgroups:
-//   warpgroup 0    TMA producer (one lane): A and B tiles through a 128B-swizzled ring of STAGES stages, one mbarrier
-//                  pair (full / empty) per stage.  It runs ahead into the next tile while the consumers store this one.
-//   warpgroups 1,2 consumers: rows 0..63 and 64..127 of the tile.  Per 64-wide K block, four wgmma m64nBNk16 (eight with
-//                  split weights), one commit group; the stage is released as soon as the group behind it has retired.
-//                  Epilogue: scale / bias / activation and row mask in registers, then 64-row x 128-byte subtiles
+// Tiles are 64 x BN, walked row-major (n fastest) and strided over a grid of at most one CTA per SM.  Three warpgroups
+// in a "ping-pong" schedule:
+//   warpgroup 0    TMA producer (one lane, 40 registers): A and B tiles of the CTA's tiles, in order, through a
+//                  128B-swizzled ring of STAGES stages, one mbarrier pair (full / empty) per stage.
+//   warpgroups 1,2 consumers (232 registers each), one whole tile at a time: warpgroup 1 the CTA's even tiles, 2 its odd
+//                  ones.  Per 64-wide K block, four wgmma m64nBNk16 (eight with split weights), one commit group; the
+//                  stage is released as soon as the group behind it has retired.  A named-barrier pair makes the two
+//                  main loops take turns, so one warpgroup's epilogue runs while the other's MMAs keep the tensor cores
+//                  busy.  Epilogue: scale / bias / activation and row mask in registers, then 64-row x 128-byte subtiles
 //                  through two swizzled shared-memory buffers per warpgroup, each handed to a TMA store (TMA reduce-add
-//                  for `accumulate`) that TMA clips at N and M.  The consumers go on to the next tile's main loop while
-//                  the stores drain.
+//                  for `accumulate`) that TMA clips at N and M.
+// The shifted-row conv mode keeps the cooperative schedule instead (template parameter PP = false): 128 x BN tiles walked
+// m-fastest, warpgroups 1 and 2 on rows 0..63 and 64..127 of the same tile, with the same main loop and epilogue.
 //
 // Used for every dense contraction of the hot path: ViT patch-embed / QKV / out-proj / FFN GEMMs (reference:
 // third-party clip `VisionTransformer.forward`, called at models/CLIP/extract_clip.py:128) and the I3D / RAFT
@@ -32,23 +35,26 @@ namespace vf {
 
 namespace {
 
-constexpr int BM = 128;          // rows per CTA tile (64 per consumer warpgroup)
 constexpr int BK = 64;           // 64 fp16 = one 128-byte swizzle row
 constexpr int THREADS = 384;     // producer warpgroup + two consumer warpgroups
-constexpr int CONSUMER_WARPS = 8;
+// 40 x 128 + 232 x 256 <= 64 K registers; a CTA of 384 threads starts at 168 each
+constexpr uint32_t PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr int EPI_ROWS = 64;                   // output rows per consumer warpgroup = rows of one TMA store box
 constexpr uint32_t STG_BYTES = EPI_ROWS * 128; // one staging subtile: 64 rows x 128 bytes (64 fp16 / 32 fp32 columns)
 constexpr uint32_t STAGING_BYTES = 2 * 2 * STG_BYTES;   // two warpgroups x two buffers
 constexpr uint32_t SMEM_LIMIT = 227 * 1024;    // opt-in dynamic shared memory per block on sm_90
 constexpr uint32_t MAX_STAGES = 8;
 // operand ring = what is left after the staging buffers, the barriers of MAX_STAGES stages and the alignment slack:
-// 194 KB, i.e. stages (plain / split weights) 4 / 2 at BN = 256, 4 / 3 at 192, 6 / 4 at 128, 8 / 6 at 64.
+// 194 KB, i.e. stages (plain / split weights) 4 / 2 at BN = 256, 6 / 3 at 192, 8 / 4 at 128, 8 / 8 at 64.
 constexpr uint32_t RING_BUDGET = SMEM_LIMIT - STAGING_BYTES - 2 * MAX_STAGES * 8 - 1024;
 
 // NSPLIT = 2: the B stage holds the hi and the lo tile of a split-fp16 weight matrix and every K step issues two
 // MMAs against the same A tile.
-template <int BN, int NSPLIT>
+// PP: ping-pong schedule, 64-row tiles each owned by one consumer warpgroup (plain GEMMs); otherwise the cooperative
+// schedule, 128-row tiles whose rows 0..63 / 64..127 the two warpgroups share (conv mode, see run_gemm).
+template <int BN, int NSPLIT, bool PP>
 struct GemmCfg {
+    static constexpr int BM = PP ? 64 : 128;
     static constexpr uint32_t A_BYTES = BM * BK * 2;
     static constexpr uint32_t B_TILE = BN * BK * 2;           // one of hi / lo
     static constexpr uint32_t B_BYTES = NSPLIT * B_TILE;
@@ -61,6 +67,11 @@ struct GemmCfg {
     static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory budget");
     static_assert(A_BYTES % 1024 == 0 && B_TILE % 1024 == 0, "swizzle-128B tiles must stay 1024-byte aligned");
 };
+
+// Schedule by entry point, from measurements on an H100 (DESIGN.md 4.1): plain GEMMs (the CLIP tower, RAFT's
+// correlation) run ping-pong; the conv mode (I3D, RAFT, ResNet, R(2+1)D) keeps the cooperative 128-row tile, whose
+// weight tile serves twice the rows -- ping-pong made those networks 13-31 % slower.
+constexpr int tile_rows(bool pp) { return pp ? GemmCfg<64, 1, true>::BM : GemmCfg<64, 1, false>::BM; }
 
 __device__ __forceinline__ float apply_act(float v, int act) {
     if (act == VF_ACT_QUICKGELU) {
@@ -78,13 +89,14 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 // SPLIT: split-fp16 output (GemmEpi::split_off) -- every fp16 pair is written twice, hi at column n (tmD) and lo at
 // split_off + n (tmD2).  A compile-time switch keeps the plain epilogue free of it.
 // tmD / tmD2: the output as dims (N, M), row pitch ldo, 64-row x 128-byte boxes; TMA clips every store at N and M.
-template <int BN, int NSPLIT, bool SPLIT>
+template <int BN, int NSPLIT, bool SPLIT, bool PP>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2, const GemmEpi ep,
                 const int M, const int N, const __grid_constant__ ConvGeom cg) {
-    using Cfg = GemmCfg<BN, NSPLIT>;
+    using Cfg = GemmCfg<BN, NSPLIT, PP>;
     constexpr int STAGES = Cfg::STAGES;
+    constexpr int BM = Cfg::BM;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sA = smem;
@@ -98,6 +110,11 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const int num_m = (M + BM - 1) / BM;
     const int num_n = (N + BN - 1) / BN;
     const int num_tiles = num_m * num_n;
+    // ping-pong: row-major (the column tiles of one A row block run together); cooperative: m fastest
+    auto tile_m0 = [&](int tile) { return (PP ? tile / num_n : tile % num_m) * BM; };
+    auto tile_n0 = [&](int tile) { return (PP ? tile % num_n : tile / num_m) * BN; };
+    // this CTA's tiles: blockIdx.x + i * gridDim.x for i < cta_tiles (the grid is at most num_tiles, so cta_tiles >= 1)
+    const int cta_tiles = (num_tiles - 1 - int(blockIdx.x)) / int(gridDim.x) + 1;
     const int kpt = (cg.k_per_tap + BK - 1) / BK;    // K blocks per filter tap (a plain GEMM is one "tap")
     const int num_k = cg.ntaps * kpt;
 
@@ -108,7 +125,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (SPLIT) tma_prefetch_desc(&tmD2);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full[i], 1);                  // the producer's arrive.expect_tx
-            mbar_init(&empty[i], CONSUMER_WARPS);    // one arrive per consumer warp
+            mbar_init(&empty[i], PP ? 4 : 8);        // one arrive per consumer warp that reads the stage
         }
         fence_mbar_init();
     }
@@ -116,11 +133,13 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
     if (warp < 4) {
         // ------------------------------------------------------------ TMA producer
+        setmaxnreg_dec<PRODUCER_REGS>();             // the whole warpgroup, before warps 1..3 leave
         if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
+            for (int i = 0; i < cta_tiles; ++i) {
+                const int tile = blockIdx.x + i * gridDim.x;
+                const int m0 = tile_m0(tile), n0 = tile_n0(tile);
                 for (int tap = 0; tap < cg.ntaps; ++tap) {
                     const int arow = m0 + cg.tap_off[tap];       // may be negative / past the end: TMA zero-fills
                     const int bcol = tap * cg.k_per_tap;
@@ -142,12 +161,11 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     }
 
     // ---------------------------------------------------------------- consumers
-    const int wg = (warp >> 2) - 1;              // 0: tile rows 0..63, 1: rows 64..127
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = (warp >> 2) - 1;              // ping-pong: 0 the CTA's even tiles, 1 its odd ones; else rows 0 / 64
     const int wq = warp & 3;                     // warp inside the warpgroup: 16 rows each
     constexpr int R = BN / 2;                    // accumulator registers per thread
     float acc[R];
-    int stage = 0;
-    uint32_t phase = 0;
     // Staging: two buffers per warpgroup.  Row r of a subtile is 128 bytes at r * 128 with its 16-byte chunk c at
     // position c ^ (r % 8) (CU_TENSOR_MAP_SWIZZLE_128B).  A thread's rows are wq * 16 + lane / 4 + 8h, so r % 8 = lane / 4.
     // Thread 0 of the warpgroup issues the stores and waits for them.
@@ -171,12 +189,30 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
         buf ^= 1;
     };
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile % num_m) * BM, n0 = (tile / num_m) * BN;
+    // Main-loop turns: tile i > 0 starts its MMAs once the other warpgroup has issued every MMA of tile i - 1 (named
+    // barrier 3 + owner of tile i: the owner syncs, the other warpgroup arrives).  Besides overlapping one epilogue with
+    // the other main loop, this keeps a warpgroup from waiting on a `full` barrier more than one ring lap ahead of the
+    // loads, where its parity would be ambiguous.  Only a tile that exists is waited for or signalled.
+    auto wait_turn = [&] {
+        if (wg == 0) named_bar_sync(3, 256);
+        else named_bar_sync(4, 256);
+    };
+    auto pass_turn = [&] {
+        if (wg == 0) named_bar_arrive(4, 256);
+        else named_bar_arrive(3, 256);
+    };
+    for (int i = PP ? wg : 0; i < cta_tiles; i += PP ? 2 : 1) {
+        const int tile = blockIdx.x + i * gridDim.x;
+        const int m0 = tile_m0(tile) + (PP ? 0 : wg * 64), n0 = tile_n0(tile);   // this warpgroup's 64 rows
+        // the producer fills the ring with the CTA's tiles in order: tile i starts at K block i * num_k of the sequence
+        const uint64_t first = uint64_t(i) * uint64_t(num_k);
+        int stage = int(first % STAGES);
+        uint32_t phase = uint32_t(first / STAGES) & 1u;
+        if (PP && i > 0) wait_turn();
         int prev = -1;
         for (int kb = 0, kk = 0; kb < num_k; ++kb) {
             mbar_wait(&full[stage], phase);
-            const uint64_t adesc = wgmma_desc_sw128(sA + stage * Cfg::A_BYTES + wg * (64 * 128));
+            const uint64_t adesc = wgmma_desc_sw128(sA + stage * Cfg::A_BYTES + (PP ? 0 : wg * (64 * 128)));
             const uint64_t bdesc = wgmma_desc_sw128(sB + stage * Cfg::B_BYTES);
             const bool lo_blk = NSPLIT == 2 && ((cg.lo_mask >> kk) & 1ull);
             wgmma_fence_regs<R>(acc);
@@ -197,6 +233,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
             if (++kk == kpt) kk = 0;              // K block index inside the current tap
         }
+        if (PP && i + 1 < cta_tiles) pass_turn();
         wgmma_wait<0>();
         wgmma_fence_regs<R>(acc);
         __syncwarp();
@@ -208,7 +245,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (cg.mask) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int mm = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h - cg.row0;
+                const int mm = m0 + wq * 16 + (lane >> 2) + 8 * h - cg.row0;
                 const int w = mm % cg.Wp, r1 = mm / cg.Wp;
                 const int hh = r1 % cg.Hp, r2 = r1 / cg.Hp;
                 const int tt = r2 % cg.Tp;
@@ -238,7 +275,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             }
         };
         // Subtiles of 128-byte rows, left to right; those wholly at or past N are skipped.
-        const int row = m0 + wg * EPI_ROWS;
+        const int row = m0;
         const uint32_t stg = smem_u32(sD) + wg * 2 * STG_BYTES + (wq * 16 + (lane >> 2)) * 128;
         const int swz = lane >> 2;
         if (!SPLIT && ep.out_f32) {              // (run_gemm refuses a split fp32 output)
@@ -322,24 +359,24 @@ EncodeTiledFn get_encode_tiled() {
     return fn;
 }
 
-template <int BN, int NSPLIT, bool SPLIT = false>
+template <int BN, int NSPLIT, bool SPLIT, bool PP>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmD2,
                 const GemmEpi& ep, int M, int N, const ConvGeom& cg, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN, NSPLIT>;
+    using Cfg = GemmCfg<BN, NSPLIT, PP>;
     // one handle per thread, but several threads (one per handle) may reach the same instantiation at once: the attribute
     // call is idempotent, the flag that remembers it is an atomic (acquire / release), so there is no data race
     static std::atomic<bool> attr_set[64];
     int dev = 0;
     VF_CUDA(cudaGetDevice(&dev));
     if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-        VF_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BN, NSPLIT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        VF_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BN, NSPLIT, SPLIT, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      Cfg::SMEM_BYTES));
         if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
     }
-    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+    const int tiles = ((M + Cfg::BM - 1) / Cfg::BM) * ((N + BN - 1) / BN);
     const int sms = device_sm_count();
     const int grid = tiles < sms ? tiles : sms;
-    gemm_f16_kernel<BN, NSPLIT, SPLIT><<<grid, THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, ep, M, N, cg);
+    gemm_f16_kernel<BN, NSPLIT, SPLIT, PP><<<grid, THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, ep, M, N, cg);
     VF_CUDA(cudaGetLastError());
     return VF_OK;
 }
@@ -386,35 +423,37 @@ struct GemmProf {
 };
 static thread_local GemmProf g_prof;
 
+template <bool PP>
 static int run_gemm_launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmD,
                            const CUtensorMap& tmD2, int bn, const GemmEpi& ep, int M, int N, const ConvGeom& cg,
                            cudaStream_t stream) {
     if (ep.split_off > 0 && !ep.out_f32) {
         if (cg.nsplit == 2) {
-            if (bn == 256) return launch_gemm<256, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-            if (bn == 192) return launch_gemm<192, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-            if (bn == 128) return launch_gemm<128, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-            return launch_gemm<64, 2, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            if (bn == 256) return launch_gemm<256, 2, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            if (bn == 192) return launch_gemm<192, 2, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            if (bn == 128) return launch_gemm<128, 2, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            return launch_gemm<64, 2, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
         }
-        if (bn == 256) return launch_gemm<256, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-        if (bn == 192) return launch_gemm<192, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-        if (bn == 128) return launch_gemm<128, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-        return launch_gemm<64, 1, true>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 256) return launch_gemm<256, 1, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 192) return launch_gemm<192, 1, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 128) return launch_gemm<128, 1, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        return launch_gemm<64, 1, true, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
     }
     if (cg.nsplit == 2) {
-        if (bn == 256) return launch_gemm<256, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-        if (bn == 192) return launch_gemm<192, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-        if (bn == 128) return launch_gemm<128, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-        return launch_gemm<64, 2>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 256) return launch_gemm<256, 2, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 192) return launch_gemm<192, 2, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        if (bn == 128) return launch_gemm<128, 2, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        return launch_gemm<64, 2, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
     }
-    if (bn == 256) return launch_gemm<256, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-    if (bn == 192) return launch_gemm<192, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-    if (bn == 128) return launch_gemm<128, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
-    return launch_gemm<64, 1>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    if (bn == 256) return launch_gemm<256, 1, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    if (bn == 192) return launch_gemm<192, 1, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    if (bn == 128) return launch_gemm<128, 1, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+    return launch_gemm<64, 1, false, PP>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
 }
 
-static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Ktot, int M, int N, const ConvGeom& cg,
-                    const GemmEpi& ep, cudaStream_t stream) {
+// pp: the ping-pong schedule (64-row tiles, tmA boxes of 64 rows) or the cooperative one (128-row tiles, boxes of 128)
+static int run_gemm(const CUtensorMap& tmA, bool pp, const __half* B, int ldb, int64_t Ktot, int M, int N,
+                    const ConvGeom& cg, const GemmEpi& ep, cudaStream_t stream) {
     if (!ep.out) return fail(VF_ERR_INVALID, "gemm: null output");
     if (reinterpret_cast<uintptr_t>(ep.out) & 15) return fail(VF_ERR_INVALID, "gemm: output must be 16-byte aligned");
     if (ep.accumulate && !ep.out_f32) return fail(VF_ERR_INVALID, "gemm: accumulate needs fp32 output");
@@ -422,9 +461,11 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
     if (ep.out_f32 ? (ep.ldo % 4) : (ep.ldo % 8)) return fail(VF_ERR_INVALID, "gemm: ldo breaks 16-byte rows");
     if (ep.split_off && (ep.out_f32 || ep.split_off < N || ep.split_off % 8))
         return fail(VF_ERR_INVALID, "gemm: split output needs fp16 out and split_off >= N, multiple of 8");
-    // Tile width: the one whose busiest SM computes the fewest columns, i.e. rounds of tiles over the SMs x width.  This
-    // counts both the padding of N and the idle SMs of a last partial wave; the widest wins a tie.
-    const int64_t num_m = (M + BM - 1) / BM, sms = device_sm_count();
+    // Tile width: the one whose busiest SM computes the fewest columns, i.e. rounds of tiles (64 rows ping-pong, 128
+    // cooperative) over the SMs x width.  This counts both the padding of N and the idle SMs of a last partial wave; the
+    // widest wins a tie.
+    const int bm = tile_rows(pp);
+    const int64_t num_m = (M + bm - 1) / bm, sms = device_sm_count();
     int bn = 256;
     int64_t best = INT64_MAX;
     for (int cand : {256, 192, 128, 64}) {
@@ -440,7 +481,11 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
                             uint64_t(ep.ldo) * eb, EPI_ROWS, 128 / eb));
     else
         tmD2 = tmD;
-    if (!g_prof.on) return run_gemm_launch(tmA, tmB, tmD, tmD2, bn, ep, M, N, cg, stream);
+    auto launch = [&] {
+        return pp ? run_gemm_launch<true>(tmA, tmB, tmD, tmD2, bn, ep, M, N, cg, stream)
+                  : run_gemm_launch<false>(tmA, tmB, tmD, tmD2, bn, ep, M, N, cg, stream);
+    };
+    if (!g_prof.on) return launch();
     if (g_prof.used + 2 > g_prof.ev.size())
         for (int i = 0; i < 2; ++i) {
             cudaEvent_t e;
@@ -448,7 +493,7 @@ static int run_gemm(const CUtensorMap& tmA, const __half* B, int ldb, int64_t Kt
             g_prof.ev.push_back(e);
         }
     VF_CUDA(cudaEventRecord(g_prof.ev[g_prof.used], stream));
-    const int st = run_gemm_launch(tmA, tmB, tmD, tmD2, bn, ep, M, N, cg, stream);
+    const int st = launch();
     VF_CUDA(cudaEventRecord(g_prof.ev[g_prof.used + 1], stream));
     g_prof.used += 2;
     double kexec = double(Ktot);
@@ -493,8 +538,8 @@ int gemm_f16(const __half* A, int lda, const __half* B, int ldb, int M, int N, i
     cg.k_per_tap = K;
     cg.nsplit = 1;
     CUtensorMap tmA;
-    VF_TRY(make_tmap_2d(&tmA, A, 2, uint64_t(M), uint64_t(K), uint64_t(lda) * 2, BM, BK));
-    return run_gemm(tmA, B, ldb, K, M, N, cg, ep, stream);
+    VF_TRY(make_tmap_2d(&tmA, A, 2, uint64_t(M), uint64_t(K), uint64_t(lda) * 2, tile_rows(true), BK));
+    return run_gemm(tmA, true, B, ldb, K, M, N, cg, ep, stream);
 }
 
 int conv_gemm_f16(const __half* X, int C, int64_t P, const __half* Wt, int N, const ConvGeom& g, const GemmEpi& ep,
@@ -513,10 +558,10 @@ int conv_gemm_f16(const __half* X, int C, int64_t P, const __half* Wt, int N, co
         return fail(VF_ERR_INVALID, "conv_gemm: bad mask volume %dx%dx%d, row0 %d", g.Tp, g.Hp, g.Wp, g.row0);
     // overlapping-row view: row p = k_per_tap contiguous elements starting at element p*C
     CUtensorMap tmA;
-    VF_TRY(make_tmap_2d(&tmA, X, 2, uint64_t(P), uint64_t(g.k_per_tap), uint64_t(C) * 2, BM, BK));
+    VF_TRY(make_tmap_2d(&tmA, X, 2, uint64_t(P), uint64_t(g.k_per_tap), uint64_t(C) * 2, tile_rows(false), BK));
     const int64_t Ktot = int64_t(g.ntaps) * g.k_per_tap * g.nsplit;
     if (Ktot % 8) return fail(VF_ERR_INVALID, "conv_gemm: K must be a multiple of 8");
-    return run_gemm(tmA, Wt, int(Ktot), Ktot, int(P), N, g, ep, stream);
+    return run_gemm(tmA, false, Wt, int(Ktot), Ktot, int(P), N, g, ep, stream);
 }
 
 }  // namespace vf
