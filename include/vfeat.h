@@ -248,6 +248,12 @@ int vf_resnet_forward_u8(vf_resnet_t* h, const uint8_t* frames, int n, int Hr, i
  * 1 maxpool, 2..5 layer1..layer4.  dims4 receives (n, C, H, W); out == NULL only queries the shape. */
 int vf_resnet_read_stage(vf_resnet_t* h, int stage, float* out, int64_t capacity, int* dims4, void* stream);
 int64_t vf_resnet_launch_count(const vf_resnet_t* h);
+/* Diagnostics: conv `index` of the trunk as uploaded, in execution order (the stem, then per block conv1, conv2, conv3
+ * of a bottleneck, the downsample if any).  geom receives 15 ints: n_out, ntaps, k_per_tap, then (dt, dh, dw) of taps
+ * 0..3 (the row shift of tap j on a volume of Hp x Wp rows is (dt Hp + dh) Wp + dw); lo_mask its K blocks without a
+ * W_lo pass.  w (n_out x 2 ntaps k_per_tap fp16: W_hi | W_lo), scale and bias (n_out fp32, the folded BatchNorm) are
+ * DEVICE buffers filled when not NULL.  An index past the last conv is VF_ERR_INVALID. */
+int vf_resnet_conv(const vf_resnet_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
 /* ---- R(2+1)D-18 clip features: replaces torchvision `r2plus1d_18(pretrained=True)` with `fc = Identity()` in eval mode,
  * and its clip transform ToFloatTensorInZeroOne -> Resize((128, 171)) -> Normalize -> CenterCrop(112)
@@ -272,6 +278,10 @@ int vf_r21d_forward_u8(vf_r21d_t* h, const uint8_t* frames, int n_frames, int H,
  * conv), 1..4 layer1..layer4.  dims5 receives (n, C, T, H, W); out == NULL only queries the shape. */
 int vf_r21d_read_stage(vf_r21d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream);
 int64_t vf_r21d_launch_count(const vf_r21d_t* h);
+/* Diagnostics: conv `index` as uploaded, in execution order (the stem's spatial and temporal convs, then per block
+ * conv1's spatial and temporal convs, conv2's, the downsample if any); the rest as vf_resnet_conv.  n_out is the width
+ * padded to a multiple of 8. */
+int vf_r21d_conv(const vf_r21d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
 #ifdef __cplusplus
 }

@@ -32,8 +32,9 @@ def _q(x, mode):
     return x.float().double()
 
 
-def forward(sd, x, scheme):
-    """scheme: class -> 'fp16' | 'split'.  Float64 arithmetic with operands rounded per class."""
+def forward(sd, x, scheme, taps=False):
+    """scheme: class -> 'fp16' | 'split'.  Float64 arithmetic with operands rounded per class.  With ``taps`` also
+    {stage name: activation} under oracle/r21d_net.py's STAGES names."""
     W = {k: (_q(v, scheme["w"]) if k.endswith("weight") and v.dim() == 5 else v) for k, v in sd.items()}
 
     def bn(p, y):
@@ -49,6 +50,7 @@ def forward(sd, x, scheme):
 
     y = F.relu(bn("stem.1", conv(x, "stem.0.weight", "stem", stride=(1, 2, 2), padding=(0, 3, 3))))
     y = F.relu(bn("stem.4", conv(y, "stem.3.weight", "temp", padding=(1, 0, 0))))
+    st = {"stem": y}
     for L in range(4):
         for b in range(2):
             p, s = f"layer{L + 1}.{b}", (2 if (b == 0 and L > 0) else 1)
@@ -59,7 +61,9 @@ def forward(sd, x, scheme):
             else:
                 r = _q(y, scheme["resid"])
             y = F.relu(r + t)
-    return torch.flatten(F.adaptive_avg_pool3d(y, 1), 1)
+        st[f"layer{L + 1}"] = y
+    out = torch.flatten(F.adaptive_avg_pool3d(y, 1), 1)
+    return (out, st) if taps else out
 
 
 def errors(y, ref):

@@ -32,8 +32,9 @@ def _q(x, mode):
     return x.float().double()
 
 
-def forward(sd, x, depth, scheme):
-    """scheme: class -> 'fp16' | 'split'.  Float64 arithmetic with operands rounded per class."""
+def forward(sd, x, depth, scheme, taps=False):
+    """scheme: class -> 'fp16' | 'split'.  Float64 arithmetic with operands rounded per class.  With ``taps`` also
+    {stage name: activation} under oracle/resnet_net.py's STAGES names."""
     bottleneck, layers = resnet_net.LAYERS[depth]
     W = {k: (_q(v, scheme["w"]) if k.endswith("conv1.weight") or ".conv" in k or "downsample.0" in k else v)
          for k, v in sd.items()}
@@ -45,8 +46,11 @@ def forward(sd, x, depth, scheme):
     def conv(y, key, cls, **kw):
         return F.conv2d(_q(y, scheme[cls]), W[key], **kw)
 
+    st = {}
     y = F.relu(bn("bn1", conv(x, "conv1.weight", "stem", stride=2, padding=3)))
+    st["stem"] = y
     y = F.max_pool2d(y, 3, 2, 1)
+    st["maxpool"] = y
     for L, nb in enumerate(layers):
         for b in range(nb):
             p, s = f"layer{L + 1}.{b}", (2 if (b == 0 and L > 0) else 1)
@@ -62,7 +66,9 @@ def forward(sd, x, depth, scheme):
             else:
                 r = _q(y, scheme["resid"])
             y = F.relu(r + t)
-    return torch.flatten(F.adaptive_avg_pool2d(y, 1), 1)
+        st[f"layer{L + 1}"] = y
+    out = torch.flatten(F.adaptive_avg_pool2d(y, 1), 1)
+    return (out, st) if taps else out
 
 
 def errors(y, ref):

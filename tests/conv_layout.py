@@ -5,7 +5,8 @@ Activations are channels-last rows of a zero-bordered volume [n][Tp][Hp][Wp], `p
 A_j[p] = X.flat[(p + tap_off[j]) * pitch : ... + k_per_tap], zero where p + tap_off[j] lies outside [0, P).
 
 volume() builds X from an NC(T)HW tensor, merged_filter() / unmerged_filter() build Wt, tap_off and lo_mask the way the
-I3D and RAFT engines do, and emulate() computes in float64 what the kernel computes.  Test infrastructure only."""
+I3D and RAFT engines do, gathered_volume() / engine_filter() the repacks and filters of the ResNet and R(2+1)D engines,
+and emulate() computes in float64 what the kernel computes.  Test infrastructure only."""
 from __future__ import annotations
 
 from dataclasses import dataclass
@@ -225,8 +226,9 @@ def emulate(X: torch.Tensor, pitch: int, vol: Vol, f: dict, bias=None, scale=Non
     if f["nsplit"] == 2:
         keep_lo = torch.ones(Kb, dtype=torch.float64, device=X.device)
         if lo_mask:
-            blk = torch.arange(Kb, device=X.device) % kpt // 64
-            keep_lo = ((f["lo_mask"] >> blk.cpu()) & 1 == 0).double().to(X.device)
+            # per K block in Python integers: bit 63 of a 64-block tap does not fit a signed int64 tensor
+            skip = torch.tensor([float((f["lo_mask"] >> kk) & 1) for kk in range((kpt + 63) // 64)])
+            keep_lo = (1.0 - skip[torch.arange(Kb) % kpt // 64]).double().to(X.device)
         W = Wt[:, :Kb] + Wt[:, Kb:] * keep_lo
     y = torch.zeros(P, Wt.shape[0], dtype=torch.float64, device=X.device)
     cols = torch.arange(kpt, device=X.device)
@@ -241,16 +243,20 @@ def emulate(X: torch.Tensor, pitch: int, vol: Vol, f: dict, bias=None, scale=Non
     return y
 
 
-def reference_conv(x_eff: torch.Tensor, w_eff: torch.Tensor, bias=None, scale=None, act: int = ACT_NONE):
-    """F.conv3d / F.conv2d in float64, stride 1, zero padding k // 2 before and k - 1 - k // 2 after (the output keeps
-    the input's extent), then the epilogue.  Returns NCTHW (or NCHW for 2-D input) with channels last moved to dim 1."""
+def reference_conv(x_eff: torch.Tensor, w_eff: torch.Tensor, bias=None, scale=None, act: int = ACT_NONE, stride=1,
+                   padding=None):
+    """F.conv3d / F.conv2d in float64, then the epilogue.  Without `padding`: stride 1, zero padding k // 2 before and
+    k - 1 - k // 2 after (the output keeps the input's extent); with it: F.conv's own `stride` and symmetric `padding`.
+    Returns NCTHW (or NCHW for 2-D input) with channels last moved to dim 1."""
     x, w = x_eff.double(), w_eff.double()
-    ks = w.shape[2:]
-    pad = []
-    for k in reversed(ks):
-        pad += [k // 2, k - 1 - k // 2]
-    xp = F.pad(x, pad)
-    y = F.conv3d(xp, w) if w.dim() == 5 else F.conv2d(xp, w)
+    conv = F.conv3d if w.dim() == 5 else F.conv2d
+    if padding is not None:
+        y = conv(x, w, stride=stride, padding=padding)
+    else:
+        pad = []
+        for k in reversed(w.shape[2:]):
+            pad += [k // 2, k - 1 - k // 2]
+        y = conv(F.pad(x, pad), w)
     shape = [1, -1] + [1] * (y.dim() - 2)
     if scale is not None:
         y = y * scale.double().view(shape)
@@ -324,6 +330,8 @@ def build_case(case: dict, nsplit: int, seed: int, n_out: int | None = None) -> 
     """Seeded operands of one case: X, the filter (merged_filter / unmerged_filter), bias, scale, and the float64
     operands x_eff / w_eff as the kernel sees them.  n_out < N keeps only the first output channels (the layout does
     not depend on them)."""
+    if case["layout"] in ENGINE_FILTERS:
+        return build_engine_case(case, nsplit, seed, n_out)
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(*case["x"], generator=g) * 0.5
     ci = case["x"][1]
@@ -341,3 +349,226 @@ def build_case(case: dict, nsplit: int, seed: int, n_out: int | None = None) -> 
     else:
         f = unmerged_filter(w, vol, kpt, chan=case.get("chan"), chan_lo=case.get("chan_lo"), nsplit=nsplit)
     return dict(X=X, pitch=pitch, vol=vol, f=f, bias=bias, scale=scale, act=case["act"], x_eff=x_eff, w_eff=f["w_eff"])
+
+
+# ----------------------------------------------------------------- the ResNet and R(2+1)D layouts (csrc/resnet.cu, r21d.cu)
+# Every activation is a split pair row [hi C | lo C]; every filter a hi + lo pair over both halves (nsplit = 2).  The
+# strided convs read repacks of their input, restated here by gathered_volume():
+#   2-D phase repack (raft_phase_repack): phase row (qh, qw) holds x[2(qh - q0) + ph][2(qw - q0) + pw] for the 4 phases
+#     (ph, pw), each a [hi C | lo C] run at column (2 ph + pw) * 2C; q0 = 1 (rows of a border-1 volume), q0 = 2 for the
+#     stems' phase volumes (rows [16 hi | 16 lo], phase p's 3 channels at 4p .. 4p + 2, column 4p + 3 unused);
+#   temporal phase repack (r21d_temporal_phase): frame row q holds [x[2(q - 1)] | x[2(q - 1) + 1]], each a pair run;
+#   (2,2,2) subsample (r21d_subsample): row (t, h, w) holds x[2(t - 1)][2(h - 1)][2(w - 1)].
+# ENGINE_FILTERS mirror the prep_* builders of resnet.cu / r21d.cu: (ntaps, k_per_tap, tap shifts (dt, dh, dw),
+# K column of the hi half of channel c at filter position (kt, kh, kw), column offset of its lo half).
+
+def pad8(c: int) -> int:
+    return (c + 7) // 8 * 8
+
+
+def _idx(n_pos: int, size: int, f) -> torch.Tensor:
+    """Source index f(q) of each volume position q, or `size` (a zero slice) outside [0, size)."""
+    i = torch.tensor([f(q) for q in range(n_pos)])
+    return torch.where((i >= 0) & (i < size), i, size)
+
+
+def gathered_volume(x: torch.Tensor, shape, placements, lo_off: int, pitch: int, chan_pad: int | None = None,
+                    tail_rows: int = 0, junk: float = 1.0, generator: torch.Generator | None = None):
+    """x [n, C, T, H, W] (or [n, C, H, W]) -> (X fp16 [rows + tail_rows, pitch], x_eff float64 hi + lo of x).
+
+    Position (b, t, h, w) of the [n][Tp][Hp][Wp] volume `shape` holds, per placement (col, ft, fh, fw), the split pair
+    of x[b, :, ft(t), fh(h), fw(w)] (zero where an index falls outside x): hi of channel c at column col + c, lo at
+    col + lo_off + c.  The pad channels C .. chan_pad of a padded width hold zeros, as the engines write them; columns
+    no channel maps to hold uniform values in [-junk, junk], and so do the tail rows."""
+    x5 = _as5d(x).double()
+    n, C, T, H, W = x5.shape
+    Tp, Hp, Wp = shape
+    X = torch.empty(n * Tp * Hp * Wp + tail_rows, pitch, dtype=torch.float64).uniform_(-junk, junk, generator=generator)
+    body = X[:n * Tp * Hp * Wp].view(n, Tp, Hp, Wp, pitch)
+    hi, lo = split_f16(x5)
+    hp, lp = F.pad(hi.double(), (0, 1, 0, 1, 0, 1)), F.pad(lo.double(), (0, 1, 0, 1, 0, 1))
+    width = chan_pad or C
+    for col, ft, fh, fw in placements:
+        it, ih, iw = _idx(Tp, T, ft), _idx(Hp, H, fh), _idx(Wp, W, fw)
+        for src, off in ((hp, col), (lp, col + lo_off)):
+            v = src[:, :, it][:, :, :, ih][:, :, :, :, iw].permute(0, 2, 3, 4, 1)
+            body[..., off:off + width] = 0.0
+            body[..., off:off + C] = v
+    return X.half(), (hi.double() + lo.double()) if x.dim() == 5 else (hi.double() + lo.double()).squeeze(2)
+
+
+def _stride2_col(kpt, cpp):
+    def col(kt, kh, kw, c):
+        a, ph, b, pw = (kh + 1) // 2, (kh + 1) % 2, (kw + 1) // 2, (kw + 1) % 2
+        return (a * 2 + b) * kpt + (ph * 2 + pw) * cpp + c
+    return col
+
+
+def _stem_col(kt, kh, kw, c):
+    a, ph, b, pw = (kh + 1) // 2, (kh + 1) % 2, (kw + 1) // 2, (kw + 1) % 2
+    return a * 128 + b * 32 + (ph * 2 + pw) * 4 + c
+
+
+ENGINE_FILTERS = {
+    # prep_same / prep_spatial: k kernel rows, each a run of k * 2ci_p; k = 1 is also the stride-2 downsample, which
+    # reads phase (0, 0), the first 2ci columns of a phase row
+    "same": lambda k, ci, ci_p: (k, 2 * k * ci_p, [(0, a - k // 2, -(k // 2)) for a in range(k)],
+                                 lambda kt, kh, kw, c: kh * 2 * k * ci_p + kw * 2 * ci_p + c, ci_p),
+    # prep_stride2 / prep_spatial2: tap (a, b) reads phase row (q + a - 1, q' + b - 1); kh = 2a + ph - 1
+    "stride2": lambda k, ci, ci_p: (4, 8 * ci, [(0, t // 2 - 1, t % 2 - 1) for t in range(4)],
+                                    _stride2_col(8 * ci, 2 * ci), ci),
+    # prep_stem (both engines): 4 taps of kernel row pairs, each 4 phase positions x 32 columns
+    "stem": lambda k, ci, ci_p: (4, 128, [(0, a - 2, -2) for a in range(4)], _stem_col, 16),
+    # prep_temporal: 3 taps one frame apart
+    "temporal": lambda k, ci, ci_p: (3, 2 * ci_p, [(a - 1, 0, 0) for a in range(3)],
+                                     lambda kt, kh, kw, c: kt * 2 * ci_p + c, ci_p),
+    # prep_temporal2: frame 2t - 1 from the odd half of row t - 1, frames 2t and 2t + 1 from row t
+    "temporal2": lambda k, ci, ci_p: (2, 4 * ci_p, [(-1, 0, 0), (0, 0, 0)],
+                                      lambda kt, kh, kw, c: 2 * ci_p + c if kt == 0 else 4 * ci_p + (kt - 1) * 2 * ci_p + c,
+                                      ci_p),
+    # prep_point: 1x1x1 over the subsampled block input
+    "point": lambda k, ci, ci_p: (1, 2 * ci, [(0, 0, 0)], lambda kt, kh, kw, c: c, ci),
+}
+
+
+def engine_filter(kind: str, w: torch.Tensor, vol: Vol, ci_p: int | None = None, n_out: int | None = None,
+                  nsplit: int = 2):
+    """The filter of one engine conv: Wt (fp16 [n_out, nsplit * ntaps * k_per_tap], rows past co zero), tap_off,
+    lo_mask (bit kk: K block kk of every tap meets only lo halves; a tap of exactly 64 blocks keeps bit 63), w_eff
+    (float64, hi or hi + lo, zero filters for the pad rows up to n_out)."""
+    w5 = _as5d(w)
+    co, ci, kt, kh, kw = w5.shape
+    ntaps, kpt, shifts, col, lo_off = ENGINE_FILTERS[kind](kh, ci, ci_p or ci)
+    n_out = n_out or co
+
+    def cols(a, b, d):
+        k = [col(a, b, d, c) for c in range(ci)]
+        return [(k, [j + lo_off for j in k])]
+
+    Wt, lo_mask, w_eff = _finish(cols, w5, n_out, ntaps, kpt, nsplit)
+    w_eff = torch.cat([w_eff, w_eff.new_zeros(n_out - co, *w_eff.shape[1:])])
+    return dict(Wt=Wt, ntaps=ntaps, k_per_tap=kpt, shifts=shifts, tap_off=[_tap_shift(vol, *s) for s in shifts],
+                lo_mask=lo_mask, nsplit=nsplit, w_eff=w_eff if w.dim() == 5 else w_eff.squeeze(2))
+
+
+def _geometry(case):
+    """(volume shape, Vol of the output, placements, lo_off, pitch, chan_pad) of a case: the output volume and the
+    rows the conv reads on it."""
+    n, C, T, H, W = case["x"] if len(case["x"]) == 5 else (case["x"][0], case["x"][1], 1) + tuple(case["x"][2:])
+    src, Cp = case["src"], case.get("ci_p", C)
+    b, tb = case["border"], case.get("t_border", 0)      # spatial / temporal border before the valid region
+    if src == "rows":                   # the activation itself, [hi Cp | lo Cp]
+        Tp, Hp, Wp = T + 2 * tb, H + b + 1, W + b + 1
+        pl = [(0, lambda t: t - tb, lambda h: h - b, lambda w: w - b)]
+        lo_off, pitch = Cp, 2 * Cp
+        valid = (tb, tb + T, b, b + H, b, b + W)
+    elif src in ("phase", "stem_phase"):
+        q0 = 2 if src == "stem_phase" else 1
+        S = H // 2
+        Tp, Hp, Wp = T + 2 * tb, S + q0 + 1, S + q0 + 1
+        cpp = 4 if src == "stem_phase" else 2 * C
+        pl = [((2 * ph + pw) * cpp, lambda t: t - tb, lambda q, ph=ph: 2 * (q - q0) + ph,
+               lambda q, pw=pw: 2 * (q - q0) + pw) for ph in (0, 1) for pw in (0, 1)]
+        lo_off, pitch = (16, 32) if src == "stem_phase" else (C, 8 * C)
+        valid = (tb, tb + T, q0, q0 + S, q0, q0 + S)
+    elif src == "temporal_phase":       # on the output's frames (T' = (T - 1) // 2 + 1), spatial border 1
+        To = (T - 1) // 2 + 1
+        Tp, Hp, Wp = To + 2, H + 2, W + 2
+        pl = [(p * 2 * Cp, lambda q, p=p: 2 * (q - 1) + p, lambda h: h - 1, lambda w: w - 1) for p in (0, 1)]
+        lo_off, pitch = Cp, 4 * Cp
+        valid = (1, To + 1, 1, H + 1, 1, W + 1)
+    else:                               # "subsample": (2,2,2) subsample of the block input on the output volume
+        To, S = (T - 1) // 2 + 1, H // 2
+        Tp, Hp, Wp = To + 2, S + 2, S + 2
+        pl = [(0, lambda q: 2 * (q - 1), lambda h: 2 * (h - 1), lambda w: 2 * (w - 1))]
+        lo_off, pitch = C, 2 * C
+        valid = (1, To + 1, 1, S + 1, 1, S + 1)
+    return (Tp, Hp, Wp), Vol(n, Tp, Hp, Wp, *valid), pl, lo_off, pitch, (Cp if Cp != C else None)
+
+
+def build_engine_case(case: dict, nsplit: int, seed: int, n_out: int | None = None) -> dict:
+    """build_case() for the ResNet / R(2+1)D layouts.  N is the padded width; pad output channels have zero filters,
+    scale and bias, as the engines upload them.  `conv` holds F.conv's stride and padding for reference_conv."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(*case["x"], generator=g) * 0.5
+    ci = case["x"][1]
+    co = case.get("co", case["N"]) if n_out is None else min(n_out, case.get("co", case["N"]))
+    N = case["N"] if n_out is None else n_out
+    k = case["k"]
+    w = torch.randn(co, ci, *k, generator=g) * (ci * float(torch.tensor(k).prod())) ** -0.5
+    bias = torch.zeros(N)
+    scale = torch.zeros(N)
+    bias[:co] = torch.randn(co, generator=g) * 0.1
+    scale[:co] = 1 + 0.1 * torch.randn(co, generator=g)
+    shape, vol, pl, lo_off, pitch, chan_pad = _geometry(case)
+    f = engine_filter(case["layout"], w, vol, ci_p=case.get("ci_p"), n_out=N, nsplit=nsplit)
+    tail = max(0, -(-(f["k_per_tap"] - pitch) // pitch))
+    X, x_eff = gathered_volume(x, shape, pl, lo_off, pitch, chan_pad=chan_pad, tail_rows=tail, generator=g)
+    return dict(X=X, pitch=pitch, vol=vol, f=f, bias=bias, scale=scale, act=case["act"], x_eff=x_eff, w_eff=f["w_eff"],
+                conv=case["conv"], co=co)
+
+
+def _res(id, layout, x, k, N, src, border, conv, act=ACT_RELU):
+    return dict(id=id, layout=layout, x=x, k=k, N=N, src=src, border=border, conv=conv, act=act, out="split",
+                c_off=0, ctot=N, row0=0)
+
+
+def _r21(id, layout, x, k, N, src, conv, co=None, ci_p=None, border=1, act=ACT_RELU):
+    c = dict(id=id, layout=layout, x=x, k=k, N=N, src=src, border=border, t_border=1, conv=conv, act=act, out="split",
+             c_off=0, ctot=N, row0=0)
+    if co is not None:
+        c["co"] = co
+    if ci_p is not None:
+        c["ci_p"] = ci_p
+    return c
+
+
+S2 = dict(stride=2, padding=1)
+RESNET_CASES = [
+    # stem 7x7/2 pad 3 on the transform's phase volume: [n][115][115] rows of 32, 4 taps x 128
+    _res("resnet-stem-115", "stem", (2, 3, 224, 224), (7, 7), 64, "stem_phase", 0, dict(stride=2, padding=3)),
+    # stride-1 3x3 at 58^2 (layer1, basic block): 3 taps of 3 x 128
+    _res("resnet-3x3-c64-58", "same", (2, 64, 56, 56), (3, 3), 64, "rows", 1, dict(stride=1, padding=1), ACT_NONE),
+    # stride-2 3x3 on the phase repack: layer2.0 conv1 of a basic block (58^2 -> 30^2), 4 taps of 8 x 64
+    _res("resnet-3x3s2-c64-30", "stride2", (2, 64, 56, 56), (3, 3), 128, "phase", 1, S2),
+    # layer3.0 conv2 of a bottleneck (width 256, 30^2 -> 16^2)
+    _res("resnet-3x3s2-c256-16", "stride2", (1, 256, 28, 28), (3, 3), 256, "phase", 1, S2),
+    # layer4.0 conv2 of a bottleneck at width 512 (16^2 -> 9^2): k_per_tap 4096 = 64 K blocks, lo_mask bit 63 set
+    _res("resnet-3x3s2-c512-9", "stride2", (2, 512, 14, 14), (3, 3), 512, "phase", 1, S2),
+    # stride-2 1x1 downsample: phase (0, 0) of the same repack, the first 2C of an 8C row
+    _res("resnet-down-c64-30", "same", (2, 64, 56, 56), (1, 1), 128, "phase", 1, dict(stride=2, padding=0), ACT_NONE),
+    # ResNet-50 layer4.0 downsample: 2048 columns of an 8192-element phase row
+    _res("resnet-down-c1024-9", "same", (2, 1024, 14, 14), (1, 1), 2048, "phase", 1, dict(stride=2, padding=0),
+         ACT_NONE),
+    # layer4 conv1 1x1 at cin 2048: 64 K blocks, the lo half in blocks 32 .. 63
+    _res("resnet-1x1-c2048-9", "same", (2, 2048, 7, 7), (1, 1), 512, "rows", 1, dict(stride=1, padding=0)),
+]
+
+R21D_CASES = [
+    # stem (1,7,7)/(1,2,2) on the per-frame phase volume [T+2][59][59], 45 outputs padded to 48
+    _r21("r21d-stem-59-T5", "stem", (1, 3, 5, 112, 112), (1, 7, 7), 48, "stem_phase", dict(stride=(1, 2, 2),
+         padding=(0, 3, 3)), co=45),
+    # the stem's temporal conv 45 -> 64 over 48-wide pair rows: K 96, the lo half from column 48 inside block 0
+    _r21("r21d-temporal-c45-59-T5", "temporal", (1, 45, 5, 56, 56), (3, 1, 1), 64, "rows",
+         dict(stride=1, padding=(1, 0, 0)), ci_p=48, border=2),
+    # layer2.0 conv1 spatial stride (1,2,2) on the phase repack of every frame: 64 -> 230 (232)
+    _r21("r21d-spatial2-c64-30-T5", "stride2", (1, 64, 5, 56, 56), (1, 3, 3), 232, "phase",
+         dict(stride=(1, 2, 2), padding=(0, 1, 1)), co=230),
+    # layer2.0 conv1 temporal stride (2,1,1) on the temporal phase repack: 230 (232) -> 128, K 928 (a 32-column tail)
+    _r21("r21d-temporal2-c230-30-T5", "temporal2", (1, 230, 5, 28, 28), (3, 1, 1), 128, "temporal_phase",
+         dict(stride=(2, 1, 1), padding=(1, 0, 0)), ci_p=232),
+    # layer2.0 downsample: 1x1x1 over the (2,2,2) subsample of the block input
+    _r21("r21d-down-c64-30-T5", "point", (1, 64, 5, 56, 56), (1, 1, 1), 128, "subsample", dict(stride=2, padding=0),
+         act=ACT_NONE),
+    # layer3 conv2 spatial 256 -> 460 (464) at 16^2
+    _r21("r21d-spatial-c256-16-T3", "same", (2, 256, 3, 14, 14), (1, 3, 3), 464, "rows",
+         dict(stride=1, padding=(0, 1, 1)), co=460),
+    # layer4.0 conv1 spatial stride (1,2,2): 256 -> 921 (928) at 9^2, k_per_tap 2048
+    _r21("r21d-spatial2-c256-9-T3", "stride2", (1, 256, 3, 14, 14), (1, 3, 3), 928, "phase",
+         dict(stride=(1, 2, 2), padding=(0, 1, 1)), co=921),
+    # layer4 conv2 temporal 921 (928) -> 512 at 9^2, T' = 1 (a 32-column tail of a 1856-column tap)
+    _r21("r21d-temporal-c921-9-T1", "temporal", (2, 921, 1, 7, 7), (3, 1, 1), 512, "rows",
+         dict(stride=1, padding=(1, 0, 0)), ci_p=928, act=ACT_NONE),
+]
+
+ENGINE_CASES = RESNET_CASES + R21D_CASES

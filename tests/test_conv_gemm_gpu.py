@@ -77,7 +77,8 @@ def launch(d, dev, out, N, ldd, c_off=0, split_off=0, region=True, lo_mask=None,
 def reference(d, dev):
     """float64 [P, N]: the valid rows from F.conv3d / F.conv2d (on the GPU, in float64), zeros elsewhere."""
     vol = d["vol"]
-    ref = cl.reference_conv(d["x_eff"].to(dev), d["w_eff"].to(dev), d["bias"].to(dev), d["scale"].to(dev), d["act"])
+    ref = cl.reference_conv(d["x_eff"].to(dev), d["w_eff"].to(dev), d["bias"].to(dev), d["scale"].to(dev), d["act"],
+                            **d.get("conv", {}))
     if ref.dim() == 4:
         ref = ref.unsqueeze(2)
     full = torch.zeros(vol.P, ref.shape[1], dtype=torch.float64, device=dev)
@@ -121,6 +122,7 @@ def _output_of(case):
 
 
 def run_and_check(case, nsplit, dev, seed=11):
+    """Returns the output buffers of the launches: fp32 always, fp16 and split when the case's output has them."""
     d = cl.build_case(case, nsplit, seed=seed)
     N, P = case["N"], d["vol"].P
     ref, keep = reference(d, dev)
@@ -133,7 +135,7 @@ def run_and_check(case, nsplit, dev, seed=11):
     assert bool((y32[~keep] == 0).all()), "rows outside the valid region must be written as 0.0"
     assert bool((D32[P:] == SENT32).all()) and bool((D32[:, N:] == SENT32).all())
     if case["out"] == "f32":
-        return
+        return dict(f32=D32)
     # fp16 out: the rounding of the fp32 result above
     D16 = launch(d, dev, "f16", N, N + 8)
     y16 = D16[:P, :N]
@@ -141,7 +143,7 @@ def run_and_check(case, nsplit, dev, seed=11):
     check_f16(y16, ref, f"{case['id']} nsplit={nsplit} fp16")
     assert bool((D16[P:] == SENT16).all()) and bool((D16[:, N:] == SENT16).all())
     if case["out"] != "split":
-        return
+        return dict(f32=D32, f16=D16)
     # split out into a channel slice of a wider concat row: columns outside both halves stay untouched
     ctot, so = o["split_off"], o["split_off"]
     Ds = launch(d, dev, "split", N, o["ldd"], c_off=c0, split_off=so)
@@ -153,6 +155,7 @@ def run_and_check(case, nsplit, dev, seed=11):
     untouched[c0:c0 + N] = False
     untouched[so + c0:so + c0 + N] = False
     assert bool((Ds[:P, untouched.to(dev)] == SENT16).all()) and bool((Ds[P:] == SENT16).all())
+    return dict(f32=D32, f16=D16, split=Ds)
 
 
 @pytest.mark.parametrize("nsplit", [1, 2])

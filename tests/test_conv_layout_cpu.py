@@ -8,11 +8,11 @@ import conv_layout as cl
 N_CPU = 8     # output channels kept here: the layout does not depend on them
 
 
-def _check(case, nsplit, mask=True):
-    d = cl.build_case(case, nsplit, seed=3, n_out=N_CPU)
+def _check(case, nsplit, mask=True, n_out=N_CPU):
+    d = cl.build_case(case, nsplit, seed=3, n_out=n_out)
     vol, f = d["vol"], d["f"]
     y = cl.emulate(d["X"], d["pitch"], vol, f, d["bias"], d["scale"], d["act"], mask=mask, lo_mask=False)
-    ref = cl.reference_conv(d["x_eff"], d["w_eff"], d["bias"], d["scale"], d["act"])
+    ref = cl.reference_conv(d["x_eff"], d["w_eff"], d["bias"], d["scale"], d["act"], **d.get("conv", {}))
     if ref.dim() == 4:
         ref = ref.unsqueeze(2)
     got = vol.valid_rows(y)
@@ -33,6 +33,36 @@ def test_emulator_equals_float64_convolution(case, nsplit):
     assert bool((y[~keep] == 0).all()) and int(keep.sum()) == vol.n * (vol.t1 - vol.t0) * (vol.h1 - vol.h0) * (vol.w1 - vol.w0)
     assert f["ntaps"] <= 64 and f["k_per_tap"] % 8 == 0 and case["pitch"] % 8 == 0
     assert f["Wt"].shape == (N_CPU, nsplit * f["ntaps"] * f["k_per_tap"])
+
+
+@pytest.mark.parametrize("case", cl.ENGINE_CASES, ids=[c["id"] for c in cl.ENGINE_CASES])
+def test_engine_layouts_equal_strided_float64_convolution(case):
+    """The ResNet / R(2+1)D repacks and filters (phase, temporal phase, subsample, stems, padded widths) against
+    F.conv2d / F.conv3d with the real strides and padding, at every output channel: pad channels come out exactly 0."""
+    y, vol, f = _check(case, 2, n_out=None)
+    N, co = case["N"], case.get("co", case["N"])
+    assert f["Wt"].shape == (N, 2 * f["ntaps"] * f["k_per_tap"]) and f["ntaps"] <= 64 and f["k_per_tap"] % 8 == 0
+    assert bool((y[:, co:] == 0).all()) and bool((y[~vol.keep()] == 0).all())
+
+
+def test_engine_lo_masks():
+    """The restated lo_mask builder against masks derived by hand from the layouts, including bit 63 of the 64-block
+    taps.  (The engines' own upload_conv masks are compared with this builder, conv by conv, on the GPU:
+    test_conv_gemm_resnet_r21d_gpu.py.)"""
+    m = {c["id"]: cl.build_case(c, 2, seed=0, n_out=8)["f"]["lo_mask"] for c in cl.ENGINE_CASES}
+    # layer4 1x1 at cin 2048: [hi 2048 | lo 2048], blocks 32 .. 63 lo only
+    assert m["resnet-1x1-c2048-9"] == ((1 << 64) - 1) ^ ((1 << 32) - 1)
+    # stride-2 3x3 at width 512: 4 phases of [hi 512 | lo 512], the lo blocks 16p + 8 .. 16p + 15
+    assert m["resnet-3x3s2-c512-9"] == sum(((1 << 8) - 1) << (16 * p + 8) for p in range(4))
+    assert m["resnet-3x3s2-c512-9"] >> 63 == 1
+    # the stems: every K block holds hi columns
+    assert m["resnet-stem-115"] == 0 and m["r21d-stem-59-T5"] == 0
+    # 48-wide pair rows of 45 channels: block 0 holds hi 0..44 and lo 48..63, block 1 only lo
+    assert m["r21d-temporal-c45-59-T5"] == 0b10
+    # temporal phase rows [even | odd] of 232-wide pairs: hi at 0..229 and 464..693 (tap 1), 464..693 (tap 0)
+    assert m["r21d-temporal2-c230-30-T5"] == sum(1 << b for b in (4, 5, 6, 11, 12, 13, 14))
+    # the downsample reads 2C columns of an 8C phase row: hi blocks 0..15, lo 16..31
+    assert m["resnet-down-c1024-9"] == ((1 << 32) - 1) ^ ((1 << 16) - 1)
 
 
 def test_lo_mask_matches_the_engines():

@@ -112,6 +112,8 @@ SIGNATURES = {
     "vf_resnet_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_resnet_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
     "vf_resnet_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_resnet_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
+                                 C.c_void_p, C.c_void_p]),
     "vf_r21d_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
     "vf_r21d_destroy": (C.c_int, [C.c_void_p]),
     "vf_r21d_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -119,6 +121,8 @@ SIGNATURES = {
                                      C.c_int, C.c_void_p, C.c_void_p]),
     "vf_r21d_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
     "vf_r21d_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_r21d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
+                               C.c_void_p, C.c_void_p]),
     "vf_clip_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "vf_clip_profile_categories": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
     "vf_clip_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
@@ -148,3 +152,20 @@ def lib() -> C.CDLL:
 def check(status: int) -> None:
     if status != VF_OK:
         raise VfError(status, lib().vf_last_error().decode("utf-8", "replace"))
+
+
+def read_conv(fn, handle, index: int, device):
+    """Diagnostics shared by ResNetEngine.conv / R21DEngine.conv: fn is vf_resnet_conv or vf_r21d_conv.  Returns dict
+    n_out, ntaps, k_per_tap, shifts [(dt, dh, dw)] per tap, lo_mask, w (fp16 [n_out, 2 ntaps k_per_tap], W_hi | W_lo),
+    scale, bias (fp32 [n_out]) as uploaded."""
+    import torch
+    geom = (C.c_int * 15)()
+    mask = C.c_uint64()
+    check(fn(handle, index, geom, C.byref(mask), None, None, None))
+    n_out, ntaps, kpt = geom[0], geom[1], geom[2]
+    w = torch.empty((n_out, 2 * ntaps * kpt), dtype=torch.float16, device=device)
+    scale = torch.empty(n_out, dtype=torch.float32, device=device)
+    bias = torch.empty(n_out, dtype=torch.float32, device=device)
+    check(fn(handle, index, geom, C.byref(mask), w.data_ptr(), scale.data_ptr(), bias.data_ptr()))
+    shifts = [tuple(geom[3 + 3 * j:6 + 3 * j]) for j in range(ntaps)]
+    return dict(n_out=n_out, ntaps=ntaps, k_per_tap=kpt, shifts=shifts, lo_mask=mask.value, w=w, scale=scale, bias=bias)

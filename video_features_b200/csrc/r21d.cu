@@ -532,4 +532,29 @@ int vf_r21d_read_stage(vf_r21d_t* h, int stage, float* out, int64_t capacity, in
 
 int64_t vf_r21d_launch_count(const vf_r21d_t* h) { return h ? h->launches : 0; }
 
+int vf_r21d_conv(const vf_r21d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias) {
+    if (!h || !geom || !lo_mask) return fail(VF_ERR_INVALID, "r21d_conv: null argument");
+    std::vector<const R21Conv*> cs{&h->stem_s, &h->stem_t};
+    for (const R21Block& B : h->blocks) {
+        for (const R21Conv* c : {&B.c1s, &B.c1t, &B.c2s, &B.c2t}) cs.push_back(c);
+        if (B.down) cs.push_back(&B.dn);
+    }
+    if (index < 0 || index >= int(cs.size()))
+        return fail(VF_ERR_INVALID, "r21d_conv: index %d outside the %d convs", index, int(cs.size()));
+    const R21Conv& c = *cs[index];
+    geom[0] = c.n_out; geom[1] = c.ntaps; geom[2] = c.k_per_tap;
+    for (int j = 0; j < 4; ++j) {
+        geom[3 + 3 * j] = c.tap_kind ? c.dt[j] : 0;
+        geom[4 + 3 * j] = c.tap_kind ? 0 : c.dh[j];
+        geom[5 + 3 * j] = c.tap_kind ? 0 : c.dw[j];
+    }
+    *lo_mask = c.lo_mask;
+    VF_CUDA(cudaSetDevice(h->device));
+    const size_t nw = size_t(c.n_out) * 2 * c.ntaps * c.k_per_tap;
+    if (w) VF_CUDA(cudaMemcpy(w, c.w, nw * sizeof(__half), cudaMemcpyDeviceToDevice));
+    if (scale) VF_CUDA(cudaMemcpy(scale, c.scale, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
+    if (bias) VF_CUDA(cudaMemcpy(bias, c.bias, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
+    return VF_OK;
+}
+
 }  // extern "C"

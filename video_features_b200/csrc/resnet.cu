@@ -471,4 +471,27 @@ int vf_resnet_read_stage(vf_resnet_t* h, int stage, float* out, int64_t capacity
 
 int64_t vf_resnet_launch_count(const vf_resnet_t* h) { return h ? h->launches : 0; }
 
+int vf_resnet_conv(const vf_resnet_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias) {
+    if (!h || !geom || !lo_mask) return fail(VF_ERR_INVALID, "resnet_conv: null argument");
+    std::vector<const ResConv*> cs{&h->stem};
+    for (const ResBlock& B : h->blocks) {
+        cs.push_back(&B.c1);
+        cs.push_back(&B.c2);
+        if (h->bottleneck) cs.push_back(&B.c3);
+        if (B.down) cs.push_back(&B.dn);
+    }
+    if (index < 0 || index >= int(cs.size()))
+        return fail(VF_ERR_INVALID, "resnet_conv: index %d outside the %d convs", index, int(cs.size()));
+    const ResConv& c = *cs[index];
+    geom[0] = c.n_out; geom[1] = c.ntaps; geom[2] = c.k_per_tap;
+    for (int j = 0; j < 4; ++j) { geom[3 + 3 * j] = 0; geom[4 + 3 * j] = c.dh[j]; geom[5 + 3 * j] = c.dw[j]; }
+    *lo_mask = c.lo_mask;
+    VF_CUDA(cudaSetDevice(h->device));
+    const size_t nw = size_t(c.n_out) * 2 * c.ntaps * c.k_per_tap;
+    if (w) VF_CUDA(cudaMemcpy(w, c.w, nw * sizeof(__half), cudaMemcpyDeviceToDevice));
+    if (scale) VF_CUDA(cudaMemcpy(scale, c.scale, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
+    if (bias) VF_CUDA(cudaMemcpy(bias, c.bias, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
+    return VF_OK;
+}
+
 }  // extern "C"

@@ -8,7 +8,7 @@ from typing import Dict, Sequence
 import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib
+from ._lib import NamedTensor, check, lib, read_conv
 
 OUT_DIM = 512
 
@@ -79,6 +79,11 @@ class R21DEngine:
             check(lib().vf_r21d_read_stage(self._h, stage, out.data_ptr(), out.numel(), dims,
                                            torch.cuda.current_stream().cuda_stream))
         return out
+
+    def conv(self, index: int) -> dict:
+        """Diagnostics: conv ``index`` as uploaded, in execution order (include/vfeat.h vf_r21d_conv); see _lib.read_conv."""
+        with torch.cuda.device(self.device):
+            return read_conv(lib().vf_r21d_conv, self._h, index, self.device)
 
     @property
     def launch_count(self) -> int:

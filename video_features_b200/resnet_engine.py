@@ -8,7 +8,7 @@ from typing import Dict
 import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib
+from ._lib import NamedTensor, check, lib, read_conv
 
 DEPTHS = (18, 34, 50, 101, 152)
 
@@ -76,6 +76,11 @@ class ResNetEngine:
             check(lib().vf_resnet_read_stage(self._h, stage, out.data_ptr(), out.numel(), dims,
                                              torch.cuda.current_stream().cuda_stream))
         return out
+
+    def conv(self, index: int) -> dict:
+        """Diagnostics: conv ``index`` as uploaded, in execution order (include/vfeat.h vf_resnet_conv); see _lib.read_conv."""
+        with torch.cuda.device(self.device):
+            return read_conv(lib().vf_resnet_conv, self._h, index, self.device)
 
     @property
     def launch_count(self) -> int:
