@@ -196,10 +196,17 @@ int vf_i3d_forward_u8_strided(vf_i3d_t* h, const uint8_t* frames, int n, int T, 
 /* flow stream with the T3 transform fused (extract_i3d.py:67-73): flow n x T x 2 x H x W fp32 on the device (the RAFT
  * output, still padded) -> crop 224 -> clamp(+-20) -> 128+255/40 f -> round -> 2x/255-1 -> I3D. */
 int vf_i3d_forward_flow(vf_i3d_t* h, const float* flow, int n, int T, int H, int W, float* out, void* stream);
-/* Diagnostics: copy a retained internal activation (0: conv3d_1a, 1: conv3d_2c, 3: mixed_5b, 4: mixed_5c) of the
- * last forward to fp32 NCTHW; dims5 receives (n, C, T, H, W); out == NULL only queries the shape. */
+/* Diagnostics: copy a retained internal activation (0: conv3d_1a, 1: conv3d_2c, 2: mixed_3c, 3: mixed_4f, 4: mixed_5c)
+ * of the last forward (of its last chunk of max_stacks clips) to fp32 NCTHW; dims5 receives (n, C, T, H, W); out == NULL
+ * only queries the shape. */
 int vf_i3d_read_stage(vf_i3d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream);
 int64_t vf_i3d_launch_count(const vf_i3d_t* h);
+/* Diagnostics: unit `index` (0 .. VF_I3D_UNITS - 1, the order of vf_i3d_weights) as uploaded.  geom receives 196 ints:
+ * n_out, ntaps, k_per_tap, nsplit (2: W_hi | W_lo along K, 1: single fp16 weights), then (dt, dh, dw) of taps 0..63 (the
+ * row shift of tap j on a volume of Tp x Hp x Wp rows is (dt Hp + dh) Wp + dw); lo_mask its K blocks without a W_lo
+ * pass.  w (n_out x nsplit ntaps k_per_tap fp16), scale and bias (n_out fp32, the folded BatchNorm) are DEVICE buffers
+ * filled when not NULL.  An index past the last unit is VF_ERR_INVALID. */
+int vf_i3d_conv(const vf_i3d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
 /* ---- RAFT optical flow: replaces `RAFT()(image1, image2, iters=20, test_mode=True)` + InputPadder
  * (models/raft/raft_src/raft.py:27-44,115-174; called at models/raft/extract_raft.py:94-104 and
@@ -228,6 +235,11 @@ int vf_raft_padded_size(int Hs, int Ws, int* H, int* W);
  * 5 the correlation pyramid rows (n, H8*W8, 1, row pitch): level l at cumulative offset of the level sizes. */
 int vf_raft_debug_read(vf_raft_t* h, int what, float* out, int64_t capacity, int* dims4, void* stream);
 int64_t vf_raft_launch_count(const vf_raft_t* h);
+/* Diagnostics: conv `index` as uploaded, as vf_i3d_conv (dt is 0).  Order: per encoder (fnet, then cnet) conv1,
+ * layer1's four convs, layer2's conv1, downsample, three convs, the same for layer3, conv2 (16 each); then the update
+ * block's convc1, convc2, convf1, convf2, conv, the stacked convz1|convr1, convq1, convz2|convr2, convq2, the flow head's
+ * conv1, conv2 and the mask head's mask.0, mask.2 (45 in all).  n_out is the GEMM width (padded rows included). */
+int vf_raft_conv(const vf_raft_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
 /* ---- ResNet-18/34/50/101/152 frame features: replaces torchvision `models.resnetXX(pretrained=True)` with
  * `fc = Identity()` in eval mode, and its per-frame transform Resize(256) -> CenterCrop(224) -> ToTensor -> Normalize

@@ -75,8 +75,26 @@ def _same_pad(k, s):
     return top, pad_along - top
 
 
-def _unit(sd, name, x, k, stride=1):
+def _fp16(t: torch.Tensor) -> torch.Tensor:
+    return t.half().to(t.dtype)
+
+
+# The operands the engine keeps as single fp16 (every other GEMM operand is a split-fp16 pair, every other weight hi +
+# lo; i3d.cu): the stem input, the inputs of conv3d_2c and of every Mixed branch_1.1 / branch_2.1 (the 1x1x1 reducers'
+# outputs), and the weights of the units in DECLARED_FP16_UNITS (indices into unit_names(): the stem and the 3x3x3
+# convs of mixed_3b / 3c; prepare_unit's `chosen`, none of them with VF_I3D_SINGLE=none).
+DECLARED_FP16_UNITS = (0, 5, 7, 11, 13)
+_FP16_INPUT = ("conv3d_1a_7x7", "conv3d_2c_3x3") + tuple(f"{m}.branch_{b}.1" for m in MIXED for b in (1, 2))
+
+
+def _unit(sd, name, x, k, stride=1, fp16=None):
+    """fp16: None, or (unit names whose input is rounded to fp16, unit names whose weights are)."""
     w = sd[f"{name}.conv3d.weight"]
+    if fp16 is not None:
+        if name in fp16[0]:
+            x = _fp16(x)
+        if name in fp16[1]:
+            w = _fp16(w)
     pt, pb = _same_pad(k, stride)
     if k > 1:
         x = F.pad(x, (pt, pb, pt, pb, pt, pb))            # zeros; symmetric for k=3,s=1, (2,3) for the 7/2 stem
@@ -96,32 +114,43 @@ def _maxpool(x, k, s):
     return F.max_pool3d(x, k, s, ceil_mode=True)
 
 
-def _mixed(sd, m, x):
-    b0 = _unit(sd, f"{m}.branch_0", x, 1)
-    b1 = _unit(sd, f"{m}.branch_1.1", _unit(sd, f"{m}.branch_1.0", x, 1), 3)
-    b2 = _unit(sd, f"{m}.branch_2.1", _unit(sd, f"{m}.branch_2.0", x, 1), 3)
-    b3 = _unit(sd, f"{m}.branch_3.1", _maxpool(x, (3, 3, 3), (1, 1, 1)), 1)
+def _mixed(sd, m, x, fp16=None):
+    b0 = _unit(sd, f"{m}.branch_0", x, 1, fp16=fp16)
+    b1 = _unit(sd, f"{m}.branch_1.1", _unit(sd, f"{m}.branch_1.0", x, 1, fp16=fp16), 3, fp16=fp16)
+    b2 = _unit(sd, f"{m}.branch_2.1", _unit(sd, f"{m}.branch_2.0", x, 1, fp16=fp16), 3, fp16=fp16)
+    b3 = _unit(sd, f"{m}.branch_3.1", _maxpool(x, (3, 3, 3), (1, 1, 1)), 1, fp16=fp16)
     return torch.cat((b0, b1, b2, b3), 1)
 
 
 @torch.no_grad()
-def forward_features(sd: Dict[str, torch.Tensor], inp: torch.Tensor, return_stages: bool = False):
-    """inp (B, C, T, 224, 224) float in [-1, 1] -> (B, 1024).  == I3D.forward(inp, features=True)."""
+def forward_features(sd: Dict[str, torch.Tensor], inp: torch.Tensor, return_stages: bool = False,
+                     declared_rounding: bool = False, fp16_units=DECLARED_FP16_UNITS, fp16_inputs=(),
+                     fp16_weights=()):
+    """inp (B, C, T, 224, 224) float in [-1, 1] -> (B, 1024).  == I3D.forward(inp, features=True), in the dtype of
+    inp and sd.  ``declared_rounding`` rounds to fp16 exactly the operands the engine keeps as single fp16: the inputs
+    listed at DECLARED_FP16_UNITS and the weights of the units `fp16_units` (() for an engine built with
+    VF_I3D_SINGLE=none).  fp16_inputs / fp16_weights (unit names) round further conv inputs / weights (precision
+    emulations: a pair tensor or a split weight left single fp16).  Stages: 1a, 2c, 3c, 4f, 5c."""
+    fp16 = None
+    if declared_rounding or fp16_inputs or fp16_weights:
+        names = unit_names()
+        fp16 = (set(fp16_inputs) | (set(_FP16_INPUT) if declared_rounding else set()),
+                set(fp16_weights) | ({names[i] for i in fp16_units} if declared_rounding else set()))
     st = {}
-    x = _unit(sd, "conv3d_1a_7x7", inp, 7, 2); st["1a"] = x
+    x = _unit(sd, "conv3d_1a_7x7", inp, 7, 2, fp16=fp16); st["1a"] = x
     x = _maxpool(x, (1, 3, 3), (1, 2, 2))
-    x = _unit(sd, "conv3d_2b_1x1", x, 1)
-    x = _unit(sd, "conv3d_2c_3x3", x, 3); st["2c"] = x
+    x = _unit(sd, "conv3d_2b_1x1", x, 1, fp16=fp16)
+    x = _unit(sd, "conv3d_2c_3x3", x, 3, fp16=fp16); st["2c"] = x
     x = _maxpool(x, (1, 3, 3), (1, 2, 2))
-    x = _mixed(sd, "mixed_3b", x)
-    x = _mixed(sd, "mixed_3c", x); st["3c"] = x
+    x = _mixed(sd, "mixed_3b", x, fp16)
+    x = _mixed(sd, "mixed_3c", x, fp16); st["3c"] = x
     x = _maxpool(x, (3, 3, 3), (2, 2, 2))
     for m in ("mixed_4b", "mixed_4c", "mixed_4d", "mixed_4e", "mixed_4f"):
-        x = _mixed(sd, m, x)
+        x = _mixed(sd, m, x, fp16)
     st["4f"] = x
     x = _maxpool(x, (2, 2, 2), (2, 2, 2))
-    x = _mixed(sd, "mixed_5b", x)
-    x = _mixed(sd, "mixed_5c", x); st["5c"] = x
+    x = _mixed(sd, "mixed_5b", x, fp16)
+    x = _mixed(sd, "mixed_5c", x, fp16); st["5c"] = x
     x = F.avg_pool3d(x, (2, 7, 7), (1, 1, 1))
     out = x.squeeze(3).squeeze(3).mean(2)
     return (out, st) if return_stages else out

@@ -83,6 +83,7 @@ def corr_pyramid(fmap1, fmap2):
 
 
 def _bilinear_sampler(img, coords):
+    # (utils.py:57-71; a size-1 axis divides by zero here: NaN / inf grid coordinates, NaN samples)
     H, W = img.shape[-2:]
     xg, yg = coords.split([1, 1], dim=-1)
     xg = 2 * xg / (W - 1) - 1
@@ -90,21 +91,42 @@ def _bilinear_sampler(img, coords):
     return F.grid_sample(img, torch.cat([xg, yg], dim=-1), align_corners=True)
 
 
-def corr_lookup(pyr, coords):
+def _pixel_sampler(img, coords):
+    """What _bilinear_sampler computes, in pixel coordinates: bilinear interpolation of img (B, 1, H, W) at coords
+    (B, h, w, 2) = (x, y), zero outside the map.  Equal to grid_sample's align_corners=True path wherever H, W > 1 and
+    defined for a size-1 axis too (the 1-pixel pyramid level of a padded side of 64 .. 127 px)."""
+    B, _, H, W = img.shape
+    flat = img.reshape(B, H * W)
+    x, y = coords[..., 0].reshape(B, -1), coords[..., 1].reshape(B, -1)
+    x0, y0 = torch.floor(x), torch.floor(y)
+    out = torch.zeros_like(x)
+    for dy in (0, 1):
+        for dx in (0, 1):
+            xi, yi = x0 + dx, y0 + dy
+            wgt = (1 - (x - xi).abs()) * (1 - (y - yi).abs())
+            inside = (xi >= 0) & (xi <= W - 1) & (yi >= 0) & (yi <= H - 1)
+            idx = (yi.clamp(0, H - 1) * W + xi.clamp(0, W - 1)).long()
+            out = out + torch.where(inside, wgt * flat.gather(1, idx), torch.zeros_like(wgt))
+    return out.view(B, 1, *coords.shape[1:3])
+
+
+def corr_lookup(pyr, coords, pixel_sampler: bool = False):
     """CorrBlock.__call__ (corr.py:29-50).  NB the window: delta = stack(meshgrid(dy, dx)) is added to (x, y), so
-    window axis 0 offsets x and axis 1 offsets y (the trained weights depend on it)."""
+    window axis 0 offsets x and axis 1 offsets y (the trained weights depend on it).  In the dtype of `coords`
+    (the reference's own float32 path ends in .float(), a no-op there)."""
     r = CORR_RADIUS
     coords = coords.permute(0, 2, 3, 1)
     b, h1, w1, _ = coords.shape
+    sampler = _pixel_sampler if pixel_sampler else _bilinear_sampler
     out = []
     for i in range(CORR_LEVELS):
         dx = torch.linspace(-r, r, 2 * r + 1)
         dy = torch.linspace(-r, r, 2 * r + 1)
         delta = torch.stack(torch.meshgrid(dy, dx, indexing="ij"), dim=-1).to(coords.device)
         centroid = coords.reshape(b * h1 * w1, 1, 1, 2) / 2 ** i
-        c = _bilinear_sampler(pyr[i], centroid + delta.view(1, 2 * r + 1, 2 * r + 1, 2))
+        c = sampler(pyr[i], centroid + delta.view(1, 2 * r + 1, 2 * r + 1, 2))
         out.append(c.view(b, h1, w1, -1))
-    return torch.cat(out, dim=-1).permute(0, 3, 1, 2).contiguous().float()
+    return torch.cat(out, dim=-1).permute(0, 3, 1, 2).contiguous()
 
 
 def motion_encoder(sd, flow, corr):
@@ -136,35 +158,59 @@ def upsample_flow(flow, mask):
     return up.reshape(N, 2, 8 * H, 8 * W)
 
 
+def _fp16(t: torch.Tensor) -> torch.Tensor:
+    return t.half().to(t.dtype)
+
+
+# The operands the engine keeps as single fp16 (every other GEMM operand is a split-fp16 pair, every weight hi + lo):
+# the convex-upsampling mask head's weights and mask.2's input (raft.cu: the nsplit = 1 / chan_lo = nullptr uploads).
+DECLARED_FP16_WEIGHTS = ("update_block.mask.0.weight", "update_block.mask.2.weight")
+
+
 @torch.no_grad()
 def forward(sd_in: Dict[str, torch.Tensor], image1: torch.Tensor, image2: torch.Tensor, iters: int = 20,
-            return_lowres: bool = False):
-    """RAFT.forward(image1, image2, iters=20, test_mode=True) -> flow_up (B,2,H,W); images float [0,255], H,W % 8 == 0."""
+            return_lowres: bool = False, taps: bool = False, declared_rounding: bool = False,
+            pixel_sampler: bool = False):
+    """RAFT.forward(image1, image2, iters=20, test_mode=True) -> flow_up (B,2,H,W); images float [0,255], H,W % 8 == 0.
+
+    Computes in the dtype of the images and the state dict (float32: the reference, bit for bit; float64: a
+    high-precision reference).  ``declared_rounding`` rounds to fp16 exactly the operands the engine keeps as single
+    fp16 (DECLARED_FP16_WEIGHTS and mask.2's input) and nothing else.  ``pixel_sampler`` samples the pyramid with
+    _pixel_sampler instead of the reference's normalised grid_sample, which divides by zero on a 1-pixel level.
+    ``taps`` adds a dict: fnet (both images), cnet (raw encoder output), pyramid, and per iteration lookup / net (GRU
+    hidden state) / lowres (coords1 - coords0) lists, and mask."""
     sd = _strip(sd_in)
+    if declared_rounding:
+        sd = {k: (_fp16(v) if k in DECLARED_FP16_WEIGHTS else v) for k, v in sd.items()}
     image1 = 2 * (image1 / 255.0) - 1.0
     image2 = 2 * (image2 / 255.0) - 1.0
     f = encoder(sd, "fnet", torch.cat([image1, image2], 0), "instance")
     fmap1, fmap2 = torch.split(f, [image1.shape[0]] * 2, 0)
-    pyr = corr_pyramid(fmap1.float(), fmap2.float())
+    pyr = corr_pyramid(fmap1, fmap2)
     cnet = encoder(sd, "cnet", image1, "batch")
     net, inp = torch.split(cnet, [HDIM, CDIM], 1)
     net, inp = torch.tanh(net), torch.relu(inp)
     N, _, H, W = image1.shape
     ys, xs = torch.meshgrid(torch.arange(H // 8), torch.arange(W // 8), indexing="ij")
-    coords0 = torch.stack([xs, ys], 0).float()[None].repeat(N, 1, 1, 1).to(image1.device)
+    coords0 = torch.stack([xs, ys], 0).to(image1.dtype)[None].repeat(N, 1, 1, 1).to(image1.device)
     coords1 = coords0.clone()
-    flow_up = None
+    st = {"fnet": f, "cnet": cnet, "pyramid": pyr, "lookup": [], "net": [], "lowres": []}
     for _ in range(iters):
-        corr = corr_lookup(pyr, coords1)
+        corr = corr_lookup(pyr, coords1, pixel_sampler)
         flow = coords1 - coords0
         x = torch.cat([inp, motion_encoder(sd, flow, corr)], 1)
         net = sep_conv_gru(sd, net, x)
         p = "update_block.flow_head."
         delta = _conv(sd, p + "conv2", F.relu(_conv(sd, p + "conv1", net, 1, 1)), 1, 1)
         coords1 = coords1 + delta
-    mask = 0.25 * _conv(sd, "update_block.mask.2", F.relu(_conv(sd, "update_block.mask.0", net, 1, 1)))
+        if taps:
+            st["lookup"].append(corr); st["net"].append(net); st["lowres"].append(coords1 - coords0)
+    m0 = F.relu(_conv(sd, "update_block.mask.0", net, 1, 1))
+    mask = 0.25 * _conv(sd, "update_block.mask.2", _fp16(m0) if declared_rounding else m0)
+    st["mask"] = mask
     flow_up = upsample_flow(coords1 - coords0, mask)      # only the last iteration's result is returned (raft.py:172)
-    return (flow_up, coords1 - coords0) if return_lowres else flow_up
+    out = (flow_up, coords1 - coords0) if return_lowres else flow_up
+    return (out, st) if taps else out
 
 
 def synthetic_frames(n: int, h: int, w: int, seed: int = 0, shift=(1.7, -0.9)) -> torch.Tensor:

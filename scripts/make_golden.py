@@ -232,6 +232,37 @@ if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "raft":
     raft_golden()
 
 
+def raft_one_pixel_level_golden():
+    """The reference RAFT module (stand-in weights, 2 iterations) at padded sizes whose 4th pyramid level is one pixel
+    tall (96x128: 12x16 /8 map, level 3 is 1x2) or one pixel in both axes (64x120: 8x15, level 3 is 1x1).  Its
+    bilinear_sampler divides by H - 1 = 0 there: the fixture records the flow it returns (NaN)."""
+    import torch
+    sys.path.insert(0, REF)
+    cwd = os.getcwd()
+    os.chdir(REF)
+    try:
+        from models.raft.raft_src.raft import RAFT
+        from oracle import raft_net
+        sd = stand_in_state_dict("raft-sintel.pth")
+        net = torch.nn.DataParallel(RAFT(), device_ids=None)
+        net.load_state_dict(sd)
+        net = net.module.eval()
+        d = {}
+        for (h, w) in ((96, 128), (64, 120)):
+            fr = raft_net.synthetic_frames(2, h, w, seed=h)
+            with torch.no_grad():
+                y_ref = net(fr[:-1], fr[1:], iters=2)
+            print(f"raft {h}x{w}: {int(torch.isnan(y_ref).sum())} of {y_ref.numel()} flow values NaN")
+            d[f"flow_{h}x{w}"] = y_ref.numpy().astype(np.float32)
+        np.savez_compressed(os.path.join(OUT, "raft_one_pixel_level.npz"), **d)
+    finally:
+        os.chdir(cwd)
+
+
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "raft_1px":
+    raft_one_pixel_level_golden()
+
+
 def resnet_golden():
     """The reference's own ExtractResNet.extract on the sample video, with torchvision's resnet constructors patched to
     return the calibrated stand-in (oracle/resnet_net.py); stores fps, timestamps, a sha1 per frame of the transform

@@ -11,6 +11,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -572,3 +573,180 @@ R21D_CASES = [
 ]
 
 ENGINE_CASES = RESNET_CASES + R21D_CASES
+
+
+# ------------------------------------------------------------------ the I3D and RAFT filters as the engines upload them
+# Restated from i3d.cu prepare_unit and raft.cu upload_conv / prep_* (vf_i3d_conv, vf_raft_conv read them back).  Each
+# returns, per conv: Wt (fp16 [n_out, nsplit * ntaps * k_per_tap], W_hi | W_lo), ntaps, k_per_tap, nsplit, the tap
+# shifts (dt, dh, dw), lo_mask, and the fp32 scale / bias of the epilogue (pad rows zero).
+
+def _f32(t):
+    return t.detach().float().numpy()
+
+
+def _bn_fold(sd, p):
+    """BatchNorm eval folded in fp32 the way the engines do it: s = g / sqrtf(v + 1e-5f), shift = b - m s.  In numpy
+    float32 (one IEEE rounding per operation, as the host C code; torch's vectorised CPU kernels may differ by 1 ulp)."""
+    g, v, b, m = (_f32(sd[p + k]) for k in (".weight", ".running_var", ".bias", ".running_mean"))
+    s = g / np.sqrt(v + np.float32(1e-5))
+    return torch.from_numpy(s), torch.from_numpy(b - m * s)
+
+
+def _upload(w, cols, n_out, ntaps, kpt, nsplit, shifts, scale, bias, lo_mask=None):
+    w5 = _as5d(w.float())
+    Wt, mask, _ = _finish(cols, w5, n_out, ntaps, kpt, nsplit)
+    co = w5.shape[0]
+    sc, bi = torch.zeros(n_out), torch.zeros(n_out)
+    sc[:co], bi[:co] = scale, bias
+    return dict(Wt=Wt, ntaps=ntaps, k_per_tap=kpt, nsplit=nsplit, shifts=shifts,
+                lo_mask=mask if lo_mask is None else lo_mask, scale=sc, bias=bi, n_out=n_out)
+
+
+# i3d.cu prepare_unit's `chosen`: the stem and the 3x3x3 convs of mixed_3b / 3c keep single fp16 weights
+I3D_SINGLE_UNITS = (0, 5, 7, 11, 13)
+
+
+def i3d_engine_filter(sd, name: str, index: int, nsplit: int):
+    """Unit `name` (index in unit_names() order) as i3d.cu uploads it with weight split nsplit:
+    1x1x1: one tap over both halves of a pair row [hi ci | lo ci], lo_mask bit kk where K block kk starts in the lo half;
+    3x3x3: 9 taps (kt, kh), each a run of the 3 kw positions x ci; the stem (7x7x7 stride 2 over the 8-phase volume):
+    4 t-taps of 4 w-positions x (4 h-slots x 8 phases x ci), filter index 2a + p, the k = 7 positions left empty."""
+    w = sd[name + ".conv3d.weight"].float()
+    co, ci, k = w.shape[0], w.shape[1], w.shape[2]
+    s, sh = _bn_fold(sd, name + ".batch3d")
+    if k == 1:
+        cols, ntaps, kpt, shifts = (lambda a, b, d: [(list(range(ci)), [ci + c for c in range(ci)])]), 1, 2 * ci, [(0, 0, 0)]
+    elif k == 3:
+        ntaps, kpt = 9, 3 * ci
+        cols = lambda a, b, d: [([(a * 3 + b) * kpt + d * ci + c for c in range(ci)], None)]
+        shifts = [(j // 3 - 1, j % 3 - 1, -1) for j in range(9)]
+    else:
+        pc = 8 * ci
+        ntaps, kpt = 4, 16 * pc
+
+        def cols(kt, kh, kw):
+            a, pt, b, ph, cw, pw = kt // 2, kt % 2, kh // 2, kh % 2, kw // 2, kw % 2
+            return [([a * kpt + cw * 4 * pc + b * pc + ((pt * 2 + ph) * 2 + pw) * ci + c for c in range(ci)], None)]
+        shifts = [(a - 1, 0, -1) for a in range(4)]
+    f = _upload(w, cols, co, ntaps, kpt, nsplit, shifts, s, sh)
+    if k != 1:
+        f["lo_mask"] = 0            # only the 1x1x1 units read pair rows
+    return f
+
+
+def i3d_engine_filters(sd, unit_names, single=I3D_SINGLE_UNITS, fast=False):
+    """Every unit; `single`: the units with single fp16 weights (() for VF_I3D_SINGLE=none), fast: all of them."""
+    return [i3d_engine_filter(sd, n, i, 1 if (fast or i in single) else 2) for i, n in enumerate(unit_names)]
+
+
+RAFT_CF_LO = 384                     # csrc/raft_kernels.h: the correlation features' lo half
+RAFT_CF, RAFT_HX = 768, 768
+
+
+def _raft_same(w, b, n_out, pitch, chan=None, chan_lo=None, nsplit=2, scale=None, shift=None, extra=1.0):
+    """prep_same_conv: taps = kernel rows (dh = a - kh/2), each a run of kw x pitch from kw/2 positions to the left."""
+    co, ci, kh, kw = w.shape
+    chan = list(range(ci)) if chan is None else list(chan)
+    kpt = kw * pitch
+
+    def cols(_, a, d):
+        base = a * kpt + d * pitch
+        return [([base + chan[c] for c in range(ci)], None if chan_lo is None else [base + k for k in chan_lo])]
+    return _upload(w, cols, n_out, kh, kpt, nsplit, [(0, a - kh // 2, -(kw // 2)) for a in range(kh)],
+                   *_raft_epilogue(b, scale, shift, extra))
+
+
+def _raft_epilogue(b, scale, shift, extra):
+    """upload_conv: scale s = bn_scale x extra, bias = b s + bn_shift x extra (fp32, no fused multiply-add)."""
+    e = np.float32(extra)
+    s = (_f32(scale) if scale is not None else np.ones(b.shape[0], np.float32)) * e
+    sh = _f32(shift) if shift is not None else np.zeros(b.shape[0], np.float32)
+    return torch.from_numpy(s), torch.from_numpy(_f32(b) * s + sh * e)
+
+
+def _raft_unmerged(w, b, n_out, nsplit=2, extra=1.0):
+    """prep_unmerged_conv with dup: one tap per (kh, kw) reading [x_hi ci | x_lo ci], the weight in both halves."""
+    co, ci, kh, kw = w.shape
+    kpt = 2 * ci
+
+    def cols(_, a, d):
+        base = (a * kw + d) * kpt
+        return [([base + c for c in range(ci)], [base + ci + c for c in range(ci)])]
+    shifts = [(0, a - kh // 2, d - kw // 2) for a in range(kh) for d in range(kw)]
+    return _upload(w, cols, n_out, kh * kw, kpt, nsplit, shifts, *_raft_epilogue(b, None, None, extra))
+
+
+def _raft_stride2(w, b, n_out, pitch, phase_stride, lo_off, scale, shift):
+    """prep_stride2_conv: k x k stride 2 over the phase repack; tap a reads phase row q + a - B (B = 2 for k = 7, 1 for
+    k = 3); filter index kh = 2a + ph - 1, kw = 2bq + pw - 1; lo half lo_off columns right of the hi half."""
+    co, ci, k, _ = w.shape
+    na, before = (4, 2) if k == 7 else (2, 1)
+    kpt = na * pitch
+
+    def col(kh, kw, c):
+        a, ph, bq, pw = (kh + 1) // 2, (kh + 1) % 2, (kw + 1) // 2, (kw + 1) % 2
+        return a * kpt + bq * pitch + (ph * 2 + pw) * phase_stride + c
+
+    def cols(_, kh, kw):
+        hi = [col(kh, kw, c) for c in range(ci)]
+        return [(hi, [j + lo_off for j in hi])]
+    return _upload(w, cols, n_out, na, kpt, 2, [(0, a - before, -before) for a in range(na)],
+                   *_raft_epilogue(b, scale, shift, 1.0))
+
+
+def raft_engine_filters(sd_in):
+    """Every conv of raft.cu in vf_raft_conv's order (include/vfeat.h), with the names of their weights."""
+    sd = {(k[7:] if k.startswith("module.") else k): v.float() for k, v in sd_in.items()}
+    out = []
+
+    def add(name, f):
+        out.append((name, f))
+
+    for p, batch in (("fnet", False), ("cnet", True)):
+        def bn(n):
+            return _bn_fold(sd, f"{p}.{n}") if batch else (None, None)
+
+        def W(n):
+            return sd[f"{p}.{n}.weight"], sd[f"{p}.{n}.bias"]
+
+        def same3(n, norm, c):
+            return _raft_same(*W(n), c, 2 * c, chan_lo=[c + i for i in range(c)], scale=bn(norm)[0], shift=bn(norm)[1])
+        # stem: input phase rows [16 hi | 16 lo], 4 (3 used) channels per phase
+        add(f"{p}.conv1", _raft_stride2(*W("conv1"), 64, 32, 4, 16, *bn("norm1")))
+        for blk in range(2):
+            for cv in (1, 2):
+                add(f"{p}.layer1.{blk}.conv{cv}", same3(f"layer1.{blk}.conv{cv}", f"layer1.{blk}.norm{cv}", 64))
+        for L, (ci, co) in ((2, (64, 96)), (3, (96, 128))):
+            lp = f"layer{L}"
+            add(f"{p}.{lp}.0.conv1", _raft_stride2(*W(f"{lp}.0.conv1"), co, 8 * ci, 2 * ci, ci, *bn(f"{lp}.0.norm1")))
+            wd, bd = W(f"{lp}.0.downsample.0")
+            # the 1x1 stride-2 downsample reads phase (0, 0) of the repacked row: [hi ci | lo ci]
+            add(f"{p}.{lp}.0.downsample.0",
+                _upload(wd, lambda a, b, d, ci=ci: [(list(range(ci)), [ci + c for c in range(ci)])], co, 1, 2 * ci, 2,
+                        [(0, 0, 0)], *_raft_epilogue(bd, *bn(f"{lp}.0.downsample.1"), 1.0)))
+            for n, norm in ((".0.conv2", ".0.norm2"), (".1.conv1", ".1.norm1"), (".1.conv2", ".1.norm2")):
+                add(f"{p}.{lp}{n}", same3(lp + n, lp + norm, co))
+        add(f"{p}.conv2", _raft_same(*W("conv2"), 256, 256, chan_lo=[128 + c for c in range(128)]))
+
+    u = "update_block."
+
+    def W(n):
+        return sd[u + n + ".weight"], sd[u + n + ".bias"]
+    lo256 = [256 + c for c in range(256)]
+    add("encoder.convc1", _raft_same(*W("encoder.convc1"), 256, RAFT_CF, chan_lo=[RAFT_CF_LO + c for c in range(324)]))
+    add("encoder.convc2", _raft_same(*W("encoder.convc2"), 192, 512, chan_lo=lo256))
+    # flow8 rows = (fx_hi, fy_hi, fx_lo, fy_lo, 0 ...)
+    add("encoder.convf1", _raft_same(*W("encoder.convf1"), 128, 8, chan_lo=[2, 3]))
+    add("encoder.convf2", _raft_same(*W("encoder.convf2"), 64, 256, chan_lo=[128 + c for c in range(128)]))
+    add("encoder.conv", _raft_same(*W("encoder.conv"), 128, 512, chan_lo=lo256))        # 126 rows padded to 128
+    for sfx in ("1", "2"):
+        wz, bz = W("gru.convz" + sfx)
+        wr, br = W("gru.convr" + sfx)
+        add("gru.convz|r" + sfx, _raft_same(torch.cat([wz, wr]), torch.cat([bz, br]), 256, RAFT_HX, chan=HX_CHAN,
+                                            chan_lo=HX_CHAN_LO))
+        add("gru.convq" + sfx, _raft_same(*W("gru.convq" + sfx), 128, RAFT_HX, chan=HX_CHAN, chan_lo=HX_CHAN_LO))
+    add("flow_head.conv1", _raft_unmerged(*W("flow_head.conv1"), 256))
+    add("flow_head.conv2", _raft_same(*W("flow_head.conv2"), 8, 512, chan_lo=lo256))      # 2 rows padded to 8
+    add("mask.0", _raft_unmerged(*W("mask.0"), 256, nsplit=1))
+    add("mask.2", _raft_same(*W("mask.2"), 576, 256, nsplit=1, extra=0.25))
+    return out

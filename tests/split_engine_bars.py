@@ -1,15 +1,18 @@
-"""Bars of the ResNet and R(2+1)D engines against a float64 forward of the same network (worst row: per frame or clip
-for a stage, per feature row), shared by test_split_engines_float64_gpu.py, which holds the engines to them, and
-test_split_engine_bars_cpu.py, which checks on the CPU that they tell the designed split-fp16 scheme apart from every
-variant that leaves one tensor class in single fp16.
+"""Bars of the split-fp16 engines against a float64 forward of the same network (worst row: per frame or clip for a
+stage, per feature row), shared by the float64 GPU tests (test_split_engines_float64_gpu.py: ResNet, R(2+1)D;
+test_i3d_raft_float64_gpu.py: I3D, RAFT, against a reference with each engine's declared fp16 rounding), and
+test_split_engine_bars_cpu.py, which checks in a CPU float64 emulation how far above each bar every variant that leaves
+one tensor class in single fp16 lies.  SEPARATION (ResNet, R(2+1)D) and SEPARATION_I3D / SEPARATION_RAFT state that
+factor per stage; a stage a class does not appear under is one where it is not told apart from the engine's own error.
 
 Each entry is (rel-L2, max-abs / max|ref|).  A bar sits 1.5x to 3x above the worst value the engine measured on an
-H100 (test_split_engines_float64_gpu.py's docstring has the numbers; the engine is deterministic, so a rerun gives the
-same values), and SEPARATION below says how far under the smallest error of any single-fp16 class it lies (the CPU test
-asserts it for ResNet-18 and R(2+1)D).  The margin is narrow because the engine's error is its fp32 accumulation:
-a change to the conv GEMM's K order, pipeline staging or tile widths that reorders the fp32 sums can move these values
-by that much with no loss of precision; such a change re-measures them.  That the engines upload every lo half, W_lo
-row and lo_mask bit is checked exactly, conv by conv and at every depth, by test_conv_gemm_resnet_r21d_gpu.py."""
+H100 (the GPU tests' docstrings and the comments below have the numbers; the engines are deterministic, so a rerun gives
+the same values).  The margin is narrow because the engine's error is its fp32 accumulation (and, for I3D, 1-ulp
+differences in its single-fp16 tensors): a change to the conv GEMM's K order, pipeline staging or tile widths that
+reorders the fp32 sums can move these values by that much with no loss of precision; such a change re-measures them.
+That the engines upload every lo half, W_lo row and lo_mask bit is checked exactly, conv by conv, by
+test_conv_gemm_resnet_r21d_gpu.py and test_i3d_raft_uploads_gpu.py: that, not these bars, is the guard for a loss
+too small to show at a stage (most I3D classes past mixed_3c)."""
 import torch
 
 RESNET_STAGES = ("stem", "maxpool", "layer1", "layer2", "layer3", "layer4", "features")
@@ -55,3 +58,68 @@ def within(err, bar, factor: float = 1.0) -> bool:
 def beyond(err, bar, factor: float = 1.0) -> bool:
     """rel-L2 or max-abs above factor x its bar: the check fails by at least that factor."""
     return err[0] > factor * bar[0] or err[1] > factor * bar[1]
+
+
+
+# ---- I3D and RAFT, against a float64 forward with the engine's declared rounding (oracle/i3d_net.py,
+# oracle/raft_net.py declared_rounding=True: the operands the engine keeps as single fp16 are rounded, nothing else),
+# held by test_i3d_raft_float64_gpu.py.  Worst rows measured on one H100 80GB HBM3 (400 W power limit), rel-L2 /
+# max-abs÷max; the bars sit 1.5x .. 3x above them (I3D rgb 1a: 2.9x / 2.4x, the rest 1.5x .. 2x):
+#   I3D rgb (T = 16, 11, two stacks; controls T = 12)      I3D flow (T = 12)
+#   1a  6.8e-7 / 2.1e-6                                    1.0e-6 / 2.1e-6
+#   2c  1.6e-5 / 1.2e-4                                    2.9e-5 / 1.5e-4
+#   3c  4.4e-5 / 1.1e-4                                    6.4e-5 / 1.1e-4
+#   4f  1.1e-4 / 2.3e-4                                    1.3e-4 / 2.4e-4
+#   5c  2.5e-4 / 3.9e-4                                    2.8e-4 / 4.8e-4
+#   features 3.8e-5 / 4.8e-5                               4.8e-5 / 4.4e-5
+# Past the stem I3D's error jumps (1a 6.8e-7, 2c 1.6e-5 with a max-abs 7x its rel-L2).  That is what 1-ulp flips of
+# the single-fp16 tensors (conv3d_2b's and every 1x1x1 reducer's output) would give: the engine rounds its fp32 value,
+# the reference its float64 value, an element near a rounding boundary lands on the other side, and each flip is a
+# 2^-11 error in that element that the Mixed blocks carry on (an estimate; the flips were not counted).  The bars therefore separate a lost lo class most sharply at 1a
+# (fp16 stem input or weights: 1.1e-4 against 2e-6) and 2c (fp16 weights: 2.8e-4, 11x the rgb bar).
+#   RAFT (128x160, 200x200, 270x480, 96x128, 64x120; 1 and 3 iterations): fnet 5.1e-6 / 5.0e-6, cnet 2.0e-6 / 2.4e-6,
+#   pyramid 3.6e-6 / 6.0e-6, lookup 3.4e-6 / 6.3e-6, GRU state 1.4e-5 / 2.5e-5, low-res flow 9.9e-5 / 1.1e-4,
+#   flow_up 4.6e-5 / 1.3e-4; flow_up after 20 iterations 2.7e-5 / 1.2e-4.
+# fp16 RAFT weights cost fnet 9.9e-4 (120x its bar).  The low-res flow's relative error is large because the flow after
+# one to three steps is small: the flow head's fp32 accumulation over K = 2 x 2304 is most of it.
+I3D_STAGES = ("1a", "2c", "3c", "4f", "5c", "features")       # read_stage 0 .. 4, then the features
+I3D_BARS = {
+    "rgb": {"1a": (2e-6, 5e-6), "2c": (2.5e-5, 2e-4), "3c": (7e-5, 2e-4), "4f": (1.8e-4, 3.5e-4),
+            "5c": (3.7e-4, 6e-4), "features": (6e-5, 8e-5)},
+    "flow": {"1a": (2e-6, 4e-6), "2c": (4.5e-5, 2.5e-4), "3c": (1e-4, 2e-4), "4f": (2e-4, 3.7e-4),
+             "5c": (4.3e-4, 7.5e-4), "features": (7.5e-5, 7e-5)},
+}
+RAFT_STAGES = ("fnet", "cnet", "pyramid", "lookup", "net", "lowres", "flow_up")
+RAFT_BARS = {"fnet": (8e-6, 8e-6), "cnet": (3.5e-6, 4e-6), "pyramid": (6e-6, 9e-6), "lookup": (6e-6, 1e-5),
+             "net": (2.2e-5, 4e-5), "lowres": (1.5e-4, 1.7e-4), "flow_up": (7e-5, 2e-4)}
+RAFT_BAR_20_ITERS = (4.5e-5, 2e-4)      # flow_up after 20 iterations
+
+# How far above the bar (bars.beyond: rel-L2 or max-abs, whichever is further) each variant that leaves one class in
+# single fp16 lies, in the CPU float64 emulation of test_split_engine_bars_cpu.py, at the stages where it is asserted.
+# I3D (rgb stand-in, 1 x 3 x 10 x 224 x 224, against the declared-rounding reference; measured in parentheses).  Every
+# class is separated at the first stage it reaches (2c: 9.7 .. 11x, 3c: 2.5 .. 4.3x); past 3c most are within 2x of
+# the bar or under it, where only the conv read-back sees them.  The 1x1x1 weights show again at the features (6.8x).
+SEPARATION_I3D = {
+    "stem output": {"2c": 8, "3c": 2},                        # (9.7, 2.5)   the stem output = conv3d_2b's input
+    "pool outputs": {"3c": 2.4},                              # (2.9)        every branch_3 pool, pool3a / 4a / 5a
+    "concat buffers": {"3c": 2.2, "4f": 1.5},                 # (2.7, 1.8)   the Mixed outputs read by the next block
+    "1x1x1 inputs": {"2c": 8, "3c": 3.5, "4f": 1.7},          # (9.7, 4.3, 2.1)
+    "2b / 2c weights": {"2c": 9, "3c": 2.3},                  # (11.0, 2.8)
+    "1x1x1 weights": {"3c": 3.3, "4f": 1.8, "features": 5},   # (4.1, 2.2, 6.8)
+    "4x / 5x 3x3x3 weights": {"features": 2.3},               # (3.2)
+}
+# RAFT (stand-in, 2 frames of 128 x 160, 3 iterations, the operand groups of scripts/precision/emulate_raft.py).
+# Strongly separated at the first stage each reaches; at the low-res flow and flow_up every class lies 1.3 .. 9x above
+# the bars and is not asserted.  The flow head's conv2 input is separated nowhere (1.3x at the low-res flow).
+SEPARATION_RAFT = {
+    "fnet weights": {"fnet": 100, "pyramid": 35, "lookup": 20, "net": 18},   # (124, 47, 44, 27)
+    "cnet weights": {"cnet": 45, "net": 9},                                    # (60, 12)
+    "motion encoder weights": {"net": 18},                                     # (23)
+    "GRU weights": {"net": 7.5},                                               # (9.5)
+    "flow head weights": {"flow_up": 7.5},                                     # (9.4)
+    "fnet inner inputs": {"fnet": 100, "pyramid": 35, "lookup": 20, "net": 15},  # (131, 50, 46, 20)
+    "cnet inner inputs": {"cnet": 50, "net": 10},                              # (77, 12.5)
+    "motion encoder intermediates": {"net": 11},                               # (14)
+    "flow head conv2 input": {},                                               # (1.3 at the low-res flow)
+    "GRU motion slice": {"net": 4.5},                                          # (5.8)
+}

@@ -99,6 +99,8 @@ SIGNATURES = {
     "vf_i3d_forward_flow": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_i3d_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
     "vf_i3d_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_i3d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p,
+                              C.c_void_p]),
     "vf_raft_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "vf_raft_destroy": (C.c_int, [C.c_void_p]),
     "vf_raft_flow": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -106,6 +108,8 @@ SIGNATURES = {
     "vf_raft_padded_size": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "vf_raft_debug_read": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
     "vf_raft_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_raft_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p,
+                               C.c_void_p]),
     "vf_resnet_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
     "vf_resnet_destroy": (C.c_int, [C.c_void_p]),
     "vf_resnet_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -169,3 +173,21 @@ def read_conv(fn, handle, index: int, device):
     check(fn(handle, index, geom, C.byref(mask), w.data_ptr(), scale.data_ptr(), bias.data_ptr()))
     shifts = [tuple(geom[3 + 3 * j:6 + 3 * j]) for j in range(ntaps)]
     return dict(n_out=n_out, ntaps=ntaps, k_per_tap=kpt, shifts=shifts, lo_mask=mask.value, w=w, scale=scale, bias=bias)
+
+
+def read_split_conv(fn, handle, index: int, device):
+    """Diagnostics shared by I3DEngine.conv / RAFTEngine.conv: fn is vf_i3d_conv or vf_raft_conv.  Returns dict n_out,
+    ntaps, k_per_tap, nsplit, shifts [(dt, dh, dw)] per tap, lo_mask, w (fp16 [n_out, nsplit ntaps k_per_tap]: W_hi,
+    then W_lo when nsplit is 2), scale, bias (fp32 [n_out]) as uploaded."""
+    import torch
+    geom = (C.c_int * 196)()
+    mask = C.c_uint64()
+    check(fn(handle, index, geom, C.byref(mask), None, None, None))
+    n_out, ntaps, kpt, nsplit = geom[0], geom[1], geom[2], geom[3]
+    w = torch.empty((n_out, nsplit * ntaps * kpt), dtype=torch.float16, device=device)
+    scale = torch.empty(n_out, dtype=torch.float32, device=device)
+    bias = torch.empty(n_out, dtype=torch.float32, device=device)
+    check(fn(handle, index, geom, C.byref(mask), w.data_ptr(), scale.data_ptr(), bias.data_ptr()))
+    shifts = [tuple(geom[4 + 3 * j:7 + 3 * j]) for j in range(ntaps)]
+    return dict(n_out=n_out, ntaps=ntaps, k_per_tap=kpt, nsplit=nsplit, shifts=shifts, lo_mask=mask.value, w=w,
+                scale=scale, bias=bias)

@@ -207,6 +207,14 @@ static int prepare_unit(vf_i3d* h, ConvUnit& u, const vf_conv_unit& src, int idx
     return VF_OK;
 }
 
+// tap j's shift in (t, h, w) rows: 3x3x3 taps are (kt, kh) with the 3 kw positions inside the run; the stem's taps are
+// its 4 t-taps (the h-taps live inside the row)
+static void unit_tap(const ConvUnit& u, int j, int* dt, int* dh, int* dw) {
+    *dt = 0; *dh = 0; *dw = 0;
+    if (u.k == 3) { *dt = j / 3 - 1; *dh = j % 3 - 1; *dw = -1; }
+    else if (u.k == 7) { *dt = j - 1; *dw = -1; }
+}
+
 // conv + BN + ReLU of one unit over a bordered volume; out rows keep the input's row indexing
 // split_off > 0: the output is a pair tensor, hi at column n and lo at column split_off + n of the rows at `out`
 static int run_unit(vf_i3d* h, const ConvUnit& u, const __half* X, int ldx_channels, const Vol& v, __half* out, int ldo,
@@ -217,12 +225,10 @@ static int run_unit(vf_i3d* h, const ConvUnit& u, const __half* X, int ldx_chann
     g.ntaps = u.ntaps;
     g.nsplit = u.nsplit;          // hi/lo weight passes share each A tile inside the kernel
     g.lo_mask = u.lo_mask;
-    const int hw = v.Hp * v.Wp;
     for (int j = 0; j < u.ntaps; ++j) {
-        int off = 0;
-        if (u.k == 3) off = (j / 3 - 1) * hw + (j % 3 - 1) * v.Wp - 1;
-        else if (u.k == 7) off = (j - 1) * hw - 1;        // t-taps only: the h-taps live inside the row
-        g.tap_off[j] = off;
+        int dt, dh, dw;
+        unit_tap(u, j, &dt, &dh, &dw);
+        g.tap_off[j] = (dt * v.Hp + dh) * v.Wp + dw;
     }
     g.mask = 1;
     g.Tp = v.Tp; g.Hp = v.Hp; g.Wp = v.Wp;
@@ -325,45 +331,65 @@ int vf_i3d_destroy(vf_i3d_t* h) {
 
 }  // extern "C"
 
+// geometry of the trunk for nb clips of T frames: the volumes after the stem, pool2a, pool3a, pool4a and pool5a, and
+// where in bufA the mixed_4x and 5b outputs go
+struct TrunkGeom { Vol v0, v1, v2, v3, v4; __half *a4, *a5; };
+static TrunkGeom trunk_geom(const vf_i3d* h, int nb, int T) {
+    TrunkGeom g;
+    const int T1 = T / 2, Tq = T1 + 3;            // torch conv3d, pad (2,3), stride 2: floor((T-2)/2)+1
+    const int T2 = ceil_div(T1, 2), T3 = ceil_div(T2, 2);
+    g.v0 = Vol{nb, Tq, 115, 115, 1, 1 + T1, 1, 113, 1, 113};
+    g.v1 = bordered(nb, T1, 56, 56);
+    g.v2 = bordered(nb, T1, 28, 28);
+    g.v3 = bordered(nb, T2, 14, 14);
+    g.v4 = bordered(nb, T3, 7, 7);
+    // bufA's later outputs go behind what stays readable for read_stage: mixed_3c (v2, 960 columns) at a4, mixed_4f
+    // (v3, 1664 columns) at a5.  All three fit in bufA (its rows2 x 2048 holds rows2 x 1384 at T = 10, less beyond).
+    g.a4 = h->bufA + size_t(g.v2.rows()) * 960;
+    g.a5 = g.a4 + size_t(g.v3.rows()) * 1664;
+    return g;
+}
+
+// the activations vf_i3d_read_stage reads after a forward of nb clips of T frames (graph replays included)
+static void set_stages(vf_i3d* h, int nb, int T) {
+    const TrunkGeom g = trunk_geom(h, nb, T);
+    h->stages[0] = {h->a1, g.v0, 64};
+    h->stages[1] = {h->c2c, g.v1, 192};
+    h->stages[2] = {h->bufA, g.v2, 480};
+    h->stages[3] = {g.a4, g.v3, 832};
+    h->stages[4] = {h->bufB, g.v4, 1024};
+}
+
 // everything after the stem's phase volume h->s0 has been filled for nb clips of T frames
 static int i3d_trunk(vf_i3d* h, int nb, int T, float* out, cudaStream_t s) {
-    const int T1 = T / 2, Tq = T1 + 3;            // torch conv3d, pad (2,3), stride 2: floor((T-2)/2)+1
-    const Vol v0{nb, Tq, 115, 115, 1, 1 + T1, 1, 113, 1, 113};
+    const TrunkGeom g = trunk_geom(h, nb, T);
+    const Vol &v0 = g.v0, &v1 = g.v1, &v2 = g.v2, &v3 = g.v3, &v4 = g.v4;
+    __half *a4 = g.a4, *a5 = g.a5;
     VF_TRY(run_unit(h, h->units[0], h->s0, 32 * h->cin, v0, h->a1, 128, s, 64));       // a1: pair tensor
     // ---- maxPool3d_2a (1,3,3)/(1,2,2), SAME pad (0,1) on H,W
-    const Vol v1 = bordered(nb, T1, 56, 56);
     VF_TRY(launch_maxpool3d(h->a1, v0, h->p1, v1, 64, 1, 3, 3, 1, 2, 2, 0, 0, 0, s));
     VF_TRY(run_unit(h, h->units[1], h->p1, 128, v1, h->c2b, 64, s));                   // pair in, single out
     VF_TRY(run_unit(h, h->units[2], h->c2b, 64, v1, h->c2c, 384, s, 192));             // single in, pair out
     // ---- maxPool3d_3a
-    const Vol v2 = bordered(nb, T1, 28, 28);
     VF_TRY(launch_maxpool3d(h->c2c, v1, h->bufA, v2, 192, 1, 3, 3, 1, 2, 2, 0, 0, 0, s));
     VF_TRY(mixed_block(h, 0, h->bufA, v2, h->bufB, s));     // 3b -> 256
     VF_TRY(mixed_block(h, 1, h->bufB, v2, h->bufA, s));     // 3c -> 480
     // ---- maxPool3d_4a 3x3x3 / 2, SAME pad (0,1)
-    const int T2 = ceil_div(T1, 2);
-    const Vol v3 = bordered(nb, T2, 14, 14);
     VF_TRY(launch_maxpool3d(h->bufA, v2, h->bufB, v3, 480, 3, 3, 3, 2, 2, 2, 0, 0, 0, s));
-    VF_TRY(mixed_block(h, 2, h->bufB, v3, h->bufA, s));     // 4b -> 512
-    VF_TRY(mixed_block(h, 3, h->bufA, v3, h->bufB, s));     // 4c
-    VF_TRY(mixed_block(h, 4, h->bufB, v3, h->bufA, s));     // 4d
-    VF_TRY(mixed_block(h, 5, h->bufA, v3, h->bufB, s));     // 4e -> 528
-    VF_TRY(mixed_block(h, 6, h->bufB, v3, h->bufA, s));     // 4f -> 832
+    VF_TRY(mixed_block(h, 2, h->bufB, v3, a4, s));          // 4b -> 512
+    VF_TRY(mixed_block(h, 3, a4, v3, h->bufB, s));          // 4c
+    VF_TRY(mixed_block(h, 4, h->bufB, v3, a4, s));          // 4d
+    VF_TRY(mixed_block(h, 5, a4, v3, h->bufB, s));          // 4e -> 528
+    VF_TRY(mixed_block(h, 6, h->bufB, v3, a4, s));          // 4f -> 832
     // ---- maxPool3d_5a 2x2x2 / 2, no padding, ceil mode
-    const int T3 = ceil_div(T2, 2);
-    if (T3 < 2) return fail(VF_ERR_INVALID, "i3d_forward: T=%d leaves %d temporal positions for the (2,7,7) pool", T, T3);
-    const Vol v4 = bordered(nb, T3, 7, 7);
-    VF_TRY(launch_maxpool3d(h->bufA, v3, h->bufB, v4, 832, 2, 2, 2, 2, 2, 2, 0, 0, 0, s));
-    VF_TRY(mixed_block(h, 7, h->bufB, v4, h->bufA, s));     // 5b -> 832
-    VF_TRY(mixed_block(h, 8, h->bufA, v4, h->bufB, s));     // 5c -> 1024
+    if (v4.T() < 2) return fail(VF_ERR_INVALID, "i3d_forward: T=%d leaves %d temporal positions for the (2,7,7) pool", T, v4.T());
+    VF_TRY(launch_maxpool3d(a4, v3, h->bufB, v4, 832, 2, 2, 2, 2, 2, 2, 0, 0, 0, s));
+    VF_TRY(mixed_block(h, 7, h->bufB, v4, a5, s));          // 5b -> 832
+    VF_TRY(mixed_block(h, 8, a5, v4, h->bufB, s));          // 5c -> 1024
     // ---- AvgPool3d((2,7,7),1) + mean over time
     VF_TRY(launch_i3d_head(h->bufB, v4, 1024, out, s));
     h->launches += 5;
-    h->stages[0] = {h->a1, v0, 64};
-    h->stages[1] = {h->c2c, v1, 192};
-    h->stages[2] = {nullptr, v2, 480};
-    h->stages[3] = {h->bufA, v3, 832};
-    h->stages[4] = {h->bufB, v4, 1024};
+    set_stages(h, nb, T);
     return VF_OK;
 }
 
@@ -392,6 +418,7 @@ static int i3d_trunk_graphed(vf_i3d* h, int nb, int T, float* out, cudaStream_t 
         h->launches = before;
     }
     VF_CUDA(cudaGraphLaunch(it->second, s));
+    set_stages(h, nb, T);
     VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(nb) * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     h->launches += 72;
     return VF_OK;
@@ -485,5 +512,24 @@ int vf_i3d_read_stage(vf_i3d_t* h, int stage, float* out, int64_t capacity, int*
 }
 
 int64_t vf_i3d_launch_count(const vf_i3d_t* h) { return h ? h->launches : 0; }
+
+int vf_i3d_conv(const vf_i3d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias) {
+    if (!h || !geom || !lo_mask) return fail(VF_ERR_INVALID, "i3d_conv: null argument");
+    if (index < 0 || index >= VF_I3D_UNITS)
+        return fail(VF_ERR_INVALID, "i3d_conv: index %d outside the %d units", index, VF_I3D_UNITS);
+    const ConvUnit& u = h->units[index];
+    geom[0] = u.cout; geom[1] = u.ntaps; geom[2] = u.k_per_tap; geom[3] = u.nsplit;
+    for (int j = 0; j < 64; ++j) {
+        geom[4 + 3 * j] = geom[5 + 3 * j] = geom[6 + 3 * j] = 0;
+        if (j < u.ntaps) unit_tap(u, j, &geom[4 + 3 * j], &geom[5 + 3 * j], &geom[6 + 3 * j]);
+    }
+    *lo_mask = u.lo_mask;
+    VF_CUDA(cudaSetDevice(h->device));
+    const size_t nw = size_t(u.cout) * u.nsplit * u.ntaps * u.k_per_tap;
+    if (w) VF_CUDA(cudaMemcpy(w, u.w, nw * sizeof(__half), cudaMemcpyDeviceToDevice));
+    if (scale) VF_CUDA(cudaMemcpy(scale, u.scale, size_t(u.cout) * sizeof(float), cudaMemcpyDeviceToDevice));
+    if (bias) VF_CUDA(cudaMemcpy(bias, u.bias, size_t(u.cout) * sizeof(float), cudaMemcpyDeviceToDevice));
+    return VF_OK;
+}
 
 }  // extern "C"

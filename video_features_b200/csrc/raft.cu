@@ -625,8 +625,12 @@ int vf_raft_flow(vf_raft_t* h, const void* frames, int is_u8, int chw_layout, in
     const int pad_h = (((Hs / 8) + 1) * 8 - Hs) % 8, pad_w = (((Ws / 8) + 1) * 8 - Ws) % 8;
     const int pl = pad_w / 2, pt = pad_h / 2;
     const int H = Hs + pad_h, W = Ws + pad_w;
-    if (H > h->max_h || W > h->max_w || H < 16 || W < 16)
+    if (H > h->max_h || W > h->max_w)
         return fail(VF_ERR_INVALID, "raft_flow: padded frame %dx%d outside the workspace (%dx%d)", H, W, h->max_h, h->max_w);
+    // below 64 px the /8 map has fewer than 8 rows or columns and the 4th pyramid level none (the reference's
+    // avg_pool2d raises there); from 64 to 127 px that level is 1 pixel wide, which the lookup samples correctly
+    if (H < 64 || W < 64)
+        return fail(VF_ERR_INVALID, "raft_flow: padded frame %dx%d is under 64 px: the 4th correlation level would be empty", H, W);
     const int F = n_frames, NP = F - 1, H8 = H / 8, W8 = W / 8, P = H8 * W8;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
     VF_CUDA(cudaSetDevice(h->device));
@@ -717,5 +721,38 @@ int vf_raft_debug_read(vf_raft_t* h, int what, float* out, int64_t capacity, int
 }
 
 int64_t vf_raft_launch_count(const vf_raft_t* h) { return h ? h->launches : 0; }
+
+int vf_raft_conv(const vf_raft_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias) {
+    if (!h || !geom || !lo_mask) return fail(VF_ERR_INVALID, "raft_conv: null argument");
+    std::vector<const ConvW*> cs;
+    for (const vf_raft::Enc& e : h->enc) {
+        cs.push_back(&e.conv1);
+        for (const ConvW& c : e.l1) cs.push_back(&c);
+        cs.push_back(&e.l2c1); cs.push_back(&e.l2down);
+        for (const ConvW& c : e.l2) cs.push_back(&c);
+        cs.push_back(&e.l3c1); cs.push_back(&e.l3down);
+        for (const ConvW& c : e.l3) cs.push_back(&c);
+        cs.push_back(&e.conv2);
+    }
+    for (const ConvW* c : {&h->convc1, &h->convc2, &h->convf1, &h->convf2, &h->convm, &h->zr1, &h->q1, &h->zr2, &h->q2,
+                           &h->fh1, &h->fh2, &h->mk0, &h->mk2})
+        cs.push_back(c);
+    if (index < 0 || index >= int(cs.size()))
+        return fail(VF_ERR_INVALID, "raft_conv: index %d outside the %d convs", index, int(cs.size()));
+    const ConvW& c = *cs[index];
+    geom[0] = c.n_out; geom[1] = c.ntaps; geom[2] = c.k_per_tap; geom[3] = c.nsplit;
+    for (int j = 0; j < 64; ++j) {
+        geom[4 + 3 * j] = 0;
+        geom[5 + 3 * j] = j < c.ntaps ? c.dh[j] : 0;
+        geom[6 + 3 * j] = j < c.ntaps ? c.dw0[j] : 0;
+    }
+    *lo_mask = c.lo_mask;
+    VF_CUDA(cudaSetDevice(h->device));
+    const size_t nw = size_t(c.n_out) * c.nsplit * c.ntaps * c.k_per_tap;
+    if (w) VF_CUDA(cudaMemcpy(w, c.w, nw * sizeof(__half), cudaMemcpyDeviceToDevice));
+    if (scale) VF_CUDA(cudaMemcpy(scale, c.scale, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
+    if (bias) VF_CUDA(cudaMemcpy(bias, c.bias, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
+    return VF_OK;
+}
 
 }  // extern "C"

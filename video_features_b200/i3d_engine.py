@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import ops  # noqa: F401  (registers torch.ops.vfeat.*)
-from ._lib import I3D_UNITS, I3DWeights, check, lib
+from ._lib import I3D_UNITS, I3DWeights, check, lib, read_split_conv
 
 _MIXED = ["mixed_3b", "mixed_3c", "mixed_4b", "mixed_4c", "mixed_4d", "mixed_4e", "mixed_4f", "mixed_5b", "mixed_5c"]
 
@@ -151,6 +151,12 @@ class I3DEngine:
             check(lib().vf_i3d_read_stage(self._h, stage, out.data_ptr(), out.numel(), dims,
                                           torch.cuda.current_stream().cuda_stream))
         return out
+
+    def conv(self, index: int) -> dict:
+        """Diagnostics: unit ``index`` (unit_names() order) as uploaded (include/vfeat.h vf_i3d_conv); see
+        _lib.read_split_conv."""
+        with torch.cuda.device(self.device):
+            return read_split_conv(lib().vf_i3d_conv, self._h, index, self.device)
 
     @property
     def launch_count(self) -> int:

@@ -8,7 +8,7 @@ from typing import Dict
 import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib
+from ._lib import NamedTensor, check, lib, read_split_conv
 
 
 class RAFTEngine:
@@ -69,6 +69,12 @@ class RAFTEngine:
             check(lib().vf_raft_debug_read(self._h, what, out.data_ptr(), out.numel(), dims,
                                            torch.cuda.current_stream().cuda_stream))
         return out
+
+    def conv(self, index: int) -> dict:
+        """Diagnostics: conv ``index`` as uploaded (include/vfeat.h vf_raft_conv gives the order); see
+        _lib.read_split_conv."""
+        with torch.cuda.device(self.device):
+            return read_split_conv(lib().vf_raft_conv, self._h, index, self.device)
 
     @property
     def launch_count(self) -> int:
