@@ -221,6 +221,21 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             if (++kk == kpt) kk = 0;              // K block index inside the current tap
         }
         if (PP && i + 1 < cta_tiles) pass_turn();
+        // Scale and bias of this thread's columns in the first 64-column subtile, loaded while the last MMAs run.  A
+        // missing scale reads as 1 and a missing bias as -0: x * 1 and x + (-0) are x bit for bit (a +0 bias would turn
+        // -0 into +0), so every launch runs the same branch-free arithmetic and gets the bits of skipping the operation.
+        // A column pair at or past N (N % 8 == 0: a pair is wholly inside or outside) reads the scale / bias of the
+        // last pair and is computed like the others, so there is no per-element bounds test: TMA clips those columns.
+        float2 sc[8], bi[8];
+        auto load_sb = [&](int s) {
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                const int n = min(n0 + 64 * s + 8 * c + 2 * (lane & 3), N - 2);
+                sc[c] = ep.scale ? __ldg(reinterpret_cast<const float2*>(ep.scale + n)) : make_float2(1.f, 1.f);
+                bi[c] = ep.bias ? __ldg(reinterpret_cast<const float2*>(ep.bias + n)) : make_float2(-0.f, -0.f);
+            }
+        };
+        load_sb(0);
         wgmma_wait<0>();
         wgmma_fence_regs<R>(acc);
         __syncwarp();
@@ -239,92 +254,80 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 keep[h] = (mm >= 0) && (w >= cg.w0) && (w < cg.w1) && (hh >= cg.h0) && (hh < cg.h1) && (tt >= cg.t0) && (tt < cg.t1);
             }
         }
-        // scale / bias / activation / row mask of accumulator column group j, in place.  A column pair at or past N
-        // (N % 8 == 0: a pair is wholly inside or outside) reads the scale / bias of the last pair and is computed like
-        // the others, so there is no per-element bounds test: TMA clips those columns.  The product and the sum are
-        // the separately rounded ones the epilogue has always computed; _rn keeps the compiler from contracting them
-        // into an fma now that nothing branches between them.
-        const float* const scale = ep.scale;
-        const float* const bias = ep.bias;
-        auto finish = [&](int j) {
-            const int n = min(n0 + 8 * j + 2 * (lane & 3), N - 2);
-            float2 s = make_float2(1.f, 1.f), b = make_float2(0.f, 0.f);
-            if (scale) s = __ldg(reinterpret_cast<const float2*>(scale + n));
-            if (bias) b = __ldg(reinterpret_cast<const float2*>(bias + n));
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                if (scale) { v0 = __fmul_rn(v0, s.x); v1 = __fmul_rn(v1, s.y); }
-                if (bias) { v0 = __fadd_rn(v0, b.x); v1 = __fadd_rn(v1, b.y); }
-                if (ACT != VF_ACT_NONE) { v0 = apply_act<ACT>(v0); v1 = apply_act<ACT>(v1); }
-                if (!keep[h]) { v0 = 0.f; v1 = 0.f; }
-                acc[4 * j + 2 * h] = v0;
-                acc[4 * j + 2 * h + 1] = v1;
-            }
-        };
-        // Subtiles of 128-byte rows, left to right; those wholly at or past N are skipped.
+        // Subtiles of 64 columns (one fp16 or split box, two fp32 boxes), left to right; those wholly at or past N are
+        // skipped.  Each is finished in registers by one copy of the scale / bias / activation / row-mask code, whatever
+        // the output, and the next subtile's scale / bias loads are issued before this one is written out.  The product
+        // and the sum are the separately rounded ones the epilogue has always computed; _rn keeps the compiler from
+        // contracting them into an fma.
         const int row = m0;
         const uint32_t stg = smem_u32(sD) + wg * 2 * STG_BYTES + (wq * 16 + (lane >> 2)) * 128;
         const int swz = lane >> 2;
-        if (!SPLIT && ep.out_f32) {              // (run_gemm refuses a split fp32 output)
 #pragma unroll
-            for (int s = 0; s < BN / 32; ++s) {  // 32 columns: j = 4s .. 4s + 3
-                if (n0 + 32 * s >= N) break;
-                const uint32_t d = stg + buf * STG_BYTES;
+        for (int s = 0; s < BN / 64; ++s) {      // j = 8s .. 8s + 7
+            if (n0 + 64 * s >= N) break;
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const int j = 4 * s + c;
-                    finish(j);
-                    const int chunk = 2 * c + ((lane & 3) >> 1);
+            for (int c = 0; c < 8; ++c)
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        st_shared_v2_f32(d + h * 8 * 128 + ((chunk ^ swz) << 4) + 8 * (lane & 1), acc[4 * j + 2 * h],
-                                         acc[4 * j + 2 * h + 1]);
+                for (int h = 0; h < 2; ++h) {
+                    const int j = 8 * s + c;
+                    float v0 = __fadd_rn(__fmul_rn(acc[4 * j + 2 * h], sc[c].x), bi[c].x);
+                    float v1 = __fadd_rn(__fmul_rn(acc[4 * j + 2 * h + 1], sc[c].y), bi[c].y);
+                    v0 = apply_act<ACT>(v0);
+                    v1 = apply_act<ACT>(v1);
+                    acc[4 * j + 2 * h] = keep[h] ? v0 : 0.f;
+                    acc[4 * j + 2 * h + 1] = keep[h] ? v1 : 0.f;
                 }
-                store_subtile(n0 + 32 * s, row);
-            }
-        } else {
+            if (s + 1 < BN / 64) load_sb(s + 1);
+            if (SPLIT) {
+                // hi into buffer 0, lo = fp16(v - hi) into buffer 1, once both stores of the previous subtile have
+                // read their buffers
+                if (issuer) bulk_wait_read<0>();
+                wg_sync();
 #pragma unroll
-            for (int s = 0; s < BN / 64; ++s) {  // 64 columns: j = 8s .. 8s + 7
-                if (n0 + 64 * s >= N) break;
-                if (SPLIT) {
-                    // hi into buffer 0, lo = fp16(v - hi) into buffer 1, in one pass: finish the values first, then
-                    // wait until both stores of the previous subtile have read their buffers
+                for (int c = 0; c < 8; ++c)
 #pragma unroll
-                    for (int c = 0; c < 8; ++c) finish(8 * s + c);
-                    if (issuer) bulk_wait_read<0>();
-                    wg_sync();
-#pragma unroll
-                    for (int c = 0; c < 8; ++c)
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const int j = 8 * s + c;
-                            const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                            const __half2 hi = __floats2half2_rn(v0, v1);
-                            const uint32_t off = h * 8 * 128 + ((c ^ swz) << 4) + 4 * (lane & 3);
-                            st_shared_b32(stg + off, *reinterpret_cast<const uint32_t*>(&hi));
-                            st_shared_b32(stg + STG_BYTES + off, pack_half2(v0 - __low2float(hi), v1 - __high2float(hi)));
-                        }
-                    fence_proxy_async();
-                    wg_sync();
-                    if (issuer) {
-                        tma_store_2d(&tmD, sD + wg * 2 * STG_BYTES, n0 + 64 * s, row);
-                        tma_store_2d(&tmD2, sD + (wg * 2 + 1) * STG_BYTES, n0 + 64 * s, row);
-                        bulk_commit();
+                    for (int h = 0; h < 2; ++h) {
+                        const int j = 8 * s + c;
+                        const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                        const __half2 hi = __floats2half2_rn(v0, v1);
+                        const uint32_t off = h * 8 * 128 + ((c ^ swz) << 4) + 4 * (lane & 3);
+                        st_shared_b32(stg + off, *reinterpret_cast<const uint32_t*>(&hi));
+                        st_shared_b32(stg + STG_BYTES + off, pack_half2(v0 - __low2float(hi), v1 - __high2float(hi)));
                     }
-                } else {
+                fence_proxy_async();
+                wg_sync();
+                if (issuer) {
+                    tma_store_2d(&tmD, sD + wg * 2 * STG_BYTES, n0 + 64 * s, row);
+                    tma_store_2d(&tmD2, sD + (wg * 2 + 1) * STG_BYTES, n0 + 64 * s, row);
+                    bulk_commit();
+                }
+            } else if (ep.out_f32) {             // (run_gemm refuses a split fp32 output)
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {    // 32 columns: j = 8s + 4q .. 8s + 4q + 3
+                    if (q == 1 && n0 + 64 * s + 32 >= N) break;
                     const uint32_t d = stg + buf * STG_BYTES;
 #pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const int j = 8 * s + c;
-                        finish(j);
+                    for (int c = 0; c < 4; ++c) {
+                        const int j = 8 * s + 4 * q + c;
+                        const int chunk = 2 * c + ((lane & 3) >> 1);
 #pragma unroll
                         for (int h = 0; h < 2; ++h)
-                            st_shared_b32(d + h * 8 * 128 + ((c ^ swz) << 4) + 4 * (lane & 3),
-                                          pack_half2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+                            st_shared_v2_f32(d + h * 8 * 128 + ((chunk ^ swz) << 4) + 8 * (lane & 1), acc[4 * j + 2 * h],
+                                             acc[4 * j + 2 * h + 1]);
                     }
-                    store_subtile(n0 + 64 * s, row);
+                    store_subtile(n0 + 64 * s + 32 * q, row);
                 }
+            } else {
+                const uint32_t d = stg + buf * STG_BYTES;
+#pragma unroll
+                for (int c = 0; c < 8; ++c)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int j = 8 * s + c;
+                        st_shared_b32(d + h * 8 * 128 + ((c ^ swz) << 4) + 4 * (lane & 3),
+                                      pack_half2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
+                    }
+                store_subtile(n0 + 64 * s, row);
             }
         }
     }
