@@ -28,6 +28,7 @@ extern "C" {
 #define VF_ACT_RELU 2
 #define VF_ACT_SIGMOID 3
 #define VF_ACT_TANH 4
+#define VF_ACT_LEAKY 5     /* LeakyReLU(0.1): built for the conv mode with split weights (nsplit = 2) only */
 
 #define VF_FILTER_BILINEAR 2 /* PIL.Image.BILINEAR */
 #define VF_FILTER_BICUBIC 3  /* PIL.Image.BICUBIC  */
@@ -240,6 +241,32 @@ int64_t vf_raft_launch_count(const vf_raft_t* h);
  * block's convc1, convc2, convf1, convf2, conv, the stacked convz1|convr1, convq1, convz2|convr2, convq2, the flow head's
  * conv1, conv2 and the mask head's mask.0, mask.2 (45 in all).  n_out is the GEMM width (padded rows included). */
 int vf_raft_conv(const vf_raft_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+
+/* ---- PWC-Net optical flow: replaces `PWCNet()(first, second)` (models/pwc/pwc_src/pwc_net.py:212-263, with
+ * correlation.py's cost volume; called at models/pwc/extract_pwc.py:97 and models/i3d/extract_i3d.py:175).  Weights: the
+ * checkpoint's tensors by name (keys of pwc_net_sintel.pt), HOST fp32. */
+typedef struct vf_pwc vf_pwc_t;
+
+/* Workspace is sized for calls of max_frames frames of at most max_h x max_w pixels (each rounded up to 64). */
+int vf_pwc_create(vf_pwc_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_frames, int max_h,
+                  int max_w);
+int vf_pwc_destroy(vf_pwc_t* h);
+/* Flow between consecutive frames: frames n_frames x (Hs x Ws x 3 if !chw_layout else 3 x Hs x Ws), uint8 or fp32 in
+ * [0,255] on the device, passed as the reference's caller passes them (the model swaps channels 0 and 2 itself);
+ * == model(frames[:-1], frames[1:]).  out: (n_frames-1) x 2 x Hs x Ws fp32. */
+int vf_pwc_flow(vf_pwc_t* h, const void* frames, int is_u8, int chw_layout, int n_frames, int Hs, int Ws, float* out,
+                void* stream);
+/* Diagnostics: tensors of the last call as fp32 NCHW at pyramid level `level` (1..6: 1/2 .. 1/64 of the size rounded up
+ * to 64).  what: 0 extractor features (all frames), 1 cost volume after the LeakyReLU (81 ch), 2 upsampled flow
+ * (moduleUpflow, levels 2..5), 3 upsampled feature (moduleUpfeat, levels 2..5), 4 decoder flow, 5 refiner output (level
+ * 2; `level` ignored), 6 warp mask (levels 2..5).  dims4 receives the shape; out == NULL only queries it. */
+int vf_pwc_debug_read(vf_pwc_t* h, int what, int level, float* out, int64_t capacity, int* dims4, void* stream);
+int64_t vf_pwc_launch_count(const vf_pwc_t* h);
+/* Diagnostics: conv `index` as uploaded, as vf_raft_conv.  Order: the extractor's three convs per level 1..6; per decoder
+ * level 6, 5, 4, 3, 2: moduleUpflow, moduleUpfeat (not at level 6; ConvTranspose2d as 9 taps x 8 columns (py*2+px)*2 +
+ * oc), moduleOne .. moduleSix; the refiner's seven convs (63 in all).  Weights carry a power-of-two scale 2^e per output
+ * row (largest |w| in [2^14, 2^15), e <= 126) and scale holds 2^-e. */
+int vf_pwc_conv(const vf_pwc_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
 /* ---- ResNet-18/34/50/101/152 frame features: replaces torchvision `models.resnetXX(pretrained=True)` with
  * `fc = Identity()` in eval mode, and its per-frame transform Resize(256) -> CenterCrop(224) -> ToTensor -> Normalize

@@ -10,7 +10,7 @@ import torch  # noqa: F401
 
 from video_features_b200.utils import form_list_from_user_input, sanity_check
 
-SUPPORTED = ['i3d', 'raft', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
+SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
              'resnet101', 'resnet152', 'r21d_rgb']
 
 
@@ -25,13 +25,16 @@ def build_extractor(args):
     if args.feature_type == 'raft':
         from video_features_b200.extract.extract_raft import ExtractRAFT
         return ExtractRAFT(args)
+    if args.feature_type == 'pwc':
+        from video_features_b200.extract.extract_pwc import ExtractPWC
+        return ExtractPWC(args)
     if args.feature_type in ['resnet18', 'resnet34', 'resnet50', 'resnet101', 'resnet152']:
         from video_features_b200.extract.extract_resnet import ExtractResNet
         return ExtractResNet(args)
     if args.feature_type == 'r21d_rgb':
         from video_features_b200.extract.extract_r21d import ExtractR21D
         return ExtractR21D(args)
-    if args.feature_type in ['vggish', 'pwc', 'vggish_torch']:
+    if args.feature_type in ['vggish', 'vggish_torch']:
         raise NotImplementedError(f'{args.feature_type}: outside the hot path this engine rebuilds (SURVEY.md §2)')
     raise NotADirectoryError                      # main.py:41
 

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VF_LIBVFEAT") or os.path.join(_HERE, "libvfeat.so")
 
 VF_OK = 0
-VF_ACT_NONE, VF_ACT_QUICKGELU, VF_ACT_RELU, VF_ACT_SIGMOID, VF_ACT_TANH = 0, 1, 2, 3, 4
+VF_ACT_NONE, VF_ACT_QUICKGELU, VF_ACT_RELU, VF_ACT_SIGMOID, VF_ACT_TANH, VF_ACT_LEAKY = 0, 1, 2, 3, 4, 5
 VF_FILTER_BILINEAR, VF_FILTER_BICUBIC = 2, 3
 
 
@@ -110,6 +110,14 @@ SIGNATURES = {
     "vf_raft_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_raft_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p,
                                C.c_void_p]),
+    "vf_pwc_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vf_pwc_destroy": (C.c_int, [C.c_void_p]),
+    "vf_pwc_flow": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                              C.c_void_p]),
+    "vf_pwc_debug_read": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_pwc_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_pwc_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p,
+                              C.c_void_p]),
     "vf_resnet_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
     "vf_resnet_destroy": (C.c_int, [C.c_void_p]),
     "vf_resnet_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

@@ -21,9 +21,10 @@
 // third-party clip `VisionTransformer.forward`, called at models/CLIP/extract_clip.py:128) and the I3D / RAFT
 // convolutions in the shifted-row mode below.
 //
-// The kernel template is in gemm_kernel.cuh.  Its 120 instantiations (tile width x split weights x split output x
-// schedule x activation) are compiled in three units that build in parallel: gemm_inst_pp.cu (the ping-pong schedule),
-// gemm_inst_conv.cu and gemm_inst_conv_w2.cu (the conv mode with plain and split weights).  This file holds the host
+// The kernel template is in gemm_kernel.cuh.  Its 128 instantiations (tile width x split weights x split output x
+// schedule x activation; LeakyReLU only with split weights in the conv mode, PWC-Net's convolutions) are compiled in
+// three units that build in parallel: gemm_inst_pp.cu (the ping-pong schedule), gemm_inst_conv.cu and
+// gemm_inst_conv_w2.cu (the conv mode with plain and split weights).  This file holds the host
 // side: argument checks, tensor maps, tile-width choice and the profiling hooks.
 #include "gemm_kernel.cuh"
 
@@ -120,7 +121,7 @@ static int run_gemm(const CUtensorMap& tmA, bool pp, const __half* B, int ldb, i
     if (reinterpret_cast<uintptr_t>(ep.out) & 15) return fail(VF_ERR_INVALID, "gemm: output must be 16-byte aligned");
     if (ep.accumulate && !ep.out_f32) return fail(VF_ERR_INVALID, "gemm: accumulate needs fp32 output");
     if (N % 8) return fail(VF_ERR_INVALID, "gemm: N=%d must be a multiple of 8", N);
-    if (ep.act < VF_ACT_NONE || ep.act > VF_ACT_TANH) return fail(VF_ERR_INVALID, "gemm: unknown activation %d", ep.act);
+    if (ep.act < VF_ACT_NONE || ep.act > VF_ACT_LEAKY) return fail(VF_ERR_INVALID, "gemm: unknown activation %d", ep.act);
     if (ep.out_f32 ? (ep.ldo % 4) : (ep.ldo % 8)) return fail(VF_ERR_INVALID, "gemm: ldo breaks 16-byte rows");
     if (ep.split_off && (ep.out_f32 || ep.split_off < N || ep.split_off % 8))
         return fail(VF_ERR_INVALID, "gemm: split output needs fp16 out and split_off >= N, multiple of 8");

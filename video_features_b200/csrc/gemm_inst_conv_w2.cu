@@ -1,5 +1,5 @@
 // gemm_f16_kernel instantiations of the conv mode (vf_conv_gemm_f16) with split-fp16 weights (nsplit = 2): plain and
-// split-fp16 output, 4 tile widths x 5 activations each.
+// split-fp16 output, 4 tile widths x 6 activations each (LeakyReLU is built here only).
 #include "gemm_kernel.cuh"
 
 namespace vf {

@@ -67,6 +67,8 @@ __device__ __forceinline__ float apply_act(float v) {
         return __fdividef(1.0f, 1.0f + __expf(-v));
     } else if (ACT == VF_ACT_TANH) {
         return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * v));   // saturates cleanly to +-1
+    } else if (ACT == VF_ACT_LEAKY) {
+        return v > 0.0f ? v : __fmul_rn(v, 0.1f);            // torch's leaky_relu: x * negative_slope below 0
     }
     return v;
 }
@@ -370,6 +372,13 @@ int launch_act(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap
             return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_SIGMOID>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
         case VF_ACT_TANH:
             return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_TANH>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+        case VF_ACT_LEAKY:
+            // PWC-Net's activation: only its split-weight convolutions use it, so only that unit
+            // (gemm_inst_conv_w2.cu) carries the kernels
+            if constexpr (NSPLIT == 2 && !PP)
+                return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_LEAKY>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            else
+                return fail(VF_ERR_INVALID, "gemm: LeakyReLU is built for split-weight convolutions (nsplit = 2) only");
         default:
             return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_NONE>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
     }

@@ -5,13 +5,14 @@ Same constructor / attributes / ``forward(indices)`` / ``extract(...)`` surface,
 float64 ``(n_stacks, 1024)`` outputs.  Underneath, per group of up to ``VF_I3D_STACKS`` (default 8) stacks:
   decoder frames (uint8, BGR kept as the reference does) -> GPU Pillow-exact bilinear resize to min side 256
   -> rgb stream : fused crop + 2x/255-1 + phase packing -> I3D on all stacks of the group (vf_i3d_forward_u8_strided)
-  -> flow stream: RAFT on the 64 consecutive pairs of each stack, padded and NOT unpadded (extract_i3d.py:172)
+  -> flow stream: PWC-Net (``--flow_type pwc``, the CLI default) on the stack's 65 resized BGR frames, as the reference
+     passes them (extract_i3d.py:175), at the frame size; or RAFT on the 64 consecutive pairs of each stack, padded
+     and NOT unpadded (extract_i3d.py:172)
      -> fused crop + clamp + 8-bit quantisation + scaling -> I3D (vf_i3d_forward_flow)
 Features stay on the device until the video is finished: one device->host copy per stream per video instead of the
 reference's ``.tolist()`` per stack (extract_i3d.py:188).
 ``--flow_type flow`` (pre-computed ``flow_x_*.jpg`` / ``flow_y_*.jpg`` pairs, extract_i3d.py:195-229,266-278) feeds
-the same fused flow transform.  ``--flow_type pwc`` (the CLI default) is outside the rebuilt path (SURVEY.md §8 f3): it
-raises NotImplementedError at construction when the flow stream is requested.
+the same fused flow transform.
 """
 from __future__ import annotations
 
@@ -27,6 +28,7 @@ from tqdm import tqdm
 from .. import ops
 from .._lib import VF_FILTER_BILINEAR
 from ..i3d_engine import I3DEngine
+from ..pwc_engine import PWCEngine
 from ..raft_engine import RAFTEngine
 from ..utils import AsyncSink, already_extracted, VideoReader, action_on_extraction, form_list_from_user_input
 
@@ -36,13 +38,13 @@ DEFAULT_I3D_STEP_SIZE = 64
 DEFAULT_I3D_STACK_SIZE = 64
 _HERE = pathlib.Path(__file__).resolve().parent
 _CKPT_DIRS = [os.environ.get("VF_CKPT_DIR"), str(_HERE / "checkpoints"), str(_HERE.parents[1] / "checkpoints")]
-_CKPT = {'rgb': 'i3d_rgb.pt', 'flow': 'i3d_flow.pt', 'raft': 'raft-sintel.pth'}
+_CKPT = {'rgb': 'i3d_rgb.pt', 'flow': 'i3d_flow.pt', 'raft': 'raft-sintel.pth', 'pwc': 'pwc_net_sintel.pt'}
 _STATE_DICTS: Dict[str, Dict[str, torch.Tensor]] = {}
 
 
 def load_checkpoint(kind: str) -> Dict[str, torch.Tensor]:
     """The reference's vendored weights (models/i3d/checkpoints/i3d_{rgb,flow}.pt, models/raft/checkpoints/
-    raft-sintel.pth), looked up in $VF_CKPT_DIR or ./checkpoints; read from disk once per process."""
+    raft-sintel.pth, models/pwc/checkpoints/pwc_net_sintel.pt), looked up in $VF_CKPT_DIR or ./checkpoints; read from disk once per process."""
     if kind not in _STATE_DICTS:
         for d in _CKPT_DIRS:
             if d and os.path.exists(os.path.join(d, _CKPT[kind])):
@@ -87,9 +89,9 @@ class ExtractI3D(torch.nn.Module):
         if external_call is False:
             self.output_direct = args.output_direct
             self.output_path = args.output_path if self.output_direct is True else os.path.join(args.output_path, self.feature_type)
-        if 'flow' in self.streams and self.flow_type not in ('raft', 'flow'):
-            raise NotImplementedError(f"flow_type '{self.flow_type}': the RAFT and pre-computed flow branches are built "
-                                      "on the H100 engine (pass --flow_type raft / flow, or --streams rgb)")
+        if 'flow' in self.streams and self.flow_type not in ('pwc', 'raft', 'flow'):
+            raise NotImplementedError(f"flow_type '{self.flow_type}': the PWC, RAFT and pre-computed flow branches are "
+                                      "built on the H100 engine")
         self.progress = tqdm(total=len(self.path_list))
         self.group_stacks = max(1, int(os.environ.get("VF_I3D_STACKS", "8")))     # stacks per engine call
         self.keep_features = False
@@ -102,7 +104,8 @@ class ExtractI3D(torch.nn.Module):
         if idx not in self._models:
             m = {s: I3DEngine(load_checkpoint(s), s, idx, max_stacks=self.group_stacks, max_T=max(self.stack_size, 16))
                  for s in self.streams}
-            self._models[idx] = {'i3d': m, 'raft': None, 'raft_cap': (0, 0, 0), 'device_index': idx}
+            self._models[idx] = {'i3d': m, 'raft': None, 'raft_cap': (0, 0, 0), 'pwc': None, 'pwc_cap': (0, 0, 0),
+                                 'device_index': idx}
         return self._models[idx]
 
     @staticmethod
@@ -118,6 +121,19 @@ class ExtractI3D(torch.nn.Module):
                                         max_w=cap[2])
             models['raft_cap'] = cap
         return models['raft']
+
+    @staticmethod
+    def _pwc(models: dict, frames: int, h: int, w: int) -> PWCEngine:
+        """The PWC-Net engine of this device, re-created like the RAFT engine (_raft) when a video outgrows it."""
+        cf, ch, cw = models['pwc_cap']
+        if models['pwc'] is None or frames > cf or h > ch or w > cw:
+            if models['pwc'] is not None:
+                models['pwc'].close()
+            cap = (max(cf, frames), max(ch, h), max(cw, w))
+            models['pwc'] = PWCEngine(load_checkpoint('pwc'), models['device_index'], max_frames=cap[0], max_h=cap[1],
+                                      max_w=cap[2])
+            models['pwc_cap'] = cap
+        return models['pwc']
 
     def forward(self, indices: torch.LongTensor):
         device = indices.device
@@ -182,6 +198,10 @@ class ExtractI3D(torch.nn.Module):
             elif stream == 'flow':
                 if flow_stacks is not None:                                        # --flow_type flow: jpg pairs
                     flow = flow_stacks
+                elif self.flow_type == 'pwc':
+                    # the stack's BGR frames as the reference passes them (extract_i3d.py:175), flow at the frame size
+                    pwc = self._pwc(models, span, x.shape[1], x.shape[2])
+                    flow = torch.stack([pwc.flow(x[s:s + span]) for s in starts])
                 else:
                     raft = self._raft(models, span, x.shape[1], x.shape[2])
                     # padded flow, never unpadded, as the reference feeds it (extract_i3d.py:172)

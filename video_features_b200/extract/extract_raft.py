@@ -81,9 +81,16 @@ class ExtractRAFT(torch.nn.Module):
             if eng is not None:
                 eng.close()
             cap = (self.pairs_per_call + 1, max(cap[1], h), max(cap[2], w))
-            eng = RAFTEngine(load_checkpoint('raft'), idx, max_frames=cap[0], max_h=cap[1], max_w=cap[2])
+            eng = self._new_engine(idx, cap)
             self._engines[idx] = (eng, cap)
         return eng
+
+    def _new_engine(self, idx: int, cap: tuple):
+        return RAFTEngine(load_checkpoint('raft'), idx, max_frames=cap[0], max_h=cap[1], max_w=cap[2])
+
+    def _flow_of_frames(self, x: torch.Tensor, device) -> torch.Tensor:
+        """x: (n+1, H, W, 3) uint8 RGB frames on the device -> (n, 2, H, W) fp32 flow."""
+        return self._engine(device, x.shape[1], x.shape[2]).flow(x, iters=20, unpad=True)
 
     def _flow_of_window(self, window, device) -> list:
         """window: n+1 RGB frames (H, W, 3) uint8 -> [one (n, 2, H, W) float64 array]."""
@@ -94,7 +101,7 @@ class ExtractRAFT(torch.nn.Module):
                 x = torch.ops.vfeat.resize_u8(x, oh, ow, VF_FILTER_BILINEAR)
         # float64 (T, 2, H, W) on the host: the same values `.tolist()` -> np.array gives the reference, without
         # materialising 8 bytes + a Python float object per flow component
-        return [self._engine(device, x.shape[1], x.shape[2]).flow(x, iters=20, unpad=True).cpu().numpy().astype(np.float64)]
+        return [self._flow_of_frames(x, device).cpu().numpy().astype(np.float64)]
 
     def extract(self, device, model, video_path=None) -> Dict[str, np.ndarray]:
         import cv2
