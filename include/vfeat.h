@@ -322,6 +322,35 @@ int64_t vf_r21d_launch_count(const vf_r21d_t* h);
  * padded to a multiple of 8. */
 int vf_r21d_conv(const vf_r21d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
+/* ---- CLIP ResNet image towers (openai/CLIP ModifiedResNet: RN50, RN101, RN50x4, RN50x16): replaces
+ * `clip.load("RN50" | ...)` and `model.encode_image(preprocess(frame))` (models/CLIP/extract_clip.py:45-64) with its
+ * transform Resize(n_px, bicubic) -> CenterCrop(n_px) -> ToTensor -> Normalize.  Weights: openai's `visual.*` keys,
+ * HOST fp32 (other keys are ignored).  Width, stage depths, resolution n_px, heads and output width are inferred from
+ * the sizes as clip.model.build_model does; a missing / mis-sized tensor is VF_ERR_INVALID naming the key. */
+typedef struct vf_clip_rn vf_clip_rn_t;
+
+/* Workspace holds max_frames frames (0 = 64 at n_px 224, 32 at 288, 16 above); larger calls run in chunks. */
+int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_frames);
+int vf_clip_rn_destroy(vf_clip_rn_t* h);
+/* info receives 11 ints: out_dim, n_px, width, embed dim, heads, tokens (HW + 1), max_frames, blocks of layer1..4. */
+int vf_clip_rn_info(const vf_clip_rn_t* h, int* info);
+/* frames: n x 3 x n_px x n_px fp32 on the device, already transformed -> out: n x out_dim fp32 on the device. */
+int vf_clip_rn_encode_f32(vf_clip_rn_t* h, const float* frames, int n, float* out, void* stream);
+/* transform fused: frames n x H x W x 3 uint8 on the device, any size, channel order untouched (the reference feeds the
+ * decoder's BGR frame as it is) -> Pillow-exact bicubic resize of the short side to n_px, CenterCrop(n_px), ToTensor,
+ * Normalize -> tower.  Bit-identical to vf_clip_rn_encode_f32 on the same transformed frames. */
+int vf_clip_rn_encode_u8(vf_clip_rn_t* h, const uint8_t* frames, int n, int H, int W, float* out, void* stream);
+/* Diagnostics: an activation of the last chunk of the last call as fp32 NCHW: stage 0 stem (conv3 + bn3 + relu, before
+ * the pool), 1..4 layer1..layer4, 5 the attention-pool tokens (n, E, T, 1: mean first, positional embedding added),
+ * 6 the attention output before c_proj (n, E, 1, 1).  dims4 receives the shape; out == NULL only queries it. */
+int vf_clip_rn_read_stage(vf_clip_rn_t* h, int stage, float* out, int64_t capacity, int* dims4, void* stream);
+int64_t vf_clip_rn_launch_count(const vf_clip_rn_t* h);
+/* Diagnostics: conv `index` as uploaded, in execution order: the stem's conv1, conv2, conv3, then per block conv1,
+ * conv2, conv3, the downsample if any, then the attention pool's q_proj, k|v (one projection of 2E outputs) and c_proj
+ * (linears: one tap, scale 1, the bias).  Same contract as vf_resnet_conv; a pooled 1x1 conv carries its weight in all
+ * four phase slots and 1/4 in its scale. */
+int vf_clip_rn_conv(const vf_clip_rn_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+
 #ifdef __cplusplus
 }
 #endif

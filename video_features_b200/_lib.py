@@ -135,6 +135,15 @@ SIGNATURES = {
     "vf_r21d_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_r21d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                                C.c_void_p, C.c_void_p]),
+    "vf_clip_rn_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
+    "vf_clip_rn_destroy": (C.c_int, [C.c_void_p]),
+    "vf_clip_rn_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "vf_clip_rn_encode_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_rn_encode_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_rn_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_clip_rn_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_clip_rn_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
     "vf_clip_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "vf_clip_profile_categories": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
     "vf_clip_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
@@ -167,7 +176,8 @@ def check(status: int) -> None:
 
 
 def read_conv(fn, handle, index: int, device):
-    """Diagnostics shared by ResNetEngine.conv / R21DEngine.conv: fn is vf_resnet_conv or vf_r21d_conv.  Returns dict
+    """Diagnostics shared by ResNetEngine.conv / R21DEngine.conv / ClipResNetEngine.conv: fn is vf_resnet_conv,
+    vf_r21d_conv or vf_clip_rn_conv.  Returns dict
     n_out, ntaps, k_per_tap, shifts [(dt, dh, dw)] per tap, lo_mask, w (fp16 [n_out, 2 ntaps k_per_tap], W_hi | W_lo),
     scale, bias (fp32 [n_out]) as uploaded."""
     import torch

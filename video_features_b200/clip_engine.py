@@ -41,6 +41,7 @@ class ClipEngine:
         if not torch.cuda.is_available():
             raise RuntimeError("ClipEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
+        self.out_dim = 512
         keep = []     # keep numpy arrays alive across the create call
         if "visual.conv1.weight" not in state_dict:
             raise KeyError("CLIP checkpoint is missing 'visual.conv1.weight'")

@@ -1,0 +1,151 @@
+"""CLIP ResNet image tower handle (RN50, RN101, RN50x4, RN50x16): stands where the reference keeps the result of
+``clip.load("RN50" | "RN101" | "RN50x4" | "RN50x16", device)`` (models/CLIP/extract_clip.py:45-64), ``preprocess`` and
+``encode_image`` included.  It offers the methods ``ExtractCLIP`` calls on its model."""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Dict, Optional
+
+import numpy as np
+import torch
+
+from ._lib import NamedTensor, check, lib, read_conv
+
+STAGES = ("stem", "layer1", "layer2", "layer3", "layer4", "tokens", "pre_cproj")     # vf_clip_rn_read_stage ids
+
+
+class ClipResNetEngine:
+    """``state_dict``: openai's ``visual.*`` keys (a full CLIP state dict or a JIT archive's ``state_dict()``; other keys
+    are ignored), any float dtype.  The configuration is inferred from the sizes.  ``max_frames``: frames per internal
+    chunk (0: the tower's default); larger calls are chunked inside the call."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, max_frames: int = 0):
+        if not torch.cuda.is_available():
+            raise RuntimeError("ClipResNetEngine needs a CUDA device (sm_90a); there is no CPU fallback")
+        self.device = torch.device("cuda", device)
+        keep = []
+        items = [(k, v) for k, v in state_dict.items()
+                 if k.startswith("visual.") and torch.is_tensor(v) and v.dtype.is_floating_point]
+        arr = (NamedTensor * max(len(items), 1))()
+        for i, (k, v) in enumerate(items):
+            a = np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
+            nm = k.encode()
+            keep.append((a, nm))
+            arr[i].name = nm
+            arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
+            arr[i].numel = a.size
+        h = C.c_void_p()
+        check(lib().vf_clip_rn_create(C.byref(h), arr, len(items), device, max_frames))
+        self._h = h
+        del keep
+        info = (C.c_int * 11)()
+        check(lib().vf_clip_rn_info(self._h, info))
+        (self.out_dim, self.n_px, self.width, self.embed, self.heads, self.tokens,
+         self.max_frames) = list(info)[:7]
+        self.layers = tuple(info[7:11])
+        self._events = {}
+        self._next_ticket = 0
+
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def encode_image(self, frames: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """frames: (n, 3, n_px, n_px), already transformed, on this device -> (n, out_dim) fp32 on this device."""
+        if not frames.is_cuda:
+            raise RuntimeError("ClipResNetEngine expects CUDA input (no CPU fallback)")
+        frames = frames.to(torch.float32).contiguous()
+        assert frames.dim() == 4 and tuple(frames.shape[1:]) == (3, self.n_px, self.n_px), frames.shape
+        n = frames.shape[0]
+        if out is None:
+            out = torch.empty((n, self.out_dim), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_rn_encode_f32(self._h, frames.data_ptr(), n, out.data_ptr(), self._stream()))
+        return out
+
+    def encode_frames_u8(self, frames: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """frames: (n, H, W, 3) uint8 on this device, any size, decoder channel order -> (n, out_dim) fp32 on this
+        device; the bicubic resize, centre crop and normalisation are fused.  Asynchronous on the current stream."""
+        if not frames.is_cuda:
+            raise RuntimeError("ClipResNetEngine expects CUDA frames (no CPU fallback)")
+        assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3, frames.shape
+        frames = frames.contiguous()
+        n, hh, ww, _ = frames.shape
+        if out is None:
+            out = torch.empty((n, self.out_dim), device=self.device, dtype=torch.float32)
+        assert out.is_cuda and out.is_contiguous() and tuple(out.shape) == (n, self.out_dim) and out.dtype == torch.float32
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_rn_encode_u8(self._h, frames.data_ptr(), n, hh, ww, out.data_ptr(), self._stream()))
+        return out
+
+    def encode_frames_u8_host(self, frames, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Host uint8 frames (numpy or CPU tensor, (n, H, W, 3)) -> (n, out_dim) fp32 on the host, synchronous."""
+        if isinstance(frames, np.ndarray):
+            frames = torch.from_numpy(np.ascontiguousarray(frames))
+        assert (not frames.is_cuda) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+        with torch.cuda.device(self.device):
+            dev = self.encode_frames_u8(frames.contiguous().to(self.device))
+            if out is None:
+                return dev.cpu()
+            out.copy_(dev)
+        return out
+
+    def encode_frames_u8_host_async(self, frames: torch.Tensor, out_host: Optional[torch.Tensor] = None,
+                                    out_dev: bool = False):
+        """Pinned host frames in; features to ``out_host`` (pinned) and / or a new device tensor (``out_dev=True``).
+        Returns ``(ticket, device tensor or None)``; ``frames`` and ``out_host`` belong to the engine until
+        ``wait(ticket)``.  The copies and the tower are enqueued on the current stream."""
+        assert (not frames.is_cuda) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+        assert frames.is_contiguous() and frames.is_pinned(), "asynchronous calls need pinned, contiguous host frames"
+        n = frames.shape[0]
+        if out_host is not None:
+            assert out_host.dtype == torch.float32 and out_host.is_contiguous() and tuple(out_host.shape) == (n, self.out_dim)
+            assert out_host.is_pinned(), "asynchronous calls need a pinned host output"
+        assert out_host is not None or out_dev
+        with torch.cuda.device(self.device):
+            dev = self.encode_frames_u8(frames.to(self.device, non_blocking=True))
+            if out_host is not None:
+                out_host.copy_(dev, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record()
+        ticket = self._next_ticket
+        self._next_ticket += 1
+        self._events[ticket] = ev
+        return ticket, (dev if out_dev else None)
+
+    def wait(self, ticket: int) -> None:
+        """Block until the asynchronous call `ticket` has finished with its host buffers."""
+        self._events.pop(int(ticket)).synchronize()
+
+    def read_stage(self, stage: int) -> torch.Tensor:
+        """Diagnostics: of the last chunk of the last call, fp32: 0 stem, 1..4 layer1..4 (n, C, H, W), 5 the
+        attention-pool tokens (n, T, E), 6 the attention output before c_proj (n, E)."""
+        dims = (C.c_int * 4)()
+        check(lib().vf_clip_rn_read_stage(self._h, stage, None, 0, dims, None))
+        out = torch.empty(tuple(dims), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_rn_read_stage(self._h, stage, out.data_ptr(), out.numel(), dims, self._stream()))
+        if stage == 5:
+            return out[..., 0].transpose(1, 2).contiguous()
+        if stage == 6:
+            return out[:, :, 0, 0]
+        return out
+
+    def conv(self, index: int) -> dict:
+        """Diagnostics: conv ``index`` as uploaded, in execution order (include/vfeat.h vf_clip_rn_conv)."""
+        with torch.cuda.device(self.device):
+            return read_conv(lib().vf_clip_rn_conv, self._h, index, self.device)
+
+    @property
+    def launch_count(self) -> int:
+        return int(lib().vf_clip_rn_launch_count(self._h))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().vf_clip_rn_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

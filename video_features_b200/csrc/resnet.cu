@@ -28,16 +28,9 @@
 
 #include "internal.h"
 #include "resnet_kernels.h"
+#include "split_conv.h"
 
 namespace vf {
-
-struct ResConv {
-    int n_out = 0, ntaps = 0, k_per_tap = 0;
-    int dh[4] = {0, 0, 0, 0}, dw[4] = {0, 0, 0, 0};   // per tap: shift in volume rows / columns
-    unsigned long long lo_mask = 0;
-    __half* w = nullptr;       // [n_out][2 * ntaps * k_per_tap]: hi pass | lo pass
-    float *scale = nullptr, *bias = nullptr;
-};
 
 struct ResBlock {
     int cin = 0, width = 0, cout = 0, stride = 1;
@@ -49,17 +42,15 @@ struct ResBlock {
 
 using namespace vf;
 
-struct vf_resnet {
+struct vf_resnet : vf::ConvHost {
     int device = 0, depth = 0, max_frames = 0, out_dim = 0;
     bool bottleneck = false;
     int nblocks[4] = {0, 0, 0, 0}, cout[4] = {0, 0, 0, 0};
-    std::vector<void*> allocs;
     ResConv stem;
     std::vector<ResBlock> blocks;
     // workspace: s0 = stem phase volume; stage outputs are kept for vf_resnet_read_stage
     __half *s0 = nullptr, *stem_out = nullptr, *pool_out = nullptr, *stage_out[4] = {nullptr, nullptr, nullptr, nullptr};
     __half *bufA = nullptr, *bufB = nullptr, *t1 = nullptr, *t2 = nullptr, *ds = nullptr, *ph1 = nullptr, *ph2 = nullptr;
-    int64_t launches = 0;
     cudaStream_t cs = nullptr;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
     bool use_graph = true;
@@ -75,122 +66,6 @@ static const int kSide[4] = {56, 28, 14, 7};
 static Vol2 stem_vol(int n) { return Vol2{n, kStemQ, kStemQ, 2, 114, 2, 114}; }
 static Vol2 stage_vol(int n, int L) { return Vol2{n, kSide[L] + 2, kSide[L] + 2, 1, kSide[L] + 1, 1, kSide[L] + 1}; }
 
-template <typename Tp>
-static int ralloc(vf_resnet* h, Tp** p, size_t count) {
-    // + 64 KB: the overlapping-row TMA view of a conv input extends up to (k_per_tap - C) elements past its last row;
-    // zero-filled so that those elements are finite (they only feed masked border rows)
-    void* q = nullptr;
-    const size_t bytes = count * sizeof(Tp) + 65536;
-    cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "cudaMalloc(%zu bytes): %s", bytes, cudaGetErrorString(e));
-    h->allocs.push_back(q);
-    VF_CUDA(cudaMemset(q, 0, bytes));
-    *p = static_cast<Tp*>(q);
-    return VF_OK;
-}
-
-// torchvision state_dict lookup by key, with or without the "module." prefix of a DataParallel checkpoint
-struct ResTensors {
-    const vf_named_tensor* t; int n;
-    int get(const std::string& name, int64_t numel, const float** out) const {
-        for (int i = 0; i < n; ++i) {
-            const char* k = t[i].name;
-            if (!k || !(name == k || (strncmp(k, "module.", 7) == 0 && name == k + 7))) continue;
-            if (!t[i].data || t[i].numel != numel)
-                return fail(VF_ERR_INVALID, "resnet_create: tensor '%s' has %lld elements, expected %lld", name.c_str(),
-                            (long long)t[i].numel, (long long)numel);
-            *out = t[i].data;
-            return VF_OK;
-        }
-        return fail(VF_ERR_INVALID, "resnet_create: missing tensor '%s'", name.c_str());
-    }
-};
-
-// eval BatchNorm (eps 1e-5) as y = x * scale + shift, folded in double
-static int bn_fold(const ResTensors& T, const std::string& p, int c, std::vector<float>& sc, std::vector<float>& sh) {
-    const float *g, *b, *m, *v;
-    VF_TRY(T.get(p + ".weight", c, &g)); VF_TRY(T.get(p + ".bias", c, &b));
-    VF_TRY(T.get(p + ".running_mean", c, &m)); VF_TRY(T.get(p + ".running_var", c, &v));
-    sc.resize(c); sh.resize(c);
-    for (int i = 0; i < c; ++i) {
-        const double s = double(g[i]) / sqrt(double(v[i]) + 1e-5);
-        sc[i] = float(s);
-        sh[i] = float(double(b[i]) - double(m[i]) * s);
-    }
-    return VF_OK;
-}
-
-// Uploads conv `name` (weight [co][ci][k][k], no bias) followed by BatchNorm `bn` as a hi + lo weight pair.
-// col(kh, kw, c) -> K column of the activation's hi half; its lo half sits lo_off columns further and gets the same
-// weight.  cw.ntaps / k_per_tap / dh / dw must be set.
-static int upload_conv(vf_resnet* h, ResConv& cw, const ResTensors& T, const std::string& name, const std::string& bn,
-                       int co, int ci, int k, int lo_off, const std::function<int(int, int, int)>& col) {
-    const float* w;
-    VF_TRY(T.get(name + ".weight", int64_t(co) * ci * k * k, &w));
-    std::vector<float> sc, sh;
-    VF_TRY(bn_fold(T, bn, co, sc, sh));
-    const int Ktot = cw.ntaps * cw.k_per_tap;
-    const size_t Kall = size_t(2) * Ktot;
-    std::vector<__half> B(size_t(co) * Kall, __float2half_rn(0.f));
-    std::vector<char> has_hi(size_t(Ktot), 0);
-    for (int o = 0; o < co; ++o)
-        for (int c = 0; c < ci; ++c)
-            for (int a = 0; a < k; ++a)
-                for (int d = 0; d < k; ++d) {
-                    const int kc = col(a, d, c);
-                    if (kc < 0 || kc + lo_off >= Ktot) return fail(VF_ERR_INVALID, "resnet_create: filter column out of range");
-                    const float wf = w[((size_t(o) * ci + c) * k + a) * k + d];
-                    const __half wh = __float2half_rn(wf), wl = __float2half_rn(wf - __half2float(wh));
-                    for (int kk : {kc, kc + lo_off}) {
-                        B[size_t(o) * Kall + kk] = wh;
-                        B[size_t(o) * Kall + Ktot + kk] = wl;
-                    }
-                    has_hi[kc] = 1;
-                }
-    cw.n_out = co;
-    // a K block none of whose columns meets a hi half needs only the W_hi pass (a_lo . w_lo < 2^-22 of the product)
-    cw.lo_mask = 0;
-    const int kpt_blocks = (cw.k_per_tap + 63) / 64;
-    if (kpt_blocks <= 64) {
-        unsigned long long m = ~0ull;
-        for (int t = 0; t < cw.ntaps; ++t)
-            for (int kk = 0; kk < kpt_blocks; ++kk)
-                for (int j = kk * 64; j < (kk + 1) * 64 && j < cw.k_per_tap; ++j)
-                    if (has_hi[size_t(t) * cw.k_per_tap + j]) { m &= ~(1ull << kk); break; }
-        cw.lo_mask = kpt_blocks == 64 ? m : (m & ((1ull << kpt_blocks) - 1));
-    }
-    VF_TRY(ralloc(h, &cw.w, B.size()));
-    VF_TRY(ralloc(h, &cw.scale, size_t(co)));
-    VF_TRY(ralloc(h, &cw.bias, size_t(co)));
-    VF_CUDA(cudaMemcpy(cw.w, B.data(), B.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    VF_CUDA(cudaMemcpy(cw.scale, sc.data(), co * sizeof(float), cudaMemcpyHostToDevice));
-    VF_CUDA(cudaMemcpy(cw.bias, sh.data(), co * sizeof(float), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-
-// stride-1 k x k (k = 1 or 3, pad k/2) on split rows of 2*ci: one tap per kernel row of k * 2ci contiguous elements.
-// Also the stride-2 1x1 downsample: one tap reading phase (0, 0) = the first 2*ci elements of a phase row.
-static int prep_same(vf_resnet* h, ResConv& cw, const ResTensors& T, const std::string& name, const std::string& bn,
-                     int co, int ci, int k) {
-    cw.ntaps = k; cw.k_per_tap = k * 2 * ci;
-    for (int a = 0; a < k; ++a) { cw.dh[a] = a - k / 2; cw.dw[a] = -(k / 2); }
-    const int kpt = cw.k_per_tap;
-    return upload_conv(h, cw, T, name, bn, co, ci, k, ci, [=](int a, int d, int c) { return a * kpt + d * 2 * ci + c; });
-}
-
-// stride-2 3x3 (pad 1) on the phase repack of split rows of 2*ci: phase row q holds x[2(q-1)+p]; tap (a, b) reads
-// phase row (q + a - 1, q' + b - 1), filter index kh = 2a + ph - 1 (likewise kw with b, pw).
-static int prep_stride2(vf_resnet* h, ResConv& cw, const ResTensors& T, const std::string& name, const std::string& bn,
-                        int co, int ci) {
-    cw.ntaps = 4; cw.k_per_tap = 8 * ci;
-    for (int t = 0; t < 4; ++t) { cw.dh[t] = t / 2 - 1; cw.dw[t] = t % 2 - 1; }
-    const int kpt = cw.k_per_tap;
-    return upload_conv(h, cw, T, name, bn, co, ci, 3, ci, [=](int kh, int kw, int c) {
-        const int a = (kh + 1) / 2, ph = (kh + 1) % 2, b = (kw + 1) / 2, pw = (kw + 1) % 2;
-        return (a * 2 + b) * kpt + (ph * 2 + pw) * 2 * ci + c;
-    });
-}
-
 // stem 7x7/2 pad 3 on the phase volume of the transform (rows [16 hi | 16 lo], 4 channels per phase, 3 used):
 // phase row q holds x[2(q-2)+p]; 4 taps (kernel row pairs), each a run of 4 phase positions x 32 elements.
 static int prep_stem(vf_resnet* h, ResConv& cw, const ResTensors& T) {
@@ -200,24 +75,6 @@ static int prep_stem(vf_resnet* h, ResConv& cw, const ResTensors& T) {
         const int a = (kh + 1) / 2, ph = (kh + 1) % 2, b = (kw + 1) / 2, pw = (kw + 1) % 2;
         return a * 128 + b * 32 + (ph * 2 + pw) * 4 + c;
     });
-}
-
-// one conv over the volume v (rows of `pitch` elements in X) -> split rows of 2*n_out in `out`, rows outside the
-// valid region zeroed
-static int run_conv(vf_resnet* h, const ResConv& cw, const __half* X, int pitch, const Vol2& v, __half* out, bool relu,
-                    cudaStream_t s) {
-    ConvGeom g;
-    memset(&g, 0, sizeof(g));
-    g.ntaps = cw.ntaps; g.k_per_tap = cw.k_per_tap; g.nsplit = 2; g.lo_mask = cw.lo_mask;
-    for (int j = 0; j < cw.ntaps; ++j) g.tap_off[j] = cw.dh[j] * v.Wp + cw.dw[j];
-    g.mask = 1; g.row0 = 0;
-    g.Tp = 1; g.Hp = v.Hp; g.Wp = v.Wp; g.t0 = 0; g.t1 = 1; g.h0 = v.h0; g.h1 = v.h1; g.w0 = v.w0; g.w1 = v.w1;
-    GemmEpi ep;
-    memset(&ep, 0, sizeof(ep));
-    ep.out = out; ep.ldo = 2 * cw.n_out; ep.out_f32 = 0; ep.bias = cw.bias; ep.scale = cw.scale;
-    ep.act = relu ? VF_ACT_RELU : VF_ACT_NONE; ep.split_off = cw.n_out;
-    h->launches += 1;
-    return conv_gemm_f16(X, pitch, v.rows(), cw.w, cw.n_out, g, ep, s);
 }
 
 // torchvision BasicBlock / Bottleneck (v1.5: the stride sits on the 3x3): x (valid region vi, cin channels) ->
@@ -309,8 +166,9 @@ int vf_resnet_create(vf_resnet_t** out, const vf_named_tensor* tensors, int n_te
     if (major != 9 || minor != 0)
         return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
     vf_resnet* h = new vf_resnet();
+    h->who = "resnet_create";
     h->device = device; h->depth = depth; h->max_frames = max_frames; h->bottleneck = bottleneck;
-    const ResTensors T{tensors, n_tensors};
+    const ResTensors T{tensors, n_tensors, "resnet_create"};
     auto body = [&]() -> int {
         VF_TRY(prep_stem(h, h->stem, T));
         // per-frame element counts of the working buffers, found while walking the blocks
@@ -482,16 +340,7 @@ int vf_resnet_conv(const vf_resnet_t* h, int index, int* geom, uint64_t* lo_mask
     }
     if (index < 0 || index >= int(cs.size()))
         return fail(VF_ERR_INVALID, "resnet_conv: index %d outside the %d convs", index, int(cs.size()));
-    const ResConv& c = *cs[index];
-    geom[0] = c.n_out; geom[1] = c.ntaps; geom[2] = c.k_per_tap;
-    for (int j = 0; j < 4; ++j) { geom[3 + 3 * j] = 0; geom[4 + 3 * j] = c.dh[j]; geom[5 + 3 * j] = c.dw[j]; }
-    *lo_mask = c.lo_mask;
-    VF_CUDA(cudaSetDevice(h->device));
-    const size_t nw = size_t(c.n_out) * 2 * c.ntaps * c.k_per_tap;
-    if (w) VF_CUDA(cudaMemcpy(w, c.w, nw * sizeof(__half), cudaMemcpyDeviceToDevice));
-    if (scale) VF_CUDA(cudaMemcpy(scale, c.scale, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
-    if (bias) VF_CUDA(cudaMemcpy(bias, c.bias, size_t(c.n_out) * sizeof(float), cudaMemcpyDeviceToDevice));
-    return VF_OK;
+    return read_back_conv(h->device, *cs[index], geom, lo_mask, w, scale, bias);
 }
 
 }  // extern "C"

@@ -3,7 +3,9 @@
 Same constructor, attributes, ``forward(indices)`` / ``extract(...)`` signatures, dict keys and file naming.  What
 changes underneath: ``clip.load`` is replaced by a ``ClipEngine`` (device weights + workspace), and ``preprocess`` +
 ``model.encode_image`` by ONE call into libvfeat.so that takes the decoder's raw uint8 frames and runs the
-Pillow-exact bicubic resize, centre crop, normalisation and the ViT-B/32 tower on the GPU.
+Pillow-exact bicubic resize, centre crop, normalisation and the ViT-B/32 tower on the GPU.  The ResNet towers
+(``CLIP-RN50``, ``CLIP-RN101``, ``CLIP-RN50x4``, ``CLIP-RN50x16``) run on a ``ClipResNetEngine`` behind the same
+calls, at their own input size (224, 224, 288, 384) and output width (1024, 512, 640, 768).
 
 A list of videos does not go through the engine one 12-frame video at a time (600 token rows would fill 3 of the
 GEMM's 74 tile slots): ``forward`` decodes ahead on a thread pool, packs the frames of consecutive videos of equal
@@ -34,10 +36,14 @@ from tqdm import tqdm
 
 from .. import synthetic_weights
 from ..clip_engine import ClipEngine
+from ..clip_resnet_engine import ClipResNetEngine
 from ..utils import (AsyncSink, FrameStream, action_on_extraction, already_extracted, extract_frames,
                      form_list_from_user_input)
 
-_CKPT_NAMES = {'CLIP-ViT-B/32': 'ViT-B-32.pt', 'CLIP-ViT-B/16': 'ViT-B-16.pt', 'CLIP4CLIP-ViT-B-32': 'CLIP4CLIP-ViT-B-32.pth'}
+# the ResNet towers' names are the basenames clip.load caches its downloads under
+_RN_CKPT_NAMES = {'CLIP-RN50': 'RN50.pt', 'CLIP-RN101': 'RN101.pt', 'CLIP-RN50x4': 'RN50x4.pt', 'CLIP-RN50x16': 'RN50x16.pt'}
+_CKPT_NAMES = {'CLIP-ViT-B/32': 'ViT-B-32.pt', 'CLIP-ViT-B/16': 'ViT-B-16.pt', 'CLIP4CLIP-ViT-B-32': 'CLIP4CLIP-ViT-B-32.pth',
+               **_RN_CKPT_NAMES}
 
 
 def read_clip_checkpoint(path: str) -> Dict[str, torch.Tensor]:
@@ -57,8 +63,9 @@ def read_clip_checkpoint(path: str) -> Dict[str, torch.Tensor]:
 def load_clip_state_dict(feature_type: str) -> Dict[str, torch.Tensor]:
     """``$VF_CLIP_CKPT``, then ``<this dir>/checkpoints/<name>`` (where the reference keeps CLIP4CLIP's file,
     extract_clip.py:56), then ``~/.cache/clip/<name>`` (where ``clip.load`` caches its download).
-    ``VF_CLIP_SYNTHETIC=<seed>[:outliers]`` selects seeded synthetic weights instead (benchmarks without the file)."""
-    if os.environ.get("VF_CLIP_SYNTHETIC") is not None:
+    ``VF_CLIP_SYNTHETIC=<seed>[:outliers]`` selects seeded synthetic ViT weights instead (benchmarks without the file);
+    it does not apply to the ResNet towers."""
+    if os.environ.get("VF_CLIP_SYNTHETIC") is not None and feature_type not in _RN_CKPT_NAMES:
         seed, outliers = synthetic_weights.parse_env(os.environ["VF_CLIP_SYNTHETIC"])
         return synthetic_weights.clip_vit_b32_state_dict(seed, outliers, patch=16 if feature_type.endswith('/16') else 32)
     name = _CKPT_NAMES[feature_type]
@@ -120,7 +127,7 @@ class ExtractCLIP(torch.nn.Module):
             self.output_direct = args.output_direct
             self.output_path = args.output_path if self.output_direct is True else os.path.join(args.output_path, self.feature_type)
         self.progress = tqdm(total=len(self.path_list))
-        self._engines: Dict[int, ClipEngine] = {}
+        self._engines: Dict[int, object] = {}             # ClipEngine or ClipResNetEngine
         # engine-side knobs (not in the reference): where frames come from, and how many go into one engine call
         self.frame_source = extract_frames                  # (path, method) -> (frames, fps, timestamps_ms)
         # two-step source used by the list path: stream = frame_stream(path, method) knows .count / .hw / .fps /
@@ -137,17 +144,19 @@ class ExtractCLIP(torch.nn.Module):
         # seconds the stages of the last batched forward spent waiting on each other (diagnostics: which side is the limiter)
         self.stage_wait = {"engine_for_decode": 0.0, "engine_enqueue": 0.0, "host_for_slot": 0.0, "deliver_for_gpu": 0.0}
 
-    def _engine(self, device: torch.device) -> ClipEngine:
+    def _engine(self, device: torch.device):
         if device.type != 'cuda':
             raise RuntimeError("the H100 engine has no CPU path: pass indices on a CUDA device "
                                "(the reference's --cpu flow is timed by bench.py --impl reference)")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if idx not in self._engines:
             if self.feature_type not in _CKPT_NAMES:
-                # the reference's clip.load would also take the ResNet towers (extract_clip.py:46-64); the ViT-B
-                # towers (patch 32: north_star; patch 16) are the ones built here
-                raise NotImplementedError(self.feature_type)
-            self._engines[idx] = ClipEngine(load_clip_state_dict(self.feature_type), device=idx)
+                raise NotImplementedError(self.feature_type)          # extract_clip.py:63-64
+            sd = load_clip_state_dict(self.feature_type)
+            if self.feature_type in _RN_CKPT_NAMES:
+                self._engines[idx] = ClipResNetEngine(sd, device=idx)
+            else:
+                self._engines[idx] = ClipEngine(sd, device=idx)
         return self._engines[idx]
 
     # ------------------------------------------------------------------ forward
@@ -230,7 +239,7 @@ class ExtractCLIP(torch.nn.Module):
                 out.append(err)
         return out
 
-    def _forward_batched(self, device, model: ClipEngine, todo, collected, sink):
+    def _forward_batched(self, device, model, todo, collected, sink):
         """Stages, each on its own thread(s), so the GPU never waits for Python:
              pool: open videos (blocks of 8)  ->  this thread: rows of a pinned staging slot are assigned in list order
              ->  pool: every stream decodes INTO its rows  ->  engine thread: ONE asynchronous engine call per
@@ -243,7 +252,7 @@ class ExtractCLIP(torch.nn.Module):
         n_slots = 3
         pinned: List[Optional[torch.Tensor]] = [None] * n_slots
         pinned_np: List[Optional[np.ndarray]] = [None] * n_slots
-        feats_out: List[Optional[torch.Tensor]] = [None] * n_slots            # pinned (batch_frames, 512) landing buffers
+        feats_out: List[Optional[torch.Tensor]] = [None] * n_slots            # pinned (batch_frames, out_dim) landing buffers
         busy = [None] * n_slots                                               # engine future still reading slot k
         delivered = []
         state = {"slot": 0, "batches": 0}
@@ -344,7 +353,7 @@ class ExtractCLIP(torch.nn.Module):
                     pinned[k] = pinned[k].pin_memory()
                 pinned_np[k] = pinned[k].numpy()
             if feats_out[k] is None:
-                feats_out[k] = torch.empty((self.batch_frames, 512), dtype=torch.float32)
+                feats_out[k] = torch.empty((self.batch_frames, getattr(model, 'out_dim', 512)), dtype=torch.float32)
                 if torch.cuda.is_available():
                     feats_out[k] = feats_out[k].pin_memory()
             first = state["batches"] == 0 and 0 < self.first_batch_frames < self.batch_frames
@@ -445,8 +454,8 @@ class ExtractCLIP(torch.nn.Module):
         self.progress.update()
 
     # ------------------------------------------------------------------ extract (one video)
-    def extract(self, device: torch.device, model: ClipEngine, preprocess_func=None, video_path=None):
-        """-> {feature_type: (T,512) float32, 'fps': (), 'timestamps_ms': (T,)}.  ``preprocess_func`` is accepted for
+    def extract(self, device: torch.device, model, preprocess_func=None, video_path=None):
+        """-> {feature_type: (T, out_dim) float32, 'fps': (), 'timestamps_ms': (T,)}.  ``preprocess_func`` is accepted for
         signature compatibility; the transform is fused into the engine call."""
         decoded, fps, stamps = self._decode(video_path)
         batch = torch.from_numpy(np.stack(decoded))         # (T,H,W,3) uint8, decoder channel order untouched
