@@ -155,6 +155,25 @@ int vf_clip_wait(vf_clip_t* h, int64_t ticket);
  * ResidualAttentionBlock.attention / nn.MultiheadAttention).  fused = 1: the QKV-projection + attention kernel the tower
  * runs; fused = 0: QKV GEMM, then the stand-alone attention kernel. */
 int vf_clip_block_attention(vf_clip_t* h, int layer, const void* x, int n_frames, void* out, int fused, void* stream);
+/* Diagnostics / parity tests: the three pieces the tower consists of, one at a time.  They run the functions the encode
+ * calls run (eagerly, on the caller's stream, on the handle's first workspace; no CUDA graph is captured or replayed), take
+ * 1 <= n <= the handle's chunk_frames frames (VF_ERR_INVALID otherwise, before any launch), and must not overlap an
+ * asynchronous call in flight.  T = tokens per frame (50 / 197); all buffers are on the device.
+ *   embed:  patchify, the patch-embedding GEMM, class / positional embedding + ln_pre -> x_out, the fp32 residual stream
+ *           n*T x 768.  _f32 takes frames n x 3 x 224 x 224 as vf_clip_encode_f32 does, _u8 frames n x src_h x src_w x 3
+ *           as vf_clip_encode_u8 does.
+ *   blocks: resblocks [layer_begin, layer_end) of 0 .. 12 on the residual stream x (n_frames*T x 768 fp32, in place), by
+ *           the handle's configured path (fused or split attention; VF_CLIP_RESID=acc|y|mix).  When layer_end == 12 the
+ *           last block runs on the class-token rows only, as in the tower: afterwards only rows frame*T of x are defined.
+ *           In the y forms the MLP increment of block layer_end - 1, which the tower would add in the next LayerNorm
+ *           pass, is added to x (fp32) before returning, by the same add + LayerNorm kernel with its LayerNorm output
+ *           dropped: x holds the same fp32 values the next pass would have normalised.
+ *   head:   ln_post on rows frame*T of x (row pitch T*768) and the 768 -> 512 projection -> out, n_frames x 512 fp32.
+ * embed -> blocks(0, 12) -> head gives the bits of vf_clip_encode_f32 / _u8. */
+int vf_clip_debug_embed_f32(vf_clip_t* h, const float* frames, int n, float* x_out, void* stream);
+int vf_clip_debug_embed_u8(vf_clip_t* h, const uint8_t* frames, int n, int src_h, int src_w, float* x_out, void* stream);
+int vf_clip_debug_blocks(vf_clip_t* h, float* x, int n_frames, int layer_begin, int layer_end, void* stream);
+int vf_clip_debug_head(vf_clip_t* h, const float* x, int n_frames, float* out, void* stream);
 /* number of kernels this library has launched on behalf of `h` so far (diagnostics / bench). */
 int64_t vf_clip_launch_count(const vf_clip_t* h);
 /* Roofline instrumentation for bench.py: while enabled, every tensor-core GEMM launch of `h` is bracketed by a

@@ -1,4 +1,6 @@
-"""fp32 CPU restatement of the CLIP ViT image tower -- test oracle only.
+"""fp32 CPU restatement of the CLIP ViT image tower -- test oracle only -- and, below it, the same tower in any float
+dtype with the engine's declared fp16 rounding (``encode_image(..., dtype=torch.float64, declared_rounding=True)``, and its
+pieces ``embed`` / ``block`` / ``head``), what tests/test_clip_float64_gpu.py holds the engine to.
 
 The reference runs ``model.encode_image(frames)`` (models/CLIP/extract_clip.py:128)
 on a model returned by ``clip.load("ViT-B/32")`` (extract_clip.py:47).  ``clip`` is
@@ -108,13 +110,20 @@ def _attention(x: torch.Tensor, w_in, b_in, w_out, b_out) -> torch.Tensor:
 
 
 @torch.no_grad()
-def encode_image(sd: Dict[str, torch.Tensor], frames: torch.Tensor, *, return_hidden: bool = False):
+def encode_image(sd: Dict[str, torch.Tensor], frames: torch.Tensor, *, return_hidden: bool = False, dtype=None,
+                 declared_rounding: bool = False):
     """``CLIP.encode_image`` == ``VisionTransformer.forward``.
+
+    ``dtype`` (e.g. torch.float64) runs the restatement built from ``embed`` / ``block`` / ``head`` below in that dtype;
+    ``declared_rounding`` rounds to fp16 there exactly what the engine holds in fp16 (``DECLARED``).
 
     frames: (B,3,224,224) float, already normalised (output of the CLIP transform).
     returns (B,512) in the weight dtype.  No L2 normalisation (the reference saves
     the raw projection, extract_clip.py:128-131).
     """
+    if dtype is not None or declared_rounding:
+        assert not return_hidden
+        return encode_image_declared(sd, frames, dtype=dtype or torch.float64, declared_rounding=declared_rounding)
     w = sd["visual.conv1.weight"]
     x = frames.to(w.dtype)
     patch = w.shape[-1]                                          # 32 (ViT-B/32) or 16 (ViT-B/16): conv stride == kernel
@@ -136,6 +145,133 @@ def encode_image(sd: Dict[str, torch.Tensor], frames: torch.Tensor, *, return_hi
     x = _ln(x[:, 0, :], sd["visual.ln_post.weight"], sd["visual.ln_post.bias"])
     out = x @ sd["visual.proj"]
     return (out, hidden) if return_hidden else out
+
+
+# ---- the tower with the engine's declared rounding --------------------------------------------------------------
+# The tensors the engine (csrc/clip.cu) holds in fp16, read off its code; a reference that rounds exactly these to fp16
+# and keeps everything else (residual stream, LayerNorm statistics, scores, softmax sums, biases, positional embedding)
+# in float64 differs from the engine by fp32 accumulation order, intrinsic error and 1-ulp flips of those roundings.
+#   weights  conv1, in_proj, out_proj, c_fc, c_proj, proj                    (upload_f16)
+#   patches  the patch matrix = the transformed frames                       (clip_patchify_*_kernel)
+#   ln       the outputs of ln_1, ln_2 and ln_post (ln_pre writes the fp32 stream)   (add_layernorm768_kernel)
+#   qkv      q, k, v after the bias                                          (GEMM epilogue / qkv_attention_kernel staging)
+#   p        the softmax probabilities before P.V: normalised at 50 tokens (attention50_kernel, attention_unit),
+#            un-normalised exp(s - running max) in two key halves at 197 (attention_long_kernel, whose 1 / sum stays fp32)
+#   att      the attention output before the out-projection
+#   mlp      the MLP hidden layer after QuickGELU
+#   y_o/y_m  the out-projection's / c_proj's result as an fp16 increment: VF_CLIP_RESID=y (both) or mix (y_o) only
+# Two more names exist for the separation tests and are part of no engine path: resid (the residual stream after each
+# add) and scores (q k^T / 8).
+DECLARED = frozenset({"weights", "patches", "ln", "qkv", "p", "att", "mlp"})
+RESID_ROUNDING = {"acc": frozenset(), "mix": frozenset({"y_o"}), "y": frozenset({"y_o", "y_m"})}
+LONG_KEY_SPLIT = 112           # attention_long_kernel: 13 key tiles of 16, the first (13 + 1) / 2 = 7 in the first half
+
+
+def _r16(t: torch.Tensor) -> torch.Tensor:
+    return t.half().to(t.dtype)
+
+
+def _rounding(declared_rounding, rounding):
+    return frozenset(rounding) if rounding is not None else (DECLARED if declared_rounding else frozenset())
+
+
+def _rw(w: torch.Tensor, r, dtype) -> torch.Tensor:
+    w = w.to(dtype)
+    return _r16(w) if "weights" in r else w
+
+
+def _ln_d(x, w, b, eps):
+    mu = x.mean(-1, keepdim=True)
+    var = ((x - mu) ** 2).mean(-1, keepdim=True)
+    return (x - mu) / torch.sqrt(var + eps) * w.to(x.dtype) + b.to(x.dtype)
+
+
+def embed(sd, frames, *, dtype=torch.float64, declared_rounding=False, rounding=None, eps=LN_EPS):
+    """frames (B,3,224,224) -> the residual stream after ln_pre, (B, tokens, 768)."""
+    r = _rounding(declared_rounding, rounding)
+    w = _rw(sd["visual.conv1.weight"], r, dtype)
+    x = frames.to(dtype)
+    if "patches" in r:
+        x = _r16(x)
+    x = F.conv2d(x, w, None, stride=w.shape[-1])
+    x = x.reshape(x.shape[0], x.shape[1], -1).permute(0, 2, 1)
+    cls = sd["visual.class_embedding"].to(dtype).expand(x.shape[0], 1, -1)
+    x = torch.cat([cls, x], dim=1) + sd["visual.positional_embedding"].to(dtype)
+    return _ln_d(x, sd["visual.ln_pre.weight"], sd["visual.ln_pre.bias"], eps)
+
+
+def attention_core(qkv, *, rounding=DECLARED):
+    """qkv (B,S,2304) = cat(q, k, v) after the bias -> concat_heads(softmax(q k^T / 8) v), (B,S,768), with the roundings
+    named in `rounding` (qkv, scores, p, att).  More than 64 tokens: the two-half form of attention_long_kernel."""
+    r = rounding
+    B, S, D3 = qkv.shape
+    D = D3 // 3
+    hd = D // HEADS
+    if "qkv" in r:
+        qkv = _r16(qkv)
+    q, k, v = (t.view(B, S, HEADS, hd).transpose(1, 2) for t in qkv.split(D, dim=-1))
+    s = (q @ k.transpose(-1, -2)) * (hd ** -0.5)
+    if "scores" in r:
+        s = _r16(s)
+    if S <= 64 or "p" not in r:
+        p = torch.softmax(s, dim=-1)
+        if "p" in r:
+            p = _r16(p)
+        o = p @ v
+    else:
+        c = LONG_KEY_SPLIT
+        m1 = s[..., :c].amax(-1, keepdim=True)
+        m = s.amax(-1, keepdim=True)
+        e1, e2 = torch.exp(s[..., :c] - m1), torch.exp(s[..., c:] - m)
+        carry = torch.exp(m1 - m)
+        o = ((_r16(e1) @ v[..., :c, :]) * carry + _r16(e2) @ v[..., c:, :]) / (e1.sum(-1, keepdim=True) * carry
+                                                                               + e2.sum(-1, keepdim=True))
+    o = o.transpose(1, 2).reshape(B, S, D)
+    return _r16(o) if "att" in r else o
+
+
+def block(sd, i, x, *, declared_rounding=False, rounding=None, resid="acc", eps=LN_EPS, gelu=1.702):
+    """Resblock i on the residual stream x (B, tokens, 768), in x's dtype.  ``resid``: the engine's VF_CLIP_RESID form
+    (its fp16 increments are part of the declared rounding of that form)."""
+    r = _rounding(declared_rounding, rounding)
+    if declared_rounding and rounding is None:
+        r = r | RESID_ROUNDING[resid]
+    dt = x.dtype
+    p = f"visual.transformer.resblocks.{i}."
+
+    def rnd(t, name):
+        return _r16(t) if name in r else t
+
+    h = rnd(_ln_d(x, sd[p + "ln_1.weight"], sd[p + "ln_1.bias"], eps), "ln")
+    qkv = F.linear(h, _rw(sd[p + "attn.in_proj_weight"], r, dt), sd[p + "attn.in_proj_bias"].to(dt))
+    att = attention_core(qkv, rounding=r)
+    y = F.linear(att, _rw(sd[p + "attn.out_proj.weight"], r, dt), sd[p + "attn.out_proj.bias"].to(dt))
+    x = rnd(x + rnd(y, "y_o"), "resid")
+    h = rnd(_ln_d(x, sd[p + "ln_2.weight"], sd[p + "ln_2.bias"], eps), "ln")
+    h = F.linear(h, _rw(sd[p + "mlp.c_fc.weight"], r, dt), sd[p + "mlp.c_fc.bias"].to(dt))
+    h = rnd(h * torch.sigmoid(gelu * h), "mlp")
+    y = F.linear(h, _rw(sd[p + "mlp.c_proj.weight"], r, dt), sd[p + "mlp.c_proj.bias"].to(dt))
+    return rnd(x + rnd(y, "y_m"), "resid")
+
+
+def head(sd, x_cls, *, declared_rounding=False, rounding=None, eps=LN_EPS):
+    """ln_post + projection on class-token rows x_cls (B, 768) -> (B, 512)."""
+    r = _rounding(declared_rounding, rounding)
+    h = _ln_d(x_cls, sd["visual.ln_post.weight"], sd["visual.ln_post.bias"], eps)
+    if "ln" in r:
+        h = _r16(h)
+    return h @ _rw(sd["visual.proj"], r, x_cls.dtype)
+
+
+@torch.no_grad()
+def encode_image_declared(sd, frames, *, dtype=torch.float64, declared_rounding=True, rounding=None, resid="acc",
+                          eps=LN_EPS, gelu=1.702):
+    """The tower from embed / block / head (what ``encode_image(dtype=...)`` runs)."""
+    kw = dict(declared_rounding=declared_rounding, rounding=rounding, eps=eps)
+    x = embed(sd, frames, dtype=dtype, **kw)
+    for i in range(LAYERS):
+        x = block(sd, i, x, resid=resid, gelu=gelu, **kw)
+    return head(sd, x[:, 0, :], **kw)
 
 
 def to_hf_state_dict(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:

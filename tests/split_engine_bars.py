@@ -123,3 +123,59 @@ SEPARATION_RAFT = {
     "flow head conv2 input": {},                                               # (1.3 at the low-res flow)
     "GRU motion slice": {"net": 4.5},                                          # (5.8)
 }
+
+
+# ---- CLIP ViT towers, piece by piece against a float64 reference with the tower's declared rounding
+# (oracle/clip_tower.py DECLARED: embed / block / head / attention_core), each piece fed the ENGINE's own input, held by
+# test_clip_float64_gpu.py.  Worst row = worst TOKEN row (768 values) for embed / block / attention, worst feature row
+# for head / features; (rel-L2, max-abs / max|ref|).  Measured values: the comment beside each bar.
+#
+# What the bars consist of.  Every fp16 rounding point sits behind fp32 arithmetic in the engine and float64 in the
+# reference; a relative difference e between the two flips the rounding of a fraction ~e / 2^-11 of the elements, each by
+# one ulp, so the rounded tensor differs by ~sqrt(e * 2^-11) rms: 7e-6 for e = 1e-7, against the 1e-7 itself.  A block has
+# six such points in a row (ln_1, q/k/v, P, attention output, ln_2, MLP hidden), which is where its 2e-5 .. 6e-5 comes
+# from, and any fp16 tensor compared directly (the attention output) has a max-abs floor of one ulp, 4.9e-4, whenever its
+# largest element flips.  Perturbations smaller than the flips they cause (unrounded P, fp16 scores, eps 1e-6 on rows
+# of unit variance, a QuickGELU constant of 1.7) therefore cannot be told apart by any rel-L2 bar; for those the tests use
+# defect_share() below, which can.
+# Measured on one H100 80GB HBM3 (700 W power limit); the engine is deterministic, a rerun gives the same values.
+CLIP_VIT = {
+    "embed": (4e-6, 7e-6),                        # 2.1e-6 / 3.9e-6   B/32 and B/16, 1 / 3 / 13 frames, both entries
+    "block": {"plain": (1e-4, 1.2e-4),            # 5.7e-5 / 6.6e-5   12 blocks x 1 / 2 / 5 / 23 frames, block 5 at 250, split path
+              "outlier": (6e-5, 6e-5),            # 3.1e-5 / 3.1e-5   residual peaks above 50 (relative to larger rows)
+              "plain16": (1e-4, 1.1e-4)},         # 5.5e-5 / 5.7e-5   B/16, 3 frames
+    # VF_CLIP_RESID=y / mix: one flip of an fp16 increment is 2^-11 of that element, straight into the stream
+    "block y": {"plain": (1.4e-4, 3.5e-4),        # 7.6e-5 / 2.0e-4   (mix: 5.9e-5 / 1.0e-4)
+                "outlier": (1e-4, 9e-5)},         # 5.3e-5 / 4.5e-5
+    "head": (7e-6, 8e-6),                         # 3.5e-6 / 4.0e-6   the row of variance 1e-6; engine stream rows 1.0e-6 / 1.3e-6
+    # A row of 768 equal values: the kernel's mean is sum * fl(1 / 768), not sum / 768, so x - mean is 2^-25 x instead of
+    # 0; times rstd = 1 / sqrt(eps) = 316 that is 1e-5 absolute in an output that consists of the bias alone (|b| ~ 0.05).
+    "head constant row": (5e-4, 5.5e-4),          # 2.5e-4 / 2.8e-4
+    "attention": (5e-4, 1.6e-3),                  # 2.7e-4 / 8.7e-4   block 5 on its own ln_1 output; an fp16 output: 1 ulp = 4.9e-4
+    # scores of 20 .. 100 (several hundred at most): one flipped q or k element moves a score by ~1e-2 and P with it
+    "attention hard": (7e-3, 1.5e-2),             # 3.6e-3 / 7.6e-3   B/32 1 / 2 / 5 / 23 frames, B/16 1 / 3 / 7
+    # The flips of 12 blocks compound, and the tower amplifies them: 6.5x a block's error, 2.7x under the 1e-3 product
+    # gate.  The declared-rounding tower in fp32 on the CPU lies as far from the float64 one (3.3e-4 / 3.7e-4).
+    "features": (6e-4, 8e-4),                     # 3.7e-4 / 5.1e-4   8 and 270 frames
+}
+# Controls: (bar the control is asserted against, factor by which it must fail it; measured on the GPU in the comment).
+CLIP_VIT_CONTROLS = {
+    "bf16 weights": ("block", 4),                 # 5.1x / 5.6x
+    "in_proj bias group zeroed": ("attention", 10),   # 19x / 36x  (6.1x / 5.3x the block bar)
+    "eps 1e-6": ("head", 1000),                   # on the row of variance 1e-6
+}
+# defect_share: the most the engine's error may carry of a defect's direction, and the least an engine with the defect
+# shows.  Measured on the GPU at block 5: P unrounded +0.28, eps 1e-6 +0.22, QuickGELU 1.7 +0.06, bias group zeroed
+# +0.001.  The first two are not 0: a perturbation far under one ulp acts only through the elements that sit on a
+# rounding boundary, and those are the elements the engine's own fp32 error flips too, in the same direction half the time.
+CLIP_VIT_SHARE = (0.5, 0.65)
+
+
+def defect_share(got: torch.Tensor, ref: torch.Tensor, ref_defect: torch.Tensor) -> float:
+    """Least-squares coefficient of (ref_defect - ref) in (got - ref): 1 when `got` was computed the way `ref_defect` was,
+    0 when the way `ref` was.  Rounding flips are uncorrelated with the direction, so over the ~1e5 elements of a block
+    output they move the coefficient by ~1e-2 even where they exceed the defect in norm."""
+    ref = ref.double().flatten()
+    d = ref_defect.double().flatten().to(ref.device) - ref
+    e = got.double().flatten().to(ref.device) - ref
+    return float((e @ d) / (d @ d))

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
 def test_version_and_error_text():
     from video_features_b200 import _lib
     lib = _lib.lib()
-    assert lib.vf_version() == 1
+    assert lib.vf_version() == 2
     b, e = ctypes.c_int64(), ctypes.c_int64()
     assert lib.vf_shard_range(10, 0, 0, ctypes.byref(b), ctypes.byref(e)) == 1
     assert b"shard_range" in lib.vf_last_error()

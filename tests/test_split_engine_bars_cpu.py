@@ -163,3 +163,85 @@ def test_raft_bars_separate_declared_from_single_fp16(monkeypatch):
         "GRU motion slice": dict(gru_motion=True),
     }
     _check_separation("raft", variants, run, run(), bars.RAFT_BARS, bars.SEPARATION_RAFT)
+
+
+def test_clip_vit_bars_and_defect_share_separate_the_controls():
+    """CLIP ViT: block 5 of the plain synthetic tower at 3 frames.  The engine is emulated by the declared-rounding block
+    in fp32 (fp32 accumulation, rounding flips against the float64 reference: what the GPU bars consist of).  Against
+    the committed block bar: the emulation passes; bf16 weights, an fp16 residual stream and a zeroed in_proj bias group
+    fail it.  Unrounded P, fp16 scores, eps 1e-6 and a QuickGELU constant of 1.7 stay within about 1x of the bar -- each is
+    smaller than the flips it causes -- and are told apart by defect_share instead: an emulated engine WITH the defect
+    carries more than 0.65 of its direction (0.78 .. 1.0 here), the one without less than 0.5 (0.0 .. 0.24).  eps 1e-6 fails the head bar on a row of
+    variance 1e-6; the zeroed bias group fails the attention bar."""
+    import torch.nn.functional as F
+    from oracle import clip_tower as C
+    torch.set_grad_enabled(False)
+    sd = C.synthetic_state_dict(0)
+    sd64 = {k: v.double() for k, v in sd.items()}
+    k = 5
+    p = f"visual.transformer.resblocks.{k}."
+    x = C.embed(sd64, torch.randn(3, 3, 224, 224, generator=torch.Generator().manual_seed(1)), declared_rounding=True)
+    for i in range(k):
+        x = C.block(sd64, i, x, declared_rounding=True)
+    x = x.float().double()                                   # the engine's stream is fp32
+    rows = lambda t: t.reshape(-1, t.shape[-1])
+    ref = C.block(sd64, k, x, declared_rounding=True)
+    bar = bars.CLIP_VIT["block"]["plain"]
+    emu = C.block(sd, k, x.float(), declared_rounding=True)
+    err = bars.row_errors(rows(emu), rows(ref))
+    print(f"clip block fp32 emulation: {err[0]:.1e} / {err[1]:.1e} (bar {bar[0]:.0e} / {bar[1]:.0e})")
+    assert bars.within(err, bar), err
+
+    sdz = dict(sd64)
+    sdz[p + "attn.in_proj_bias"] = sd64[p + "attn.in_proj_bias"].clone()
+    sdz[p + "attn.in_proj_bias"][-8:] = 0
+    sdb = {n: (v.bfloat16().double() if v.dim() >= 2 and "positional" not in n else v) for n, v in sd64.items()}
+    f32 = lambda d: {n: v.float() for n, v in d.items()}
+    # name -> (kwargs of the defect, state dict, least factor over the block bar or None where it is not separated)
+    variants = {
+        "bf16 weights": (dict(declared_rounding=True), sdb, bars.CLIP_VIT_CONTROLS["bf16 weights"][1]),
+        "fp16 residual stream": (dict(rounding=C.DECLARED | {"resid"}), sd64, 2.5),
+        "in_proj bias group zeroed": (dict(declared_rounding=True), sdz, 2.5),
+        "P unrounded": (dict(rounding=C.DECLARED - {"p"}), sd64, None),
+        "fp16 scores": (dict(rounding=C.DECLARED | {"scores"}), sd64, None),
+        "eps 1e-6": (dict(declared_rounding=True, eps=1e-6), sd64, None),
+        "QuickGELU 1.7": (dict(declared_rounding=True, gelu=1.7), sd64, None),
+    }
+    lo, hi = bars.CLIP_VIT_SHARE
+    failures = []
+    for name, (kw, sdv, factor) in variants.items():
+        refd = C.block(sdv, k, x, **kw)
+        e = bars.row_errors(rows(refd), rows(ref))
+        with_defect = bars.defect_share(C.block(f32(sdv), k, x.float(), **kw), ref, refd)
+        without = bars.defect_share(emu, ref, refd)
+        print(f"clip {name:<26s} {e[0] / bar[0]:5.1f}x / {e[1] / bar[1]:5.1f}x the block bar; share with the defect "
+              f"{with_defect:+.2f}, without {without:+.2f}")
+        if factor is not None and not bars.beyond(e, bar, factor):
+            failures.append((name, e, factor))
+        if factor is None and bars.beyond(e, bar, 2):
+            failures.append((name, e, "stated as not separated, yet 2x over the bar"))
+        if not (with_defect > hi and abs(without) < lo):
+            failures.append((name, with_defect, without))
+    assert not failures, failures
+
+    # the head: a row of variance 1e-6, where eps = 1e-5 decides the result
+    row = (1e-3 * torch.randn(1, 768, generator=torch.Generator().manual_seed(3))).double()
+    h_ref = C.head(sd64, row, declared_rounding=True)
+    h_emu = C.head(sd, row.float(), declared_rounding=True)
+    assert bars.within(bars.row_errors(h_emu, h_ref), bars.CLIP_VIT["head"])
+    what, factor = bars.CLIP_VIT_CONTROLS["eps 1e-6"]
+    assert bars.beyond(bars.row_errors(C.head(sd64, row, declared_rounding=True, eps=1e-6), h_ref), bars.CLIP_VIT[what], factor)
+
+    # the attention half on the block's own ln_1 output: the zeroed bias group
+    h = C._r16(C._ln_d(x, sd64[p + "ln_1.weight"], sd64[p + "ln_1.bias"], C.LN_EPS))
+    w = C._r16(sd64[p + "attn.in_proj_weight"])
+    att = frozenset({"qkv", "p", "att"})
+    a_ref = C.attention_core(F.linear(h, w, sd64[p + "attn.in_proj_bias"]), rounding=att)
+    a_emu = C.attention_core(F.linear(h.float(), w.float(), sd[p + "attn.in_proj_bias"]), rounding=att)
+    a_ctl = C.attention_core(F.linear(h, w, sdz[p + "attn.in_proj_bias"]), rounding=att)
+    what, factor = bars.CLIP_VIT_CONTROLS["in_proj bias group zeroed"]
+    abar = bars.CLIP_VIT[what]
+    assert bars.within(bars.row_errors(rows(a_emu), rows(a_ref)), abar)
+    ctl = bars.row_errors(rows(a_ctl), rows(a_ref))
+    print(f"clip attention, bias group zeroed: {ctl[0] / abar[0]:.1f}x / {ctl[1] / abar[1]:.1f}x the attention bar")
+    assert bars.beyond(ctl, abar, factor), ctl

@@ -89,6 +89,10 @@ SIGNATURES = {
                                                C.c_void_p, C.POINTER(C.c_int64)]),
     "vf_clip_wait": (C.c_int, [C.c_void_p, C.c_int64]),
     "vf_clip_block_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "vf_clip_debug_embed_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_debug_embed_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_debug_blocks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vf_clip_debug_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_clip_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_i3d_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(I3DWeights), C.c_int, C.c_int, C.c_int, C.c_int]),
     "vf_i3d_destroy": (C.c_int, [C.c_void_p]),

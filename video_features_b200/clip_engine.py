@@ -161,6 +161,47 @@ class ClipEngine:
                                                 torch.cuda.current_stream().cuda_stream))
         return out
 
+    # ---- diagnostics: the tower's three pieces one at a time (vf_clip_debug_*); at most one chunk of frames per call
+    def debug_embed(self, frames: torch.Tensor) -> torch.Tensor:
+        """Patchify + patch embedding + ln_pre: (n,3,224,224) float32 or (n,H,W,3) uint8 on this device -> the fp32
+        residual stream (n*tokens, 768)."""
+        assert frames.is_cuda and frames.dim() == 4
+        frames = frames.contiguous()
+        n = frames.shape[0]
+        x = torch.empty((n * self.tokens, 768), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream().cuda_stream
+            if frames.dtype == torch.uint8:
+                assert frames.shape[3] == 3, frames.shape
+                check(lib().vf_clip_debug_embed_u8(self._h, frames.data_ptr(), n, frames.shape[1], frames.shape[2],
+                                                   x.data_ptr(), stream))
+            else:
+                assert frames.dtype == torch.float32 and tuple(frames.shape[1:]) == (3, 224, 224), frames.shape
+                check(lib().vf_clip_debug_embed_f32(self._h, frames.data_ptr(), n, x.data_ptr(), stream))
+        return x
+
+    def debug_blocks(self, x: torch.Tensor, begin: int, end: int) -> torch.Tensor:
+        """Resblocks [begin, end) on a copy of the residual stream x (n*tokens, 768) float32.  end == 12: only the
+        class-token rows (frame * tokens) of the result are defined."""
+        t = self.tokens
+        assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.shape[1] == 768 and x.shape[0] % t == 0
+        x = x.contiguous().clone()
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_debug_blocks(self._h, x.data_ptr(), x.shape[0] // t, begin, end,
+                                             torch.cuda.current_stream().cuda_stream))
+        return x
+
+    def debug_head(self, x: torch.Tensor) -> torch.Tensor:
+        """ln_post on the class-token rows of x (n*tokens, 768) float32 + the projection -> (n, 512)."""
+        t = self.tokens
+        assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.shape[1] == 768 and x.shape[0] % t == 0
+        x = x.contiguous()
+        out = torch.empty((x.shape[0] // t, 512), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_debug_head(self._h, x.data_ptr(), x.shape[0] // t, out.data_ptr(),
+                                           torch.cuda.current_stream().cuda_stream))
+        return out
+
     @property
     def launch_count(self) -> int:
         return int(lib().vf_clip_launch_count(self._h))

@@ -189,26 +189,36 @@ static int tower_attention(vf_clip* h, int c, cudaStream_t s) {
     return launch_attention(h->qkv, h->att, c, h->T, H, s);
 }
 
-// The tower on one chunk whose patch matrix is already in h->patches; writes c x 512 fp32 to out.
+// The tower on one chunk is three pieces -- embed, blocks, head -- that vf_clip_debug_embed / _blocks / _head also run one
+// at a time (the float64 tests hold each to a reference of its own).
 // GEMM epilogues never read global memory: bias / QuickGELU in registers, then global stores -- or, for the two GEMMs
 // that end a residual branch, fp32 reductions that add the tile into the fp32 residual stream x.
-static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
-    const int T = h->T, P = h->P, PK = h->PK;
-    const int M = c * T;
+
+// h->patches (c frames) -> h->x: the patch-embedding GEMM, then token assembly + ln_pre
+static int tower_embed(vf_clip* h, int c, cudaStream_t s) {
+    const int P = h->P, PK = h->PK;
     // patch embedding: [c*P, PK] x [768, PK]^T -> emb (fp32)
     VF_TRY(tower_gemm(h, h->patches, PK, h->w_patch, PK, c * P, W, PK, epi(h->emb, W, 1, nullptr, VF_ACT_NONE), s));
     // token assembly (+ class / positional embedding) fused with ln_pre -> x
     VF_TRY(tower_embed_ln(h, c, s));
     h->launches += 2;
+    return VF_OK;
+}
+
+// resblocks [l0, l1) on h->x.  In the y forms the MLP increment of block l1 - 1 is left in h->y, not yet added (the next
+// ln_1, or the head, adds it); h->x must hold no such pending increment on entry.
+static int tower_blocks(vf_clip* h, int c, int l0, int l1, cudaStream_t s) {
+    const int T = h->T;
+    const int M = c * T;
     // The residual stream x stays fp32 in HBM.  A GEMM that ends a residual branch either ADDS its result into x from the
     // epilogue (fp32 global reductions; the LayerNorm pass that follows then only reads x and writes h: 6 bytes per
     // element), or writes an fp16 increment y that the LayerNorm kernel adds ("x += y; h = LN(x)": 12 bytes per element).
     // acc_o / acc_m select the form for the attention out-projection / the MLP's second GEMM (VF_CLIP_RESID=acc|y|mix).
     const bool acc_o = h->acc_o, acc_m = h->acc_m;
-    for (int l = 0; l < L; ++l) {
+    for (int l = l0; l < l1; ++l) {
         const ClipLayerDev& w = h->layer[l];
         // h = ln_1(x)   (y form: x += y of the previous block's MLP first)
-        VF_TRY(tower_add_ln(h, h->x, W, (acc_m || l == 0) ? nullptr : h->y, W, 1, w.ln1_w, w.ln1_b, h->h, W, M, s));
+        VF_TRY(tower_add_ln(h, h->x, W, (acc_m || l == l0) ? nullptr : h->y, W, 1, w.ln1_w, w.ln1_b, h->h, W, M, s));
         if (h->fused_attn) {
             VF_TRY(tower_qkv_attention(h, w, c, s));
         } else {
@@ -233,11 +243,23 @@ static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
         else       VF_TRY(tower_gemm(h, h->mlp, MLPW, w.w_proj, MLPW, rows, W, MLPW, epi(h->y, W, 0, w.b_proj, VF_ACT_NONE), s));
         h->launches += h->fused_attn ? 6 : 7;
     }
-    // CLS rows: (y form: x += y of the last MLP;) ln_post; then the 768 -> 512 projection
-    VF_TRY(tower_add_ln(h, h->x, int64_t(T) * W, acc_m ? nullptr : h->y, W, 0, h->lnpost_w, h->lnpost_b, h->cls, W, c, s));
+    return VF_OK;
+}
+
+// CLS rows of h->x (row pitch T*768): (y != nullptr: + the last MLP's increment, compact rows of pitch 768;) ln_post; then
+// the 768 -> 512 projection -> out (c x 512 fp32)
+static int tower_head(vf_clip* h, int c, const __half* y, float* out, cudaStream_t s) {
+    VF_TRY(tower_add_ln(h, h->x, int64_t(h->T) * W, y, W, 0, h->lnpost_w, h->lnpost_b, h->cls, W, c, s));
     VF_TRY(tower_gemm(h, h->cls, W, h->w_proj, W, c, E, W, epi(out, E, 1, nullptr, VF_ACT_NONE), s));
     h->launches += 2;
     return VF_OK;
+}
+
+// The tower on one chunk whose patch matrix is already in h->patches; writes c x 512 fp32 to out.
+static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
+    VF_TRY(tower_embed(h, c, s));
+    VF_TRY(tower_blocks(h, c, 0, L, s));
+    return tower_head(h, c, h->acc_m ? nullptr : h->y, out, s);
 }
 
 constexpr int TOWER_LAUNCHES_SPLIT = 2 + 7 * L + 2, TOWER_LAUNCHES_FUSED = 2 + 6 * L + 2;
@@ -668,6 +690,68 @@ int vf_clip_block_attention(vf_clip_t* h, int layer, const void* x, int n_frames
     __half* qkv = h->lanes[0].qkv;
     VF_TRY(gemm_f16(xin, W, w.w_qkv, W, n_frames * T, 3 * W, W, epi(qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
     return launch_attention(qkv, o, n_frames, T, H, s);
+}
+
+// The three pieces of the tower one at a time, eagerly, on lane 0's workspace and the caller's stream.
+static int debug_args(vf_clip_t* h, const void* a, const void* b, int n, const char* what) {
+    if (!h || !a || !b) return fail(VF_ERR_INVALID, "%s: null argument", what);
+    if (n <= 0 || n > h->chunk) return fail(VF_ERR_INVALID, "%s: %d frames (1 .. %d, the handle's chunk)", what, n, h->chunk);
+    VF_CUDA(cudaSetDevice(h->device));
+    return VF_OK;
+}
+
+int vf_clip_debug_embed_f32(vf_clip_t* h, const float* frames, int n, float* x_out, void* stream) {
+    VF_TRY(debug_args(h, frames, x_out, n, "clip_debug_embed_f32"));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    LaneScope lane(h, 0);
+    VF_TRY(launch_clip_patchify_f32(frames, n, h->patches, h->patch, s));
+    h->launches += 1;
+    VF_TRY(tower_embed(h, n, s));
+    VF_CUDA(cudaMemcpyAsync(x_out, h->x, size_t(n) * h->T * W * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return VF_OK;
+}
+
+int vf_clip_debug_embed_u8(vf_clip_t* h, const uint8_t* frames, int n, int src_h, int src_w, float* x_out, void* stream) {
+    VF_TRY(debug_args(h, frames, x_out, n, "clip_debug_embed_u8"));
+    ClipGeom g;
+    VF_TRY(clip_geometry(src_h, src_w, &g));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    LaneScope lane(h, 0);
+    VF_TRY(clip_transform_chunk(h, frames, n, src_h, src_w, g, s));
+    VF_TRY(tower_embed(h, n, s));
+    VF_CUDA(cudaMemcpyAsync(x_out, h->x, size_t(n) * h->T * W * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return VF_OK;
+}
+
+int vf_clip_debug_blocks(vf_clip_t* h, float* x, int n_frames, int layer_begin, int layer_end, void* stream) {
+    VF_TRY(debug_args(h, x, x, n_frames, "clip_debug_blocks"));
+    if (layer_begin < 0 || layer_begin >= layer_end || layer_end > L)
+        return fail(VF_ERR_INVALID, "clip_debug_blocks: layers [%d, %d) are not a range within [0, %d)", layer_begin, layer_end, L);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    LaneScope lane(h, 0);
+    const int T = h->T;
+    const size_t bytes = size_t(n_frames) * T * W * sizeof(float);
+    VF_CUDA(cudaMemcpyAsync(h->x, x, bytes, cudaMemcpyDeviceToDevice, s));
+    VF_TRY(tower_blocks(h, n_frames, layer_begin, layer_end, s));
+    if (!h->acc_m) {
+        // y forms: add the last MLP's pending increment the way the tower does, with the add + LayerNorm kernel writing x
+        // back (x += y); its LayerNorm output lands in scratch (cls / h) and is dropped.  After block 11 the increment is
+        // the compact CLS-row buffer and x is addressed at the CLS rows, as the head would.
+        const bool cls_only = layer_end == L;
+        VF_TRY(tower_add_ln(h, h->x, cls_only ? int64_t(T) * W : W, h->y, W, 1, h->lnpost_w, h->lnpost_b,
+                            cls_only ? h->cls : h->h, W, cls_only ? n_frames : n_frames * T, s));
+        h->launches += 1;
+    }
+    VF_CUDA(cudaMemcpyAsync(x, h->x, bytes, cudaMemcpyDeviceToDevice, s));
+    return VF_OK;
+}
+
+int vf_clip_debug_head(vf_clip_t* h, const float* x, int n_frames, float* out, void* stream) {
+    VF_TRY(debug_args(h, x, out, n_frames, "clip_debug_head"));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    LaneScope lane(h, 0);
+    VF_CUDA(cudaMemcpyAsync(h->x, x, size_t(n_frames) * h->T * W * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return tower_head(h, n_frames, nullptr, out, s);
 }
 
 int64_t vf_clip_launch_count(const vf_clip_t* h) { return h ? h->launches : 0; }

@@ -156,7 +156,7 @@ using namespace vf;
 
 extern "C" {
 
-int vf_version(void) { return 1; }
+int vf_version(void) { return 2; }
 const char* vf_last_error(void) { return g_err; }
 
 int vf_sample_indices(const char* method, int param, int64_t frame_cnt, double fps, int64_t* out_idx, int64_t cap,
