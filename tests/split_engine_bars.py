@@ -179,3 +179,65 @@ def defect_share(got: torch.Tensor, ref: torch.Tensor, ref_defect: torch.Tensor)
     d = ref_defect.double().flatten().to(ref.device) - ref
     e = got.double().flatten().to(ref.device) - ref
     return float((e @ d) / (d @ d))
+
+
+# ---- PWC-Net and RAFT under motion (test_flow_motion_gpu.py; premise: test_flow_steering_cpu.py)
+# The seeded stand-ins warp PWC's second frame by ~1 px and move RAFT's lookup centre by under half a cell; the steered
+# state dicts of tests/flow_steering.py reach 8 px and 3 .. 45 cells.  SEPARATION_FLOW_MOTION: how far above the bar a
+# defective sampler lies in the float64 oracle (PWC: worst rel-L2 of the cost volume, decoder flow and final flow over
+# its bar; RAFT: bars.beyond at lookup / GRU state / flow_up), on the stand-in's small motion (128 x 160, the inputs
+# and bars of test_pwc_gpu.py / test_i3d_raft_float64_gpu.py) and on the steered inputs (PWC_MOTION_BARS /
+# RAFT_MOTION_BARS below).  Measured in parentheses; 0 = stated as NOT separated (under the bar).
+# What it shows: the gross sampler defects -- truncation for floor, border clamp for zero padding, a dropped mask,
+# align_corners=False, an untransposed window, the level scaling misplaced -- were already far above the bars on the
+# small-motion inputs, through the border pixels alone (a border sample with negative flow has a negative coordinate
+# and an outside tap).  What small motion does NOT separate is a lost lo half of PWC's upsampled-flow pair: 2^-11 of
+# the flow is under the bars while the flow is about a pixel (0.34x), and above them once it is eight (5.6x, 7.7x).
+# RAFT's flow pair is separated by neither.  `mask >= 0.999` is
+# separated by no input (a raw mask of exactly 0.999 does not occur); the GPU test brackets the threshold instead, with
+# border raw masks of 0.9995 and 0.9985.
+SEPARATION_FLOW_MOTION = {
+    "pwc": {
+        "truncation for floor": {"small motion": 5000, "uniform level 2": 800, "varying level 2": 2500},   # (7950, 1300, 3820)
+        "border clamp for zeros": {"small motion": 5500, "uniform level 2": 7000, "varying level 2": 5000},  # (8410, 10600, 8120)
+        "mask >= 0.999": {"small motion": 0, "uniform level 2": 0, "varying level 2": 0},                 # (1e-11)
+        "mask dropped": {"small motion": 5500, "uniform level 2": 2000, "varying level 2": 2300},         # (8380, 3210, 3540)
+        "align_corners=False": {"small motion": 3000, "uniform level 2": 3000, "varying level 2": 4000},  # (4590, 4620, 6570)
+        "upflow pair's lo half lost": {"small motion": 0, "uniform level 2": 3.5, "varying level 2": 5},  # (0.34, 5.6, 7.7)
+    },
+    "raft": {
+        "truncation for floor": {"small motion": 9e4, "uniform step": 6e4, "varying flow": 1e4},          # (1.4e5, 9.1e4, 1.6e4)
+        "border clamp for zeros": {"small motion": 1.7e5, "uniform step": 2e5, "varying flow": 2.5e4},    # (2.5e5, 3.2e5, 4.0e4)
+        "window not transposed": {"small motion": 9e4, "uniform step": 9e4, "varying flow": 1.3e4},       # (1.4e5, 1.3e5, 2.0e4)
+        "level scaling after the floor": {"small motion": 6e4, "uniform step": 7.5e4, "varying flow": 6e3},  # (9.3e4, 1.2e5, 9.1e3)
+        # Not separated by any input: 2^-11 of a 3.5-cell flow is 0.65x the 20-iteration bars (the refinement's own
+        # error has grown as much).  (A uniform step's flow is a multiple of 2^-3: its pair has no lo half to lose.)
+        "flow pair's lo half lost": {"small motion": 0, "uniform step": 0, "varying flow": 0},            # (0.07, 2e-10, 0.65)
+    },
+}
+
+# Bars of test_flow_motion_gpu.py, 1.5x .. 3x above the worst value measured on one H100 80GB HBM3 (700 W power limit;
+# the engines are deterministic).  PWC: rel-L2 of the cost volume against the oracle's warp of the engine's own features
+# and upflow, of each decoder flow and of the final flow (rel-L2, max-abs / max) against the oracle's forward, over
+# uniform warps at levels 5 .. 2 (128x160, 200x333), the threshold warps, the varying warps and the 40x50 frames.
+PWC_MOTION_BARS = {"volume": 3.5e-5,              # 1.70e-5 (level 5; 3.4e-6 and under below it)
+                   "flow": 1.5e-4,                # 7.2e-5
+                   "final": (1.8e-4, 2.5e-4)}     # 9.1e-5 / 1.24e-4 (the level-4 varying warp; 7.4e-5 / 7.4e-5 at level 2)
+# RAFT, per steered input, the stages of RAFT_STAGES; a stage not listed keeps its RAFT_BARS entry (fnet, cnet and the
+# pyramid do not depend on the flow: 4.95e-6 / 4.4e-6, 1.93e-6 / 2.35e-6, 3.5e-6 / 5.2e-6 as in RAFT_BARS' own runs).
+RAFT_MOTION_BARS = {
+    # lookup 3.5e-6 / 5.7e-6 (centres up to 45 cells from the query: no worse than in the query's own cell)
+    "uniform": dict(RAFT_BARS, net=(2.2e-5, 6e-5),            # 1.17e-5 / 3.0e-5
+                    lowres=(0.0, 0.0),                        # exact: dyadic steps
+                    flow_up=(1.2e-5, 2.6e-4)),                # 5.7e-6 / 1.30e-4
+    "varying 3": dict(RAFT_BARS, lowres=(5e-5, 6e-5),         # 2.34e-5 / 2.89e-5 (net 1.41e-5 / 2.19e-5)
+                      flow_up=(5e-5, 3.5e-4)),                # 2.33e-5 / 1.78e-4
+    # after 20 iterations of a 3.5-cell flow the lookup is taken at coordinates that carry the flow's own error
+    "varying 20": dict(RAFT_BARS, lookup=(4e-5, 1.5e-4),      # 1.85e-5 / 7.11e-5
+                       net=(7e-5, 2.2e-4),                    # 3.35e-5 / 1.08e-4
+                       lowres=(6e-5, 9e-5),                   # 2.90e-5 / 4.20e-5
+                       flow_up=(6.5e-5, 2.5e-4)),             # 3.13e-5 / 1.22e-4
+    # logits of +-60: where two of the nine are tied a logit error of 1e-5 x 60 moves the weights by as much, times
+    # the difference between the two neighbours' flows
+    "sharp": dict(RAFT_BARS, flow_up=(2.7e-4, 3.4e-3)),       # 1.33e-4 / 1.68e-3 (low-res flow 4.7e-5 / 5.6e-5)
+}

@@ -47,7 +47,10 @@ def _assert_masks_clear(st, rel=1e-4):
     of the sample position, i.e. of the displacement dblBackward * upflow; at the 1e-4 relative flow bar of the stage
     test that is 1e-4 x the level's largest displacement.  (A fixed 1e-4 would reject every input at level 5: the
     stand-in's level-6 features are leaky(bias), constant over the image, so its level-5 displacements are ~0.01 px
-    and the same border pixel sits 3e-5 from the threshold whatever the frames.)"""
+    and the same border pixel sits 3e-5 from the threshold whatever the frames.)
+
+    The threshold itself, and warps large enough to mask interior pixels, are tested in test_flow_motion_gpu.py, where a
+    uniform displacement makes the raw mask a known function of its fractional part."""
     from oracle import pwc_net
     for l in (5, 4, 3, 2):
         tol = rel * float((st[f"upflow{l}"] * pwc_net.DBL_BACKWARD[l]).abs().max())
