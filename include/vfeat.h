@@ -370,6 +370,40 @@ int64_t vf_clip_rn_launch_count(const vf_clip_rn_t* h);
  * four phase slots and 1/4 in its scale. */
 int vf_clip_rn_conv(const vf_clip_rn_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
+/* ---- VGGish audio embeddings (torchvggish VGG, postprocess=False): replaces models/vggish_torch's
+ * vggish_input.wavfile_to_examples + VGG.forward for PCM-16 samples.  Weights: torchvggish keys features.{0,3,6,8,11,13}
+ * and embeddings.{0,2,4} (.weight / .bias), HOST fp32.  The front end's float64 tables come from the caller: hann[400]
+ * (periodic Hann), mel[257][64] (HTK mel matrix, DC row zero) and resampy's kaiser_best interp_win[n_win] with
+ * num_table entries per zero crossing. */
+typedef struct vf_vggish vf_vggish_t;
+
+/* Workspace holds max_examples examples of 0.96 s (0 = 64); longer inputs run in chunks with the same features. */
+int vf_vggish_create(vf_vggish_t** out, const vf_named_tensor* tensors, int n_tensors, const double* hann,
+                     const double* mel, const double* interp_win, int n_win, int num_table, int device,
+                     int max_examples);
+int vf_vggish_destroy(vf_vggish_t* h);
+/* samples: n_samples x channels interleaved int16 on the device, at sample_rate -> *n_out examples (complete 96-frame
+ * examples of the 16 kHz log-mel; 0 when the audio is shorter than 15600 samples at 16 kHz, and nothing is written) ->
+ * out: n_out x 128 fp32 on the device (capacity in floats).  Mono mix and /32768 in float64, resampy 0.2.2
+ * kaiser_best to 16 kHz unless sample_rate is 16000, log-mel in float64, rounded to fp32 once. */
+int vf_vggish_forward_pcm16(vf_vggish_t* h, const int16_t* samples, int64_t n_samples, int channels, int sample_rate,
+                            float* out, int64_t capacity, int64_t* n_out, void* stream);
+/* examples: n x 96 x 64 fp32 log-mel on the device (the network input) -> out: n x 128 fp32 on the device. */
+int vf_vggish_forward_logmel_f32(vf_vggish_t* h, const float* examples, int n, float* out, void* stream);
+/* Diagnostics, of the last chunk of the last call: stage 0 the resampled 16 kHz waveform the chunk's frames read
+ * (float64, dims (count, 1, 1, 1); only after vf_vggish_forward_pcm16), 1 the log-mel (n, 1, 96, 64), 2..5 the
+ * outputs of max-pools 1..4 as NCHW, 6..8 fc1..fc3 after their ReLU (n, D, 1, 1); fp32 except stage 0.  out == NULL
+ * only queries dims4; capacity in elements. */
+int vf_vggish_read_stage(vf_vggish_t* h, int stage, void* out, int64_t capacity, int* dims4, void* stream);
+int64_t vf_vggish_launch_count(const vf_vggish_t* h);
+/* Diagnostics: conv `index` as uploaded: 0..5 conv1..conv6, 6..8 fc1..fc3.  Same contract as vf_resnet_conv; scale 1,
+ * bias the layer's.  conv1 is one tap of 32 over im2col rows (hi at kh * 3 + kw, lo 16 further); fc1 reads the
+ * position-major split rows of pool 4 (input feature (h * 4 + w) * 512 + c at column (h * 4 + w) * 1024 + c). */
+int vf_vggish_conv(const vf_vggish_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+/* Host only: resampy's time register (the sequential float64 sum of sample_rate / 16000) of outputs [t0, t0 + count),
+ * as the resampling kernel evaluates it. */
+int vf_vggish_time_register(int sample_rate, int64_t t0, int64_t count, double* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,7 +11,7 @@ import torch  # noqa: F401
 from video_features_b200.utils import form_list_from_user_input, sanity_check
 
 SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
-             'resnet101', 'resnet152', 'r21d_rgb']
+             'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch']
 
 
 def build_extractor(args):
@@ -34,8 +34,12 @@ def build_extractor(args):
     if args.feature_type == 'r21d_rgb':
         from video_features_b200.extract.extract_r21d import ExtractR21D
         return ExtractR21D(args)
-    if args.feature_type in ['vggish', 'vggish_torch']:
-        raise NotImplementedError(f'{args.feature_type}: outside the hot path this engine rebuilds (SURVEY.md §2)')
+    if args.feature_type == 'vggish_torch':
+        from video_features_b200.extract.extract_vggish import ExtractVGGish
+        return ExtractVGGish(args)
+    if args.feature_type == 'vggish':
+        raise NotImplementedError('vggish: the TF1 VGGish (a TF .ckpt, PCA and 8-bit quantisation) is not built; '
+                                  'use vggish_torch')
     raise NotADirectoryError                      # main.py:41
 
 

@@ -366,3 +366,32 @@ def r21d_golden():
 
 if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "r21d":
     r21d_golden()
+
+
+def vggish_golden():
+    """The reference's own VGGish pieces (models/vggish_torch/vggish_src) on a seeded ~7 s 16 kHz mono clip
+    (oracle/vggish_net.py synthetic_audio): vggish_input.waveform_to_examples of samples / 32768.0 (what
+    wavfile_to_examples feeds it) and VGG.forward on the calibrated stand-in (postprocess=False).  resampy and soundfile
+    need not be installed: they are stubbed in sys.modules, and neither is called at 16 kHz.  Stores the int16 samples, the
+    fp32 examples and the features."""
+    import torch
+    from oracle import vggish_net
+    for name in ("resampy", "soundfile"):
+        sys.modules.setdefault(name, types.ModuleType(name))
+    sys.path.insert(0, os.path.join(REF, "models", "vggish_torch"))
+    from vggish_src import vggish, vggish_input
+    samples = vggish_net.synthetic_audio(7.0, 16000, 1, seed=7)
+    ex = vggish_input.waveform_to_examples(samples / 32768.0, 16000)          # (n, 1, 96, 64) fp32
+    net = vggish.VGG(vggish.make_layers())
+    net.load_state_dict(vggish_net.stand_in_state_dict())
+    net.eval()
+    with torch.no_grad():
+        feats = net(ex).numpy()
+    ex = ex.detach().numpy()[:, 0]
+    print(f"vggish: {samples.shape[0]} samples -> examples {ex.shape}, features {feats.shape}")
+    np.savez_compressed(os.path.join(OUT, "vggish_outputs.npz"), samples=samples, sample_rate=np.array(16000),
+                        examples=ex, vggish_torch=feats)
+
+
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "vggish":
+    vggish_golden()

@@ -148,6 +148,17 @@ SIGNATURES = {
     "vf_clip_rn_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_clip_rn_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),
+    "vf_vggish_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vf_vggish_destroy": (C.c_int, [C.c_void_p]),
+    "vf_vggish_forward_pcm16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                          C.POINTER(C.c_int64), C.c_void_p]),
+    "vf_vggish_forward_logmel_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_vggish_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_vggish_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_vggish_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
+                                 C.c_void_p, C.c_void_p]),
+    "vf_vggish_time_register": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
     "vf_clip_profile": (C.c_int, [C.c_void_p, C.c_int]),
     "vf_clip_profile_categories": (C.c_int, [C.c_void_p, C.POINTER(C.c_double)]),
     "vf_clip_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
