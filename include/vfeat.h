@@ -404,6 +404,22 @@ int vf_vggish_conv(const vf_vggish_t* h, int index, int* geom, uint64_t* lo_mask
  * as the resampling kernel evaluates it. */
 int vf_vggish_time_register(int sample_rate, int64_t t0, int64_t count, double* out);
 
+/* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
+ * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),
+ * and the softmax + sort of utils/utils.py:19-47.  weight: n_classes x n_features, bias: n_classes, HOST fp32. */
+typedef struct vf_head vf_head_t;
+
+int vf_head_create(vf_head_t** out, const float* weight, const float* bias, int n_classes, int n_features, int device);
+int vf_head_destroy(vf_head_t* h);
+int vf_head_info(const vf_head_t* h, int* n_classes, int* n_features);
+/* feats: n x n_features fp32 on the device (n_features must equal the head's) -> logits, probs: n x n_classes fp32;
+ * top_idx (int32), top_logit, top_prob: n x k, 1 <= k <= min(8, n_classes); all on the device, on `stream`.
+ * Each logit is one sequential fp32 FMA chain over the features, plus the bias.  probs = expf(l - max) / sum, as torch's
+ * softmax.  Top-k order: probability descending, equal probabilities by the lower class index.  Two launches; n == 0
+ * writes nothing. */
+int vf_head_forward(vf_head_t* h, const float* feats, int n, int n_features, float* logits, float* probs, int k,
+                    int32_t* top_idx, float* top_logit, float* top_prob, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

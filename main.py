@@ -100,7 +100,8 @@ _FLAGS = [
     ('--resize_to_larger_edge', dict(dest='resize_to_smaller_edge', action='store_false', default=True,
                                     help='--side_size applies to the larger edge instead of the smaller one')),
     ('--side_size', dict(type=int, help='RAFT: resize frames to this edge length first')),
-    ('--show_pred', dict(dest='show_pred', action='store_true', default=False, help='print class predictions (not built here)')),
+    ('--show_pred', dict(dest='show_pred', action='store_true', default=False,
+                         help='print the top-5 classes of every feature (I3D, R(2+1)D: Kinetics-400; ResNet: ImageNet)')),
     # not in the reference: after extraction, ONE all-gather (NCCL over NVLink) returns every rank's feature blocks and
     # rank 0 writes them, list order, to this .npz
     ('--gather_features', dict(type=str, default=None, help='also all-gather the features of all GPUs into this .npz')),
@@ -121,6 +122,9 @@ if __name__ == "__main__":
     if args.keep_tmp_files:
         print(f'scratch files stay in {args.tmp_path}')
     sanity_check(args)
+    if args.show_pred and args.feature_type in ('raft', 'pwc'):
+        # the reference shows the flow in a cv2.imshow window; this engine ships headless OpenCV
+        print(f'--show_pred: ignored for {args.feature_type} (the reference shows flow in a GUI window)')
     if args.cpu:
         raise SystemExit('--cpu: this engine has no CPU path (the reference CPU flow is timed by '
                          '`python bench.py --impl reference`); pass --device_ids')

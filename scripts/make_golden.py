@@ -395,3 +395,81 @@ def vggish_golden():
 
 if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "vggish":
     vggish_golden()
+
+
+def show_pred_golden():
+    """--show_pred fixtures: (1) the reference's own printer (utils/utils.py show_predictions_on_dataset) on seeded
+    logits for both datasets, its stdout captured; (2) both label maps, as data; (3) the reference I3D module's
+    (softmax, logits) = model(x, features=False) on the stand-in weights (oracle/stand_in.py) for the rgb and flow
+    streams at T = 64 and 16; (4) with the reference's real i3d_rgb.pt, the logits of the first five 64-frame rgb stacks
+    of sample/v_GGSY1Qvo990.mp4, decoded (cv2, BGR kept) and transformed with the reference's own transforms."""
+    import contextlib
+    import io
+    import torch
+    import torchvision
+    install_mmcv_shim()
+    sys.path.insert(0, REF)
+    cwd = os.getcwd()
+    os.chdir(REF)
+    try:
+        from utils.utils import show_predictions_on_dataset
+        from models.i3d.i3d_src.i3d_net import I3D
+        from models.i3d.transforms.transforms import (PermuteAndUnsqueeze, PILToTensor, ResizeImproved, ScaleTo1_1,
+                                                      TensorCenterCrop, ToFloat)
+        from oracle import class_heads
+        d = {}
+        # (1) + (2)
+        for ds, n_cls, fname in (("kinetics", 400, "K400_label_map.txt"), ("imagenet", 1000, "IN_label_map.txt")):
+            g = torch.Generator().manual_seed(31 if ds == "kinetics" else 32)
+            logits = torch.randn(6, n_cls, generator=g) * 3.0
+            buf = io.StringIO()
+            with contextlib.redirect_stdout(buf):
+                show_predictions_on_dataset(logits, ds)
+            d[f"{ds}_logits"] = logits.numpy()
+            d[f"{ds}_text"] = np.array(buf.getvalue())
+            d[f"{ds}_labels"] = np.array([x.strip() for x in open(os.path.join(REF, "utils", fname))])
+        # (3)
+        for mod, cin in (("rgb", 3), ("flow", 2)):
+            sd = stand_in_state_dict(f"i3d_{mod}.pt")
+            net = I3D(num_classes=400, modality=mod).eval()
+            net.load_state_dict(sd)
+            for T in (64, 16):
+                x = torch.rand(1, cin, T, 224, 224, generator=torch.Generator().manual_seed(200 + T)) * 2 - 1
+                with torch.no_grad():
+                    smax, logits = net(x, features=False)
+                osm, olg = class_heads.i3d_forward_logits(sd, x)
+                rel = float((olg - logits).norm() / logits.norm())
+                print(f"i3d {mod} T={T} features=False: oracle vs reference logits rel {rel:.2e}")
+                assert rel < 1e-5
+                d[f"{mod}_T{T}_softmax"], d[f"{mod}_T{T}_logits"] = smax.numpy(), logits.numpy()
+        # (4)
+        real = os.path.join(REF, "models", "i3d", "checkpoints", "i3d_rgb.pt")
+        import cv2
+        cap = cv2.VideoCapture(os.path.join(REF, "sample", "v_GGSY1Qvo990.mp4"))
+        frames = []
+        while True:
+            ok, f = cap.read()
+            if not ok:
+                break
+            frames.append(f)
+        resize = torchvision.transforms.Compose([torchvision.transforms.ToPILImage(), ResizeImproved(256), PILToTensor(),
+                                                 ToFloat()])
+        tf = torchvision.transforms.Compose([TensorCenterCrop(224), ScaleTo1_1(), PermuteAndUnsqueeze()])
+        net = I3D(num_classes=400, modality="rgb").eval()
+        net.load_state_dict(torch.load(real, map_location="cpu"))
+        sm, lg = [], []
+        for s in range(5):                      # stacks of 65 frames, step 64; rgb_stack[:-1]
+            stack = torch.stack([resize(f) for f in frames[64 * s:64 * s + 64]])
+            with torch.no_grad():
+                a, b = net(tf(stack), features=False)
+            sm.append(a.numpy())
+            lg.append(b.numpy())
+        d["real_rgb_softmax"], d["real_rgb_logits"] = np.concatenate(sm), np.concatenate(lg)
+        print("real i3d_rgb top-1:", d["real_rgb_logits"].argmax(1).tolist())
+        np.savez_compressed(os.path.join(OUT, "show_pred.npz"), **d)
+    finally:
+        os.chdir(cwd)
+
+
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "show_pred":
+    show_pred_golden()

@@ -13,6 +13,9 @@ Features stay on the device until the video is finished: one device->host copy p
 reference's ``.tolist()`` per stack (extract_i3d.py:188).
 ``--flow_type flow`` (pre-computed ``flow_x_*.jpg`` / ``flow_y_*.jpg`` pairs, extract_i3d.py:195-229,266-278) feeds
 the same fused flow transform.
+``--show_pred``: the checkpoint's conv3d_0c_1x1 runs on each group's device features (I3DEngine.head); per stack and
+per stream, the header ``{video_path} @ stack {i} ({stream} stream)`` and the Kinetics top-5 are printed, stack-major as
+the reference loops (extract_i3d.py:180-229); with ``--flow_type flow`` only the flow stream prints, as there.
 """
 from __future__ import annotations
 
@@ -27,10 +30,12 @@ from tqdm import tqdm
 
 from .. import ops
 from .._lib import VF_FILTER_BILINEAR
+from ..class_head import TopKQueue
 from ..i3d_engine import I3DEngine
 from ..pwc_engine import PWCEngine
 from ..raft_engine import RAFTEngine
-from ..utils import AsyncSink, already_extracted, VideoReader, action_on_extraction, form_list_from_user_input
+from ..utils import (AsyncSink, already_extracted, VideoReader, action_on_extraction, form_list_from_user_input,
+                     print_top_predictions)
 
 PRE_CENTRAL_CROP_MIN_SIDE_SIZE = 256
 CENTRAL_CROP_MIN_SIDE_SIZE = 224
@@ -210,6 +215,18 @@ class ExtractI3D(torch.nn.Module):
             else:
                 raise NotImplementedError
 
+    def _show_group(self, preds: TopKQueue, feats: Dict[str, list], g0: int, n: int, models: dict, video_path):
+        """Queues the Kinetics top-5 of the group's last feature block per stream, printed stack-major once they are
+        on the host; only the top-5 crosses to the host."""
+        shown = [s for s in self.streams if not (self.flow_type == 'flow' and s != 'flow')]   # extract_i3d.py:226
+
+        def emit(tops):
+            for j in range(n):
+                for s, top in zip(shown, tops):
+                    print(f'{video_path} @ stack {g0 + j} ({s} stream)')
+                    print_top_predictions(*(t[j:j + 1] for t in top), 'kinetics')
+        preds.submit([(models['i3d'][s].head(), feats[s][-1]) for s in shown], emit)
+
     @staticmethod
     def _read_flow_pair(fx, fy) -> torch.Tensor:
         import cv2                                        # mmcv.imread(flag='grayscale') is cv2.imread(IMREAD_GRAYSCALE)
@@ -250,6 +267,7 @@ class ExtractI3D(torch.nn.Module):
             windows = stack_windows(n, self.stack_size, self.step_size, extra=0)
         else:
             windows = stack_windows(len(frames), self.stack_size, self.step_size, extra=1)
+        preds = TopKQueue() if self.show_pred else None
         for g0 in range(0, len(windows), self.group_stacks):
             group = windows[g0:g0 + self.group_stacks]
             first, last = group[0].start, group[-1].stop
@@ -259,6 +277,10 @@ class ExtractI3D(torch.nn.Module):
                 fl = torch.stack([torch.stack([self._read_flow_pair(*flows[i]) for i in w]) for w in group])
                 fl = fl.to(device, non_blocking=True).float()                      # uint8 grey levels, as the reference reads them
             self._run_group(feats, x, first, group, models, fl)
+            if preds is not None:
+                self._show_group(preds, feats, g0, len(group), models, video_path)
+        if preds is not None:
+            preds.flush()
         # one device->host copy per stream; float64 like the reference's `.tolist()` -> np.array
         feats_dict = {s: (torch.cat(v).cpu().numpy().astype(np.float64) if v else np.array([])) for s, v in feats.items()}
         feats_dict['fps'] = np.array(fps)

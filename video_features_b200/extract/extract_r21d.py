@@ -13,6 +13,8 @@ grow with the video.  Per call of CLIPS_PER_CALL stacks:
      (vf_r21d_forward_u8)
 The engine call is asynchronous, so decoding the next stacks overlaps the network on the current ones; the features
 stay on the device until the video is finished (one device->host copy per video).
+``--show_pred``: after every engine call the checkpoint's ``fc`` runs on its device features (class_head.py); per stack,
+the header ``{video_path} @ frames ({start}, {end})`` and the Kinetics top-5 are printed (extract_r21d.py:113-121).
 """
 from __future__ import annotations
 
@@ -25,8 +27,9 @@ import numpy as np
 import torch
 from tqdm import tqdm
 
+from ..class_head import FC_KEYS, ClassHead, TopKQueue
 from ..r21d_engine import R21DEngine
-from ..utils import AsyncSink, action_on_extraction, already_extracted, form_list_from_user_input
+from ..utils import AsyncSink, action_on_extraction, already_extracted, form_list_from_user_input, print_top_predictions
 from .extract_resnet import checkpoint_dirs
 
 CENTRAL_CROP_MIN_SIDE_SIZE = 112
@@ -82,6 +85,7 @@ class ExtractR21D(torch.nn.Module):
         self.progress = tqdm(total=len(self.path_list))
         self.keep_features = False
         self._engines: Dict[int, R21DEngine] = {}
+        self._heads: Dict[int, ClassHead] = {}
         self._pinned: Dict[tuple, List[torch.Tensor]] = {}
 
     def forward(self, indices: torch.LongTensor):
@@ -125,6 +129,12 @@ class ExtractR21D(torch.nn.Module):
                                             max_T=T)
         return self._engines[idx]
 
+    def _head(self, device: torch.device) -> ClassHead:
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        if idx not in self._heads:
+            self._heads[idx] = ClassHead.from_state_dict(load_r21d_weights(), FC_KEYS, idx, "r2plus1d_18 checkpoint")
+        return self._heads[idx]
+
     def _staging(self, shape) -> List[torch.Tensor]:
         """Two pinned uint8 staging buffers per frame size, each large enough for the frames of CLIPS_PER_CALL stacks:
         one fills while the other's host->device copy runs."""
@@ -137,6 +147,8 @@ class ExtractR21D(torch.nn.Module):
     def extract(self, device: torch.device, model=None, classifier=None, video_path=None) -> Dict[str, np.ndarray]:
         import cv2
         eng = self._engine(device)
+        head = self._head(device) if self.show_pred else None
+        preds = TopKQueue() if self.show_pred else None
         T, step = self.stack_size, self.step_size
         cap = cv2.VideoCapture(video_path)
         if not cap.isOpened():             # the reference's read_video raises on an unreadable file
@@ -161,6 +173,12 @@ class ExtractR21D(torch.nn.Module):
                 copied[s] = torch.cuda.Event()
                 copied[s].record()
                 outs.append(eng.forward_u8(x, [pos[i * step] for i in range(first, last + 1)], T))
+                if head is not None:               # only the top-5 crosses to the host, printed one call later
+                    def emit(tops, stacks=range(first, last + 1)):
+                        for j, i in enumerate(stacks):
+                            print(f'{video_path} @ frames ({i * step}, {i * step + T})')
+                            print_top_predictions(*(t[j:j + 1] for t in tops[0]), 'kinetics')
+                    preds.submit([(head, outs[-1])], emit)
             state["next"], state["slot"] = last + 1, s ^ 1
             while kept and kept[0][0] < state["next"] * step:
                 kept.popleft()
@@ -182,6 +200,8 @@ class ExtractR21D(torch.nn.Module):
         n_stacks = (f - T) // step + 1 if f >= T else 0
         if n_stacks > state["next"]:
             submit(n_stacks - 1)
+        if preds is not None:
+            preds.flush()
         # one device->host copy per video; float64 like the reference's `.tolist()` -> np.array
         feats = torch.cat(outs).cpu().numpy().astype(np.float64) if outs else np.array([])
         return {self.feature_type: feats}

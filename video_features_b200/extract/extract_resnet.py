@@ -8,6 +8,8 @@ OpenCV (a failed FIRST read is skipped, extract_resnet.py:130-137).  Underneath,
   -> fused BGR->RGB swap + CenterCrop(224) + ToTensor + Normalize + ResNet trunk (vf_resnet_forward_u8)
 The engine call is asynchronous, so decoding the next chunk overlaps the network on the current one; the features stay
 on the device until the video is finished (one device->host copy per video).
+``--show_pred``: after every engine call the checkpoint's ``fc`` runs on its device features (class_head.py) and the
+ImageNet top-5 of each frame is printed in frame order, as the reference prints per batch (extract_resnet.py:105-114).
 """
 from __future__ import annotations
 
@@ -21,8 +23,9 @@ from tqdm import tqdm
 
 from .. import ops
 from .._lib import VF_FILTER_BILINEAR
+from ..class_head import FC_KEYS, ClassHead, TopKQueue
 from ..resnet_engine import DEPTHS, ResNetEngine
-from ..utils import AsyncSink, action_on_extraction, already_extracted, form_list_from_user_input
+from ..utils import AsyncSink, action_on_extraction, already_extracted, form_list_from_user_input, print_top_predictions
 
 RESIZE_SIZE = 256
 CENTER_CROP_SIZE = 224
@@ -77,6 +80,7 @@ class ExtractResNet(torch.nn.Module):
         self.progress = tqdm(total=len(self.path_list))
         self.keep_features = False
         self._engines: Dict[int, ResNetEngine] = {}
+        self._heads: Dict[int, ClassHead] = {}
         self._pinned: Dict[tuple, List[torch.Tensor]] = {}
 
     def forward(self, indices: torch.LongTensor):
@@ -117,6 +121,13 @@ class ExtractResNet(torch.nn.Module):
             self._engines[idx] = ResNetEngine(load_resnet_weights(self.depth), self.depth, idx, max_frames=FRAMES_PER_CALL)
         return self._engines[idx]
 
+    def _head(self, device: torch.device) -> ClassHead:
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        if idx not in self._heads:
+            self._heads[idx] = ClassHead.from_state_dict(load_resnet_weights(self.depth), FC_KEYS, idx,
+                                                         f"resnet{self.depth} checkpoint")
+        return self._heads[idx]
+
     def _staging(self, shape) -> List[torch.Tensor]:
         """Two pinned (FRAMES_PER_CALL, H, W, 3) uint8 staging buffers per frame size: one fills while the other's
         host->device copy runs."""
@@ -128,6 +139,8 @@ class ExtractResNet(torch.nn.Module):
     def extract(self, device: torch.device, model=None, classifier=None, video_path=None) -> Dict[str, np.ndarray]:
         import cv2
         eng = self._engine(device)
+        head = self._head(device) if self.show_pred else None
+        preds = TopKQueue() if self.show_pred else None
         cap = cv2.VideoCapture(video_path)
         fps = cap.get(cv2.CAP_PROP_FPS)
         timestamps_ms, outs = [], []
@@ -144,6 +157,8 @@ class ExtractResNet(torch.nn.Module):
                 if (oh, ow) != (h, w):
                     x = torch.ops.vfeat.resize_u8(x, oh, ow, VF_FILTER_BILINEAR)      # ToPILImage -> Resize(256)
                 outs.append(eng.forward_u8(x))
+                if head is not None:                # only the top-5 crosses to the host, printed one call later
+                    preds.submit([(head, outs[-1])], lambda tops: print_top_predictions(*tops[0], 'imagenet'))
 
         first_frame = True
         while cap.isOpened():
@@ -167,6 +182,8 @@ class ExtractResNet(torch.nn.Module):
             if k == FRAMES_PER_CALL:
                 submit(slot, k)
                 slot, k = slot ^ 1, 0
+        if preds is not None:
+            preds.flush()
         # one device->host copy per video; float64 like the reference's `.tolist()` -> np.array
         feats = torch.cat(outs).cpu().numpy().astype(np.float64) if outs else np.array([])
         return {self.feature_type: feats, 'fps': np.array(fps), 'timestamps_ms': np.array(timestamps_ms)}

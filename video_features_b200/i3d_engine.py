@@ -1,5 +1,8 @@
 """I3D feature extractor handle: stands where the reference keeps ``I3D(num_classes=400, modality=...)`` with its
-checkpoint loaded (models/i3d/extract_i3d.py:109-118); ``engine(x, features=True)`` mirrors ``model(x, features=True)``.
+checkpoint loaded (models/i3d/extract_i3d.py:109-118); ``engine(x, features=True)`` mirrors ``model(x, features=True)``
+and ``engine(x, features=False)`` mirrors ``model(x, features=False)``: the checkpoint's conv3d_0c_1x1 head applied to the
+1024-d feature by the classifier-head kernel (class_head.py).  The head is linear and dropout is the identity in eval,
+so ``W . mean_t(pooled) + b`` equals the reference's conv-per-position-then-mean up to rounding; the trunk runs once.
 """
 from __future__ import annotations
 
@@ -11,6 +14,7 @@ import torch
 
 from . import ops  # noqa: F401  (registers torch.ops.vfeat.*)
 from ._lib import I3D_UNITS, I3DWeights, check, lib, read_split_conv
+from .class_head import I3D_KEYS, ClassHead
 
 _MIXED = ["mixed_3b", "mixed_3c", "mixed_4b", "mixed_4c", "mixed_4d", "mixed_4e", "mixed_4f", "mixed_5b", "mixed_5c"]
 
@@ -58,19 +62,29 @@ class I3DEngine:
         check(lib().vf_i3d_create(C.byref(h), C.byref(w), self.cin, device, max_stacks, max_T))
         self._h = h
         del keep
+        # the classifier head is uploaded on first use only: without it the checkpoint needs no head keys
+        self._head_sd = {k: v for k, v in state_dict.items() if k.endswith(I3D_KEYS)}
+        self._class_head = None
 
-    def __call__(self, x: torch.Tensor, features: bool = True) -> torch.Tensor:
-        """x (B, C, T, 224, 224) float on this device, values in [-1, 1] -> (B, 1024) float32."""
-        if not features:
-            raise NotImplementedError("only features=True (the extraction path) is built")
+    def head(self) -> ClassHead:
+        """The checkpoint's conv3d_0c_1x1 (400 x 1024) as a ClassHead on this device (KeyError without it)."""
+        if self._class_head is None:
+            self._class_head = ClassHead.from_state_dict(self._head_sd, I3D_KEYS, self.device.index, "I3D checkpoint")
+        return self._class_head
+
+    def __call__(self, x: torch.Tensor, features: bool = True):
+        """x (B, C, T, 224, 224) float on this device, values in [-1, 1] -> (B, 1024) float32; with
+        ``features=False`` -> (softmax, logits), each (B, 400) float32, as the reference's I3D returns them."""
         if not x.is_cuda:
             raise RuntimeError("I3DEngine expects CUDA input (no CPU fallback)")
         x = x.to(torch.float32).contiguous()
         assert x.dim() == 5 and x.shape[1] == self.cin and tuple(x.shape[3:]) == (224, 224), x.shape
-        return torch.ops.vfeat.i3d_forward(int(self._h.value), x)             # PyTorch custom op over vf_i3d_forward_f32
+        y = torch.ops.vfeat.i3d_forward(int(self._h.value), x)                # PyTorch custom op over vf_i3d_forward_f32
+        return y if features else self.head()(y)
 
-    def forward_frames_u8(self, frames: torch.Tensor) -> torch.Tensor:
-        """rgb stream from resized uint8 frames (n, T, Hr, Wr, 3) on this device; crop/scale/permute fused."""
+    def forward_frames_u8(self, frames: torch.Tensor, features: bool = True):
+        """rgb stream from resized uint8 frames (n, T, Hr, Wr, 3) on this device; crop/scale/permute fused.
+        ``features=False`` -> (softmax, logits) as in __call__."""
         assert frames.is_cuda and frames.dtype == torch.uint8 and frames.dim() == 5 and frames.shape[4] == 3
         n, T, Hr, Wr, _ = frames.shape
         fsz = Hr * Wr * 3
@@ -84,7 +98,7 @@ class I3DEngine:
         with torch.cuda.device(self.device):
             check(lib().vf_i3d_forward_u8_strided(self._h, frames.data_ptr(), n, T, stride, Hr, Wr, out.data_ptr(),
                                                   torch.cuda.current_stream().cuda_stream))
-        return out
+        return out if features else self.head()(out)
 
     def forward_frames_u8_host(self, frames: torch.Tensor, T: int, group: int = 8, wait: bool = True):
         """rgb stream from HOST stacks (n, >=T, Hr, Wr, 3) uint8 (pinned memory for asynchronous copies): the first T
@@ -131,8 +145,9 @@ class I3DEngine:
             main.synchronize()
         return out
 
-    def forward_flow(self, flow: torch.Tensor) -> torch.Tensor:
-        """flow stream from raw optical flow (n, T, 2, H, W) fp32 on this device; T3 transform fused."""
+    def forward_flow(self, flow: torch.Tensor, features: bool = True):
+        """flow stream from raw optical flow (n, T, 2, H, W) fp32 on this device; T3 transform fused.
+        ``features=False`` -> (softmax, logits) as in __call__."""
         assert flow.is_cuda and flow.dtype == torch.float32 and flow.dim() == 5 and flow.shape[2] == 2
         flow = flow.contiguous()
         n, T, _, H, W = flow.shape
@@ -140,7 +155,7 @@ class I3DEngine:
         with torch.cuda.device(self.device):
             check(lib().vf_i3d_forward_flow(self._h, flow.data_ptr(), n, T, H, W, out.data_ptr(),
                                             torch.cuda.current_stream().cuda_stream))
-        return out
+        return out if features else self.head()(out)
 
     def read_stage(self, stage: int) -> torch.Tensor:
         """Diagnostics: a retained internal activation of the last forward as fp32 (n, C, T, H, W)."""
@@ -163,6 +178,9 @@ class I3DEngine:
         return int(lib().vf_i3d_launch_count(self._h))
 
     def close(self):
+        if getattr(self, "_class_head", None) is not None:
+            self._class_head.close()
+            self._class_head = None
         if getattr(self, "_h", None):
             lib().vf_i3d_destroy(self._h)
             self._h = None

@@ -6,7 +6,7 @@ stream to libvfeat.so.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional
+from typing import List, Optional
 
 import numpy as np
 import torch
@@ -114,6 +114,30 @@ def i3d_forward(handle: int, x: torch.Tensor) -> torch.Tensor:
 @i3d_forward.register_fake
 def _(handle, x):
     return x.new_empty((x.shape[0], 1024), dtype=torch.float32)
+
+
+@torch.library.custom_op("vfeat::class_head", mutates_args=())
+def class_head(handle: int, feats: torch.Tensor, n_classes: int, k: int) -> List[torch.Tensor]:
+    """Classifier head (vf_head_forward): (n, K) fp32 features on the device -> [logits (n, C), probs (n, C),
+    top_idx (n, k) int32, top_logit (n, k), top_prob (n, k)].  `handle` is the vf_head_t* of a ClassHead."""
+    _need_cuda(feats)
+    assert feats.dtype == torch.float32 and feats.dim() == 2
+    n, K = feats.shape
+    f32 = dict(device=feats.device, dtype=torch.float32)
+    logits, probs = torch.empty((n, n_classes), **f32), torch.empty((n, n_classes), **f32)
+    idx = torch.empty((n, k), device=feats.device, dtype=torch.int32)
+    tl, tp = torch.empty((n, k), **f32), torch.empty((n, k), **f32)
+    with torch.cuda.device(feats.device):
+        check(lib().vf_head_forward(C.c_void_p(handle), feats.data_ptr(), n, K, logits.data_ptr(), probs.data_ptr(), k,
+                                    idx.data_ptr(), tl.data_ptr(), tp.data_ptr(), _stream()))
+    return [logits, probs, idx, tl, tp]
+
+
+@class_head.register_fake
+def _(handle, feats, n_classes, k):
+    n = feats.shape[0]
+    f = feats.new_empty
+    return [f((n, n_classes)), f((n, n_classes)), f((n, k), dtype=torch.int32), f((n, k)), f((n, k))]
 
 
 # ----------------------------------------------------------------------------- transforms

@@ -8,6 +8,7 @@ reference's thin wrapper over ``cv2.VideoCapture``; it is not installed here).
 from __future__ import annotations
 
 import argparse
+import functools
 import os
 import pathlib as plb
 import pickle
@@ -212,6 +213,50 @@ class AsyncSink:
     def __exit__(self, *exc):
         self.close()
         return False
+
+
+@functools.lru_cache(maxsize=None)
+def _class_names(dataset: str):
+    if dataset == 'kinetics':
+        from torchvision.models.video import R2Plus1D_18_Weights
+        return tuple(R2Plus1D_18_Weights.KINETICS400_V1.meta["categories"])
+    if dataset == 'imagenet':
+        from torchvision.models import ResNet50_Weights
+        return tuple(ResNet50_Weights.IMAGENET1K_V1.meta["categories"])
+    raise NotImplementedError
+
+
+def class_names(dataset: str) -> List[str]:
+    """Class names of 'imagenet' (1000) or 'kinetics' (400), from the metadata torchvision ships with its weight enums
+    (no download).  The Kinetics list equals the reference's K400_label_map.txt; the ImageNet names are the first name
+    of each IN_label_map.txt line (two differ in spelling: 'crane bird', 'maillot tank suit')."""
+    return list(_class_names(dataset))
+
+
+def print_top_predictions(top_idx, top_logit, top_prob, dataset: str, classes: Optional[List[str]] = None):
+    """Per row, the reference's lines `{logit:.3f} {softmax:.3f} {class}` for each of the k entries, then an empty
+    line (utils/utils.py:44-47); top_* are (n, k) host tensors, as ClassHead.top_k_host returns them."""
+    classes = _class_names(dataset) if classes is None else classes
+    for idx, lg, pr in zip(top_idx.tolist(), top_logit.tolist(), top_prob.tolist()):
+        for i, logit, smax in zip(idx, lg, pr):
+            print(f'{logit:.3f} {smax:.3f} {classes[i]}')
+        print()
+
+
+def show_predictions_on_dataset(logits, dataset: str, classes: Optional[List[str]] = None):
+    """utils/utils.py:19-47 on (B, classes) logits that are already at hand: softmax, sorted descending (equal
+    probabilities by the lower class index), the top 5 printed per row.  The extractors do not come through here:
+    they print the top-k the classifier-head kernel returns (print_top_predictions)."""
+    import torch
+    import torch.nn.functional as F
+    if dataset not in ('imagenet', 'kinetics'):
+        raise NotImplementedError
+    logits = torch.as_tensor(logits)
+    softmaxes = F.softmax(logits, dim=-1)
+    _, top_idx = torch.sort(softmaxes, dim=-1, descending=True, stable=True)
+    k = 5
+    top_idx = top_idx[:, :k]
+    print_top_predictions(top_idx, logits.gather(1, top_idx), softmaxes.gather(1, top_idx), dataset, classes)
 
 
 def form_slices(size: int, stack_size: int, step_size: int):
