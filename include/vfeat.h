@@ -404,6 +404,34 @@ int vf_vggish_conv(const vf_vggish_t* h, int index, int* geom, uint64_t* lo_mask
  * as the resampling kernel evaluates it. */
 int vf_vggish_time_register(int sample_rate, int64_t t0, int64_t count, double* out);
 
+/* ---- S3D clip features: torchvision `s3d()` in eval mode, the 1024-d `avgpool(features(x)).mean((2, 3, 4))`, and the
+ * S3D_Weights.KINETICS400_V1 clip transform.  Weights: the torchvision state_dict by key (optionally with the "module."
+ * prefix), HOST fp32; classifier.* is ignored.  A missing / mis-sized tensor is VF_ERR_INVALID. */
+typedef struct vf_s3d vf_s3d_t;
+
+/* Workspace holds max_clips clips of max_T frames (0 = 2 and 64; max_T >= 13); a call runs in chunks of as many clips
+ * of its T as the workspace holds (at most 256), so device memory does not grow with the call. */
+int vf_s3d_create(vf_s3d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips, int max_T);
+int vf_s3d_destroy(vf_s3d_t* h);
+/* clips: n x 3 x T x 224 x 224 fp32 on the device, already transformed; T >= 13 (the smallest clip whose (2,7,7)
+ * average pool has a position) -> out: n x 1024 fp32. */
+int vf_s3d_forward_f32(vf_s3d_t* h, const float* clips, int n, int T, float* out, void* stream);
+/* transform fused: frames n_frames x H x W x 3 uint8 BGR on the device (the decoder's order, any size); clip i is
+ * frames starts[i] .. starts[i] + T - 1 (starts: HOST array of n ints) -> BGR->RGB, bilinear Resize((256, 256)) on
+ * uint8 of the 224 x 224 CenterCrop window, /255, Normalize -> network -> out: n x 1024 fp32.  A frame that several
+ * clips of one chunk share is transformed once. */
+int vf_s3d_forward_u8(vf_s3d_t* h, const uint8_t* frames, int n_frames, int H, int W, const int* starts, int n, int T,
+                      float* out, void* stream);
+/* Diagnostics: an activation of the last chunk of the last call as fp32 NCTHW: stage 0 stem (after the temporal conv),
+ * 1 features.3 (the separable conv before the second pool), 2 Mixed 3c, 3 Mixed 4f, 4 Mixed 5c.  dims5 receives
+ * (n, C, T, H, W); out == NULL only queries the shape. */
+int vf_s3d_read_stage(vf_s3d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream);
+int64_t vf_s3d_launch_count(const vf_s3d_t* h);
+/* Diagnostics: conv `index` as uploaded, in execution order (the stem's spatial and temporal convs, features.2,
+ * features.3's spatial and temporal convs, then per Mixed block branch0, branch1's 1x1x1, spatial and temporal convs,
+ * branch2's likewise, branch3's 1x1x1); the rest as vf_r21d_conv. */
+int vf_s3d_conv(const vf_s3d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),
  * and the softmax + sort of utils/utils.py:19-47.  weight: n_classes x n_features, bias: n_classes, HOST fp32. */

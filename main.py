@@ -1,6 +1,9 @@
 """CLI of the H100-native video-feature engine: the flags of the reference's main.py (main.py:93-149), same names,
 defaults and choices.  ``--device_ids`` starts one process per GPU (reference: one thread per GPU); ``--cpu`` is
 refused -- the reference's CPU path is what ``bench.py --impl reference`` times, the engine itself has no CPU path.
+Beyond the reference: ``--gather_features`` (one all-gather of every GPU's features into one .npz) and the ``s3d``
+feature type (torchvision's S3D, the Kinetics-400 clip feature upstream video_features added later), the first choice
+outside the reference's list.
 """
 import argparse
 import functools
@@ -11,7 +14,7 @@ import torch  # noqa: F401
 from video_features_b200.utils import form_list_from_user_input, sanity_check
 
 SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
-             'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch']
+             'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch', 's3d']
 
 
 def build_extractor(args):
@@ -34,6 +37,9 @@ def build_extractor(args):
     if args.feature_type == 'r21d_rgb':
         from video_features_b200.extract.extract_r21d import ExtractR21D
         return ExtractR21D(args)
+    if args.feature_type == 's3d':
+        from video_features_b200.extract.extract_s3d import ExtractS3D
+        return ExtractS3D(args)
     if args.feature_type == 'vggish_torch':
         from video_features_b200.extract.extract_vggish import ExtractVGGish
         return ExtractVGGish(args)
@@ -73,7 +79,7 @@ def parallel_feature_extraction(args):
 
 
 _FEATURE_TYPES = ('i3d vggish r21d_rgb resnet18 resnet34 resnet50 resnet101 resnet152 raft pwc CLIP-ViT-B/32 CLIP-ViT-B/16 '
-                  'CLIP4CLIP-ViT-B-32 vggish_torch').split()
+                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d').split()
 
 # (flag, argparse keywords): names, types, defaults, choices and dests are the reference's (main.py:93-149)
 _FLAGS = [
@@ -92,8 +98,8 @@ _FLAGS = [
     ('--output_direct', dict(action='store_true', help='save as <output_path>/<video stem>.npy')),
     ('--extraction_fps', dict(type=float, help='resample to this frame rate first (I3D)')),
     ('--extract_method', dict(type=str, help='frame sampler: uni_N or fix_N')),
-    ('--stack_size', dict(type=int, help='frames per I3D / R(2+1)D stack')),
-    ('--step_size', dict(type=int, help='frames between I3D / R(2+1)D stacks')),
+    ('--stack_size', dict(type=int, help='frames per I3D / R(2+1)D / S3D stack')),
+    ('--step_size', dict(type=int, help='frames between I3D / R(2+1)D / S3D stacks')),
     ('--streams', dict(nargs='+', choices=['flow', 'rgb'], help='I3D streams (default: both)')),
     ('--flow_type', dict(choices=['raft', 'pwc', 'flow'], default='pwc', help='optical flow feeding the I3D flow stream')),
     ('--batch_size', dict(type=int, default=1, help='frame pairs per RAFT call')),
@@ -101,7 +107,7 @@ _FLAGS = [
                                     help='--side_size applies to the larger edge instead of the smaller one')),
     ('--side_size', dict(type=int, help='RAFT: resize frames to this edge length first')),
     ('--show_pred', dict(dest='show_pred', action='store_true', default=False,
-                         help='print the top-5 classes of every feature (I3D, R(2+1)D: Kinetics-400; ResNet: ImageNet)')),
+                         help='print the top-5 classes of every feature (I3D, R(2+1)D, S3D: Kinetics-400; ResNet: ImageNet)')),
     # not in the reference: after extraction, ONE all-gather (NCCL over NVLink) returns every rank's feature blocks and
     # rank 0 writes them, list order, to this .npz
     ('--gather_features', dict(type=str, default=None, help='also all-gather the features of all GPUs into this .npz')),

@@ -139,6 +139,15 @@ SIGNATURES = {
     "vf_r21d_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_r21d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                                C.c_void_p, C.c_void_p]),
+    "vf_s3d_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vf_s3d_destroy": (C.c_int, [C.c_void_p]),
+    "vf_s3d_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_s3d_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int,
+                                    C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_s3d_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_s3d_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_s3d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
+                              C.c_void_p, C.c_void_p]),
     "vf_clip_rn_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
     "vf_clip_rn_destroy": (C.c_int, [C.c_void_p]),
     "vf_clip_rn_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
@@ -196,8 +205,8 @@ def check(status: int) -> None:
 
 
 def read_conv(fn, handle, index: int, device):
-    """Diagnostics shared by ResNetEngine.conv / R21DEngine.conv / ClipResNetEngine.conv: fn is vf_resnet_conv,
-    vf_r21d_conv or vf_clip_rn_conv.  Returns dict
+    """Diagnostics shared by ResNetEngine.conv / R21DEngine.conv / S3DEngine.conv / ClipResNetEngine.conv: fn is
+    vf_resnet_conv, vf_r21d_conv, vf_s3d_conv or vf_clip_rn_conv.  Returns dict
     n_out, ntaps, k_per_tap, shifts [(dt, dh, dw)] per tap, lo_mask, w (fp16 [n_out, 2 ntaps k_per_tap], W_hi | W_lo),
     scale, bias (fp32 [n_out]) as uploaded."""
     import torch
