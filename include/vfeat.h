@@ -370,6 +370,37 @@ int64_t vf_clip_rn_launch_count(const vf_clip_rn_t* h);
  * four phase slots and 1/4 in its scale. */
 int vf_clip_rn_conv(const vf_clip_rn_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
+/* ---- CLIP ViT-L/14 image towers (224 px, 257 tokens; 336 px, 577 tokens): replace `clip.load("ViT-L/14" |
+ * "ViT-L/14@336px")` and `model.encode_image(preprocess(frame))` with its transform Resize(n_px, bicubic) ->
+ * CenterCrop(n_px) -> ToTensor -> Normalize.  Weights: openai's `visual.*` keys, HOST fp32 (other keys are ignored).
+ * Width, patch, depth, heads, n_px and output width are inferred from the sizes as clip.model.build_model does; exactly
+ * (1024, 14, 24, 16, 224 | 336, 768) is accepted, anything else is refused naming the key. */
+typedef struct vf_clip_vitl vf_clip_vitl_t;
+
+/* Workspace holds max_frames frames (0 = 352 at 224 px, 160 at 336 px: about 2.5 GB); larger calls run in chunks. */
+int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_frames);
+int vf_clip_vitl_destroy(vf_clip_vitl_t* h);
+/* info receives 8 ints: out_dim (768), n_px, width, layers, heads, patch, tokens, max_frames. */
+int vf_clip_vitl_info(const vf_clip_vitl_t* h, int* info);
+/* frames: n x 3 x n_px x n_px fp32 on the device, already transformed -> out: n x 768 fp32 on the device. */
+int vf_clip_vitl_encode_f32(vf_clip_vitl_t* h, const float* frames, int n, float* out, void* stream);
+/* transform fused: frames n x H x W x 3 uint8 on the device, any size, channel order untouched -> Pillow-exact bicubic
+ * resize of the short side to n_px, CenterCrop(n_px), ToTensor, Normalize -> tower.  Bit-identical to
+ * vf_clip_vitl_encode_f32 on the same transformed frames. */
+int vf_clip_vitl_encode_u8(vf_clip_vitl_t* h, const uint8_t* frames, int n, int H, int W, float* out, void* stream);
+/* Diagnostics, eager, n <= max_frames, on `stream`: the embedding (patch GEMM, tokens, ln_pre) -> x_out n x tokens x
+ * 1024 fp32; resblocks [layer_begin, layer_end) in place on x (block 23 updates the class rows only); ln_post + proj
+ * on the class rows of x -> out n x 768. */
+int vf_clip_vitl_debug_embed_f32(vf_clip_vitl_t* h, const float* frames, int n, float* x_out, void* stream);
+int vf_clip_vitl_debug_embed_u8(vf_clip_vitl_t* h, const uint8_t* frames, int n, int H, int W, float* x_out,
+                                void* stream);
+int vf_clip_vitl_debug_blocks(vf_clip_vitl_t* h, float* x, int n, int layer_begin, int layer_end, void* stream);
+int vf_clip_vitl_debug_head(vf_clip_vitl_t* h, const float* x, int n, float* out, void* stream);
+/* The tower's attention on caller rows: qkv n_frames x tokens x 3072 fp16 (q | k | v after the bias, 16 heads of 64)
+ * -> out n_frames x tokens x 1024 fp16; 1 <= tokens <= 577. */
+int vf_clip_vitl_attention(vf_clip_vitl_t* h, const void* qkv, int n_frames, int tokens, void* out, void* stream);
+int64_t vf_clip_vitl_launch_count(const vf_clip_vitl_t* h);
+
 /* ---- VGGish audio embeddings (torchvggish VGG, postprocess=False): replaces models/vggish_torch's
  * vggish_input.wavfile_to_examples + VGG.forward for PCM-16 samples.  Weights: torchvggish keys features.{0,3,6,8,11,13}
  * and embeddings.{0,2,4} (.weight / .bias), HOST fp32.  The front end's float64 tables come from the caller: hann[400]

@@ -3,7 +3,8 @@ defaults and choices.  ``--device_ids`` starts one process per GPU (reference: o
 refused -- the reference's CPU path is what ``bench.py --impl reference`` times, the engine itself has no CPU path.
 Beyond the reference: ``--gather_features`` (one all-gather of every GPU's features into one .npz) and the ``s3d``
 feature type (torchvision's S3D, the Kinetics-400 clip feature upstream video_features added later), the first choice
-outside the reference's list.
+outside the reference's list, and the ``CLIP-ViT-L/14`` / ``CLIP-ViT-L/14@336px`` feature types (openai's largest
+released ViT, 768-d features), which the reference does not offer either.
 """
 import argparse
 import functools
@@ -14,12 +15,12 @@ import torch  # noqa: F401
 from video_features_b200.utils import form_list_from_user_input, sanity_check
 
 SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
-             'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch', 's3d']
+             'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch', 's3d', 'CLIP-ViT-L/14', 'CLIP-ViT-L/14@336px']
 
 
 def build_extractor(args):
     """feature_type -> extractor (main.py:15-41)."""
-    if args.feature_type in ['CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32']:
+    if args.feature_type in ['CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'CLIP-ViT-L/14', 'CLIP-ViT-L/14@336px']:
         from video_features_b200.extract.extract_clip import ExtractCLIP
         return ExtractCLIP(args)
     if args.feature_type == 'i3d':
@@ -79,7 +80,7 @@ def parallel_feature_extraction(args):
 
 
 _FEATURE_TYPES = ('i3d vggish r21d_rgb resnet18 resnet34 resnet50 resnet101 resnet152 raft pwc CLIP-ViT-B/32 CLIP-ViT-B/16 '
-                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d').split()
+                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d CLIP-ViT-L/14 CLIP-ViT-L/14@336px').split()
 
 # (flag, argparse keywords): names, types, defaults, choices and dests are the reference's (main.py:93-149)
 _FLAGS = [

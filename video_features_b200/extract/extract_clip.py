@@ -5,7 +5,8 @@ changes underneath: ``clip.load`` is replaced by a ``ClipEngine`` (device weight
 ``model.encode_image`` by ONE call into libvfeat.so that takes the decoder's raw uint8 frames and runs the
 Pillow-exact bicubic resize, centre crop, normalisation and the ViT-B/32 tower on the GPU.  The ResNet towers
 (``CLIP-RN50``, ``CLIP-RN101``, ``CLIP-RN50x4``, ``CLIP-RN50x16``) run on a ``ClipResNetEngine`` behind the same
-calls, at their own input size (224, 224, 288, 384) and output width (1024, 512, 640, 768).
+calls, at their own input size (224, 224, 288, 384) and output width (1024, 512, 640, 768), and so do the ViT-L/14
+towers (``CLIP-ViT-L/14``, ``CLIP-ViT-L/14@336px``: 224 / 336 px, 768-d) on a ``ClipViTLEngine``.
 
 A list of videos does not go through the engine one 12-frame video at a time (600 token rows would fill 3 of the
 GEMM's 74 tile slots): ``forward`` decodes ahead on a thread pool, packs the frames of consecutive videos of equal
@@ -37,13 +38,16 @@ from tqdm import tqdm
 from .. import synthetic_weights
 from ..clip_engine import ClipEngine
 from ..clip_resnet_engine import ClipResNetEngine
+from ..clip_vitl_engine import ClipViTLEngine
 from ..utils import (AsyncSink, FrameStream, action_on_extraction, already_extracted, extract_frames,
                      form_list_from_user_input)
 
 # the ResNet towers' names are the basenames clip.load caches its downloads under
 _RN_CKPT_NAMES = {'CLIP-RN50': 'RN50.pt', 'CLIP-RN101': 'RN101.pt', 'CLIP-RN50x4': 'RN50x4.pt', 'CLIP-RN50x16': 'RN50x16.pt'}
+# the ViT-L/14 towers likewise (clip.load's names for "ViT-L/14" and "ViT-L/14@336px")
+_VITL_CKPT_NAMES = {'CLIP-ViT-L/14': 'ViT-L-14.pt', 'CLIP-ViT-L/14@336px': 'ViT-L-14-336px.pt'}
 _CKPT_NAMES = {'CLIP-ViT-B/32': 'ViT-B-32.pt', 'CLIP-ViT-B/16': 'ViT-B-16.pt', 'CLIP4CLIP-ViT-B-32': 'CLIP4CLIP-ViT-B-32.pth',
-               **_RN_CKPT_NAMES}
+               **_RN_CKPT_NAMES, **_VITL_CKPT_NAMES}
 
 
 def read_clip_checkpoint(path: str) -> Dict[str, torch.Tensor]:
@@ -67,6 +71,8 @@ def load_clip_state_dict(feature_type: str) -> Dict[str, torch.Tensor]:
     it does not apply to the ResNet towers."""
     if os.environ.get("VF_CLIP_SYNTHETIC") is not None and feature_type not in _RN_CKPT_NAMES:
         seed, outliers = synthetic_weights.parse_env(os.environ["VF_CLIP_SYNTHETIC"])
+        if feature_type in _VITL_CKPT_NAMES:
+            return synthetic_weights.clip_vit_l14_state_dict(seed, outliers, n_px=336 if feature_type.endswith('336px') else 224)
         return synthetic_weights.clip_vit_b32_state_dict(seed, outliers, patch=16 if feature_type.endswith('/16') else 32)
     name = _CKPT_NAMES[feature_type]
     cands = [os.environ.get("VF_CLIP_CKPT"), os.path.join(pathlib.Path(__file__).parent, 'checkpoints', name),
@@ -127,7 +133,7 @@ class ExtractCLIP(torch.nn.Module):
             self.output_direct = args.output_direct
             self.output_path = args.output_path if self.output_direct is True else os.path.join(args.output_path, self.feature_type)
         self.progress = tqdm(total=len(self.path_list))
-        self._engines: Dict[int, object] = {}             # ClipEngine or ClipResNetEngine
+        self._engines: Dict[int, object] = {}             # ClipEngine, ClipResNetEngine or ClipViTLEngine
         # engine-side knobs (not in the reference): where frames come from, and how many go into one engine call
         self.frame_source = extract_frames                  # (path, method) -> (frames, fps, timestamps_ms)
         # two-step source used by the list path: stream = frame_stream(path, method) knows .count / .hw / .fps /
@@ -155,6 +161,8 @@ class ExtractCLIP(torch.nn.Module):
             sd = load_clip_state_dict(self.feature_type)
             if self.feature_type in _RN_CKPT_NAMES:
                 self._engines[idx] = ClipResNetEngine(sd, device=idx)
+            elif self.feature_type in _VITL_CKPT_NAMES:
+                self._engines[idx] = ClipViTLEngine(sd, device=idx)
             else:
                 self._engines[idx] = ClipEngine(sd, device=idx)
         return self._engines[idx]

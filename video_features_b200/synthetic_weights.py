@@ -17,11 +17,22 @@ def clip_vit_b16_state_dict(seed: int = 0, outliers: bool = False) -> "OrderedDi
 
 
 def clip_vit_b32_state_dict(seed: int = 0, outliers: bool = False, patch: int = PATCH) -> "OrderedDict[str, torch.Tensor]":
+    """openai ``visual.*`` key layout, fp32 (see ``_vit_state_dict``)."""
+    return _vit_state_dict(seed, outliers, WIDTH, LAYERS, patch, 224, EMBED)
+
+
+def clip_vit_l14_state_dict(seed: int = 0, outliers: bool = False, n_px: int = 224) -> "OrderedDict[str, torch.Tensor]":
+    """The same scheme at the ViT-L/14 shape: width 1024, 24 blocks, patch 14, ``n_px`` 224 (257 tokens) or 336 (577
+    tokens), output 768."""
+    return _vit_state_dict(seed, outliers, 1024, 24, 14, n_px, 768)
+
+
+def _vit_state_dict(seed, outliers, WIDTH, LAYERS, patch, n_px, EMBED) -> "OrderedDict[str, torch.Tensor]":
     """openai ``visual.*`` key layout, fp32.  Initialisation scales are the ones openai/CLIP's
     ``initialize_parameters`` uses (width**-0.5 etc.), with perturbed LayerNorm gains / biases so that every term of the
     forward matters.
 
-    ``outliers=True`` adds what trained ViT-B/32 weights have and random ones lack: a handful of residual-stream
+    ``outliers=True`` adds what trained ViT weights have and random ones lack: a handful of residual-stream
     channels that carry magnitudes of 50-200 through every block (set up by the positional embedding and fed by the
     projection biases), LayerNorm gains with a heavy tail (a few entries near 0.05, a few above 4), and a few large
     rows in the attention / MLP output projections.  This is the regime where fp16 storage of intermediate tensors is
@@ -37,7 +48,7 @@ def clip_vit_b32_state_dict(seed: int = 0, outliers: bool = False, patch: int = 
     fc_std = (2 * WIDTH) ** -0.5
     sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
     sd["visual.class_embedding"] = rn(WIDTH, std=scale)
-    sd["visual.positional_embedding"] = rn((224 // patch) ** 2 + 1, WIDTH, std=scale)
+    sd["visual.positional_embedding"] = rn((n_px // patch) ** 2 + 1, WIDTH, std=scale)
     sd["visual.proj"] = rn(WIDTH, EMBED, std=scale)
     sd["visual.conv1.weight"] = rn(WIDTH, 3, patch, patch, std=(3 * patch * patch) ** -0.5)
     for name in ("ln_pre", "ln_post"):
@@ -51,9 +62,9 @@ def clip_vit_b32_state_dict(seed: int = 0, outliers: bool = False, patch: int = 
         sd[p + "attn.out_proj.bias"] = rn(WIDTH, std=0.02)
         sd[p + "ln_1.weight"] = 1.0 + rn(WIDTH, std=0.1)
         sd[p + "ln_1.bias"] = rn(WIDTH, std=0.05)
-        sd[p + "mlp.c_fc.weight"] = rn(MLP, WIDTH, std=fc_std)
-        sd[p + "mlp.c_fc.bias"] = rn(MLP, std=0.02)
-        sd[p + "mlp.c_proj.weight"] = rn(WIDTH, MLP, std=proj_std)
+        sd[p + "mlp.c_fc.weight"] = rn(4 * WIDTH, WIDTH, std=fc_std)
+        sd[p + "mlp.c_fc.bias"] = rn(4 * WIDTH, std=0.02)
+        sd[p + "mlp.c_proj.weight"] = rn(WIDTH, 4 * WIDTH, std=proj_std)
         sd[p + "mlp.c_proj.bias"] = rn(WIDTH, std=0.02)
         sd[p + "ln_2.weight"] = 1.0 + rn(WIDTH, std=0.1)
         sd[p + "ln_2.bias"] = rn(WIDTH, std=0.05)
