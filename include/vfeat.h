@@ -227,6 +227,13 @@ int64_t vf_i3d_launch_count(const vf_i3d_t* h);
  * pass.  w (n_out x nsplit ntaps k_per_tap fp16), scale and bias (n_out fp32, the folded BatchNorm) are DEVICE buffers
  * filled when not NULL.  An index past the last unit is VF_ERR_INVALID. */
 int vf_i3d_conv(const vf_i3d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+/* Diagnostics: Mixed block `block` (0 .. 8: mixed_3b .. mixed_5c) once, on the engine's uploaded weights, buffers and
+ * kernels.  x_pairs: DEVICE fp16 pair volume [n][T+2][S+2][S+2][2 cin] (rows [hi cin | lo cin], border 1, zero border)
+ * with S = 28 (blocks 0, 1), 14 (2 .. 6), 7 (7, 8); out_pairs receives the concat pair volume [n][T+2][S+2][S+2]
+ * [2 ctot] (rows [hi ctot | lo ctot], branches in order, border rows included).  The volume goes through the engine's
+ * own activation buffers: more rows than the workspace holds is VF_ERR_INVALID before any launch, and afterwards
+ * vf_i3d_read_stage is VF_ERR_INVALID until the next forward. */
+int vf_i3d_debug_mixed(vf_i3d_t* h, int block, const void* x_pairs, int n, int T, void* out_pairs, void* stream);
 
 /* ---- RAFT optical flow: replaces `RAFT()(image1, image2, iters=20, test_mode=True)` + InputPadder
  * (models/raft/raft_src/raft.py:27-44,115-174; called at models/raft/extract_raft.py:94-104 and
@@ -462,6 +469,22 @@ int64_t vf_s3d_launch_count(const vf_s3d_t* h);
  * features.3's spatial and temporal convs, then per Mixed block branch0, branch1's 1x1x1, spatial and temporal convs,
  * branch2's likewise, branch3's 1x1x1); the rest as vf_r21d_conv. */
 int vf_s3d_conv(const vf_s3d_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+/* Diagnostics: Mixed block `block` (0 .. 8: features.5, 6, 8 .. 12, 14, 15) once, as vf_i3d_debug_mixed (same volume
+ * layout, S and rules; afterwards vf_s3d_read_stage is VF_ERR_INVALID until the next forward). */
+int vf_s3d_debug_mixed(vf_s3d_t* h, int block, const void* x_pairs, int n, int T, void* out_pairs, void* stream);
+
+/* ---- diagnostics of the pool and head kernels I3D and S3D share.  A volume is 10 ints: n, Tp, Hp, Wp (the padded
+ * extents of a channels-last volume of pair rows [hi C | lo C]), then t0, t1, h0, h1, w0, w1 (its valid region). */
+#define VF_POOL_GENERAL 0   /* bounds-checked kernel, any window */
+#define VF_POOL_FAST 1      /* fixed windows 1x3x3/1x2x2, 3x3x3/2, 2x2x2/2 with no leading padding, every window
+                               inside the input's padded extent */
+#define VF_POOL_SAME3 2     /* 3x3x3 / 1 pad 1 onto the input's own geometry, border >= 1: the rolling-max kernel */
+/* Max pool of the valid region with zero padding (k, s, p: kt kh kw, st sh sw, pt ph pw), pair rows in and out, border
+ * rows of the output written as zeros; path receives the VF_POOL_* kernel that ran.  C must be a multiple of 8. */
+int vf_debug_maxpool3d(const void* in, const int* vol_in, void* out, const int* vol_out, int C, const int* k,
+                       const int* s, const int* p, int* path, void* stream);
+/* AvgPool3d((2,7,7), 1) of a T3 (>= 2) x 7 x 7 valid region, then the mean over time: out n x C fp32. */
+int vf_debug_i3d_head(const void* in, const int* vol, int C, float* out, void* stream);
 
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),

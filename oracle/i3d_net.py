@@ -114,6 +114,15 @@ def _maxpool(x, k, s):
     return F.max_pool3d(x, k, s, ceil_mode=True)
 
 
+def _fp16_sets(declared_rounding, fp16_units, fp16_inputs=(), fp16_weights=()):
+    """The ``fp16`` argument of _unit: (unit names whose input is rounded, unit names whose weights are), or None."""
+    if not (declared_rounding or fp16_inputs or fp16_weights):
+        return None
+    names = unit_names()
+    return (set(fp16_inputs) | (set(_FP16_INPUT) if declared_rounding else set()),
+            set(fp16_weights) | ({names[i] for i in fp16_units} if declared_rounding else set()))
+
+
 def _mixed(sd, m, x, fp16=None):
     b0 = _unit(sd, f"{m}.branch_0", x, 1, fp16=fp16)
     b1 = _unit(sd, f"{m}.branch_1.1", _unit(sd, f"{m}.branch_1.0", x, 1, fp16=fp16), 3, fp16=fp16)
@@ -131,11 +140,7 @@ def forward_features(sd: Dict[str, torch.Tensor], inp: torch.Tensor, return_stag
     listed at DECLARED_FP16_UNITS and the weights of the units `fp16_units` (() for an engine built with
     VF_I3D_SINGLE=none).  fp16_inputs / fp16_weights (unit names) round further conv inputs / weights (precision
     emulations: a pair tensor or a split weight left single fp16).  Stages: 1a, 2c, 3c, 4f, 5c."""
-    fp16 = None
-    if declared_rounding or fp16_inputs or fp16_weights:
-        names = unit_names()
-        fp16 = (set(fp16_inputs) | (set(_FP16_INPUT) if declared_rounding else set()),
-                set(fp16_weights) | ({names[i] for i in fp16_units} if declared_rounding else set()))
+    fp16 = _fp16_sets(declared_rounding, fp16_units, fp16_inputs, fp16_weights)
     st = {}
     x = _unit(sd, "conv3d_1a_7x7", inp, 7, 2, fp16=fp16); st["1a"] = x
     x = _maxpool(x, (1, 3, 3), (1, 2, 2))
@@ -154,6 +159,39 @@ def forward_features(sd: Dict[str, torch.Tensor], inp: torch.Tensor, return_stag
     x = F.avg_pool3d(x, (2, 7, 7), (1, 1, 1))
     out = x.squeeze(3).squeeze(3).mean(2)
     return (out, st) if return_stages else out
+
+
+@torch.no_grad()
+def mixed_block(sd: Dict[str, torch.Tensor], m: str, x: torch.Tensor, declared_rounding: bool = False,
+                fp16_units=DECLARED_FP16_UNITS, fp16_inputs=(), fp16_weights=()):
+    """Mixed block ``m`` (a key of MIXED) on x, as forward_features runs it (the same rounding arguments): the concat
+    (b0, b1, b2, b3) along channels."""
+    return _mixed(sd, m, x, _fp16_sets(declared_rounding, fp16_units, fp16_inputs, fp16_weights))
+
+
+@torch.no_grad()
+def mixed_inputs(sd: Dict[str, torch.Tensor], inp: torch.Tensor, declared_rounding: bool = False,
+                 fp16_units=DECLARED_FP16_UNITS):
+    """The input of every Mixed block (MIXED order) in forward_features(inp) with the same rounding arguments."""
+    fp16 = _fp16_sets(declared_rounding, fp16_units)
+    x = _unit(sd, "conv3d_1a_7x7", inp, 7, 2, fp16=fp16)
+    x = _maxpool(x, (1, 3, 3), (1, 2, 2))
+    x = _unit(sd, "conv3d_2b_1x1", x, 1, fp16=fp16)
+    x = _maxpool(_unit(sd, "conv3d_2c_3x3", x, 3, fp16=fp16), (1, 3, 3), (1, 2, 2))
+    ins = []
+    for m in MIXED:
+        ins.append(x)
+        x = _mixed(sd, m, x, fp16)
+        if m == "mixed_3c":
+            x = _maxpool(x, (3, 3, 3), (2, 2, 2))
+        elif m == "mixed_4f":
+            x = _maxpool(x, (2, 2, 2), (2, 2, 2))
+    return ins
+
+
+def maxpool(x: torch.Tensor, k, s) -> torch.Tensor:
+    """MaxPool3dTFPadding(k, s, 'SAME'): zero padding, then a ceil-mode max pool (the trunk's pools)."""
+    return _maxpool(x, k, s)
 
 
 def rgb_transform(stack: torch.Tensor) -> torch.Tensor:

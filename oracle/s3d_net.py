@@ -41,7 +41,10 @@ def _sep(sd, p, x, k, s, pad):
     return _cna(sd, p + ".1", x, (s, 1, 1), (pad, 0, 0))
 
 
-def _mixed(sd, p, x):
+def mixed_block(sd, i, x):
+    """SepInceptionBlock3D ``features[i]`` (i a key of MIXED) on x: the concat of its four branches."""
+    p = f"features.{i}"
+    sd = _plain(sd)
     x0 = _cna(sd, p + ".branch0", x)
     x1 = _sep(sd, p + ".branch1.1", _cna(sd, p + ".branch1.0", x), 3, 1, 1)
     x2 = _sep(sd, p + ".branch2.1", _cna(sd, p + ".branch2.0", x), 3, 1, 1)
@@ -49,28 +52,50 @@ def _mixed(sd, p, x):
     return torch.cat((x0, x1, x2, x3), 1)
 
 
+def _plain(sd):
+    """The state dict without a DataParallel "module." prefix."""
+    if not any(k.startswith("module.") for k in sd):
+        return sd
+    return {k[7:] if k.startswith("module.") else k: v for k, v in sd.items()}
+
+
+def _layer(sd, i, x):
+    """``model.features[i]`` on x (sd without the "module." prefix)."""
+    if i == 0:
+        return _sep(sd, "features.0", x, 7, 2, 3)
+    if i in (1, 4):
+        return F.max_pool3d(x, (1, 3, 3), (1, 2, 2), (0, 1, 1))
+    if i == 2:
+        return _cna(sd, "features.2", x)
+    if i == 3:
+        return _sep(sd, "features.3", x, 3, 1, 1)
+    if i == 7:
+        return F.max_pool3d(x, 3, 2, 1)
+    if i == 13:
+        return F.max_pool3d(x, 2, 2, 0)
+    return mixed_block(sd, i, x)
+
+
 def features(sd, x, taps: bool = False):
     """``model.features(x)``; with ``taps`` also {stage name: activation} (STAGES)."""
-    sd = {k[7:] if k.startswith("module.") else k: v for k, v in sd.items()}
+    sd = _plain(sd)
     st = {}
     for i in range(16):
-        if i == 0:
-            x = _sep(sd, "features.0", x, 7, 2, 3)
-        elif i in (1, 4):
-            x = F.max_pool3d(x, (1, 3, 3), (1, 2, 2), (0, 1, 1))
-        elif i == 2:
-            x = _cna(sd, "features.2", x)
-        elif i == 3:
-            x = _sep(sd, "features.3", x, 3, 1, 1)
-        elif i == 7:
-            x = F.max_pool3d(x, 3, 2, 1)
-        elif i == 13:
-            x = F.max_pool3d(x, 2, 2, 0)
-        else:
-            x = _mixed(sd, f"features.{i}", x)
+        x = _layer(sd, i, x)
         if taps and i in STAGE_AFTER:
             st[STAGE_AFTER[i]] = x
     return (x, st) if taps else x
+
+
+def mixed_inputs(sd, x):
+    """The input of every Mixed block of ``model.features(x)``, in MIXED order (features.5, 6, 8 .. 12, 14, 15)."""
+    sd = _plain(sd)
+    ins = []
+    for i in range(16):
+        if i in MIXED:
+            ins.append(x)
+        x = _layer(sd, i, x)
+    return ins
 
 
 def forward(sd, x, taps: bool = False):
@@ -86,7 +111,7 @@ def forward(sd, x, taps: bool = False):
 def logits(sd, feats):
     """classifier.1 (Conv3d 1024 -> 400 with bias) on the feature: ``model(x)`` in exact arithmetic (dropout is the
     identity in eval and the head is linear, so it commutes with the spatio-temporal mean)."""
-    sd = {k[7:] if k.startswith("module.") else k: v for k, v in sd.items()}
+    sd = _plain(sd)
     w, b = sd[HEAD_KEYS[0]], sd[HEAD_KEYS[1]]
     return feats @ w.reshape(w.shape[0], -1).to(feats.dtype).T + b.to(feats.dtype)
 

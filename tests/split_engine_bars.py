@@ -11,8 +11,9 @@ the same values).  The margin is narrow because the engine's error is its fp32 a
 differences in its single-fp16 tensors): a change to the conv GEMM's K order, pipeline staging or tile widths that
 reorders the fp32 sums can move these values by that much with no loss of precision; such a change re-measures them.
 That the engines upload every lo half, W_lo row and lo_mask bit is checked exactly, conv by conv, by
-test_conv_gemm_resnet_r21d_gpu.py and test_i3d_raft_uploads_gpu.py: that, not these bars, is the guard for a loss
-too small to show at a stage (most I3D classes past mixed_3c)."""
+test_conv_gemm_resnet_r21d_gpu.py and test_i3d_raft_uploads_gpu.py.  That read-back sees weights only; a loss too small
+to show at a stage (most I3D classes past mixed_3c, or one branch's store, conv input or pool) is guarded by the
+per-branch block tests of test_inception_blocks_gpu.py (bars in inception_block_bars.py)."""
 import torch
 
 RESNET_STAGES = ("stem", "maxpool", "layer1", "layer2", "layer3", "layer4", "features")

@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("VF_LIBVFEAT") or os.path.join(_HERE, "libvfeat.so")
 VF_OK = 0
 VF_ACT_NONE, VF_ACT_QUICKGELU, VF_ACT_RELU, VF_ACT_SIGMOID, VF_ACT_TANH, VF_ACT_LEAKY = 0, 1, 2, 3, 4, 5
 VF_FILTER_BILINEAR, VF_FILTER_BICUBIC = 2, 3
+VF_POOL_GENERAL, VF_POOL_FAST, VF_POOL_SAME3 = 0, 1, 2
 
 
 class VfError(RuntimeError):
@@ -105,6 +106,7 @@ SIGNATURES = {
     "vf_i3d_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_i3d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p,
                               C.c_void_p]),
+    "vf_i3d_debug_mixed": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_raft_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "vf_raft_destroy": (C.c_int, [C.c_void_p]),
     "vf_raft_flow": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -148,6 +150,11 @@ SIGNATURES = {
     "vf_s3d_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_s3d_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                               C.c_void_p, C.c_void_p]),
+    "vf_s3d_debug_mixed": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_debug_maxpool3d": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.POINTER(C.c_int), C.c_int,
+                                     C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                     C.c_void_p]),
+    "vf_debug_i3d_head": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p]),
     "vf_clip_rn_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
     "vf_clip_rn_destroy": (C.c_int, [C.c_void_p]),
     "vf_clip_rn_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
@@ -232,6 +239,67 @@ def read_conv(fn, handle, index: int, device):
     check(fn(handle, index, geom, C.byref(mask), w.data_ptr(), scale.data_ptr(), bias.data_ptr()))
     shifts = [tuple(geom[3 + 3 * j:6 + 3 * j]) for j in range(ntaps)]
     return dict(n_out=n_out, ntaps=ntaps, k_per_tap=kpt, shifts=shifts, lo_mask=mask.value, w=w, scale=scale, bias=bias)
+
+
+# Mixed block index (0 .. 8) -> the side S of its S x S frames, and (cin, branch 0, 1, 2, 3 widths): I3D's mixed_3b ..
+# mixed_5c and S3D's features.5 .. 15 are the same Inception widths
+MIXED_SIDE = (28, 28, 14, 14, 14, 14, 14, 7, 7)
+MIXED_WIDTHS = ((192, 64, 128, 32, 32), (256, 128, 192, 96, 64), (480, 192, 208, 48, 64), (512, 160, 224, 64, 64),
+                (512, 128, 256, 64, 64), (512, 112, 288, 64, 64), (528, 256, 320, 128, 128), (832, 256, 320, 128, 128),
+                (832, 384, 384, 128, 128))
+
+
+def debug_mixed(fn, handle, block: int, x, device):
+    """Diagnostics shared by I3DEngine.debug_mixed / S3DEngine.debug_mixed: fn is vf_i3d_debug_mixed or
+    vf_s3d_debug_mixed.  x: fp16 pair volume (n, T + 2, S + 2, S + 2, 2 cin) on the device, zero border -> the block's
+    concat pair volume (n, T + 2, S + 2, S + 2, 2 cout), border rows included."""
+    import torch
+    if not 0 <= block < len(MIXED_SIDE):
+        raise ValueError(f"Mixed block {block} outside 0 .. {len(MIXED_SIDE) - 1}")
+    S, cin, cout = MIXED_SIDE[block], MIXED_WIDTHS[block][0], sum(MIXED_WIDTHS[block][1:])
+    # the entry copies n (T + 2) (S + 2)^2 rows of 2 cin halves from x: a wrong shape must not reach it
+    if x.dtype != torch.float16 or x.dim() != 5 or tuple(x.shape[2:]) != (S + 2, S + 2, 2 * cin) or x.shape[1] < 3:
+        raise ValueError(f"block {block} takes an fp16 pair volume (n, T + 2, {S + 2}, {S + 2}, {2 * cin}), T >= 1; "
+                         f"got {x.dtype} {tuple(x.shape)}")
+    if x.device != torch.device(device):
+        raise ValueError(f"the volume is on {x.device}, the engine on {device}")
+    x = x.contiguous()
+    out = torch.empty(tuple(x.shape[:4]) + (2 * cout,), dtype=torch.float16, device=device)
+    with torch.cuda.device(device):
+        check(fn(handle, block, x.data_ptr(), x.shape[0], x.shape[1] - 2, out.data_ptr(),
+                 torch.cuda.current_stream().cuda_stream))
+    return out
+
+
+def debug_maxpool3d(x, vol_in, vol_out, channels: int, k, s, p):
+    """Diagnostics: vf_debug_maxpool3d.  x: fp16 pair rows [hi channels | lo channels] of the volume vol_in on the
+    device; vol_in / vol_out: 10 ints (n, Tp, Hp, Wp, t0, t1, h0, h1, w0, w1); k, s, p: (t, h, w) window, stride and
+    leading padding.  Returns (the pair volume (n, Tp, Hp, Wp, 2 channels) of vol_out, the VF_POOL_* kernel that ran)."""
+    import torch
+    assert x.dtype == torch.float16 and x.is_cuda
+    assert x.numel() == vol_in[0] * vol_in[1] * vol_in[2] * vol_in[3] * 2 * channels, (x.shape, vol_in, channels)
+    x = x.contiguous()
+    out = torch.empty(tuple(vol_out[:4]) + (2 * channels,), dtype=torch.float16, device=x.device)
+    path = C.c_int(-1)
+    with torch.cuda.device(x.device):
+        check(lib().vf_debug_maxpool3d(x.data_ptr(), (C.c_int * 10)(*vol_in), out.data_ptr(), (C.c_int * 10)(*vol_out),
+                                       channels, (C.c_int * 3)(*k), (C.c_int * 3)(*s), (C.c_int * 3)(*p), C.byref(path),
+                                       torch.cuda.current_stream().cuda_stream))
+    return out, path.value
+
+
+def debug_i3d_head(x, vol, channels: int):
+    """Diagnostics: vf_debug_i3d_head, AvgPool3d((2,7,7), 1) and the mean over time of the pair volume x (rows of
+    2 channels; vol: 10 ints as for debug_maxpool3d) -> (n, channels) fp32."""
+    import torch
+    assert x.dtype == torch.float16 and x.is_cuda
+    assert x.numel() == vol[0] * vol[1] * vol[2] * vol[3] * 2 * channels, (x.shape, vol, channels)
+    x = x.contiguous()
+    out = torch.empty((vol[0], channels), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(lib().vf_debug_i3d_head(x.data_ptr(), (C.c_int * 10)(*vol), channels, out.data_ptr(),
+                                      torch.cuda.current_stream().cuda_stream))
+    return out
 
 
 def read_split_conv(fn, handle, index: int, device):

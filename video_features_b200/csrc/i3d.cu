@@ -500,7 +500,7 @@ int vf_i3d_forward_flow(vf_i3d_t* h, const float* flow, int n, int T, int H, int
 int vf_i3d_read_stage(vf_i3d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream) {
     if (!h || stage < 0 || stage > 4 || !dims5) return fail(VF_ERR_INVALID, "i3d_read_stage: bad argument");
     const vf_i3d::StageRef& r = h->stages[stage];
-    if (!r.p) return fail(VF_ERR_UNSUPPORTED, "i3d_read_stage: stage %d is not retained", stage);
+    if (!r.p) return fail(VF_ERR_INVALID, "i3d_read_stage: no forward has run (since the last vf_i3d_debug_mixed)");
     dims5[0] = r.v.n; dims5[1] = r.C; dims5[2] = r.v.T(); dims5[3] = r.v.H(); dims5[4] = r.v.W();
     const int64_t need = int64_t(r.v.n) * r.C * r.v.T() * r.v.H() * r.v.W();
     if (!out) return VF_OK;
@@ -508,6 +508,26 @@ int vf_i3d_read_stage(vf_i3d_t* h, int stage, float* out, int64_t capacity, int*
     cudaStream_t user = static_cast<cudaStream_t>(stream);
     VF_TRY(i3d_enter(h, user));
     VF_TRY(launch_unpack_ndhwc(r.p, r.v, r.C, 0, r.C, 2 * r.C, r.C, out, h->cs));      // retained stages are pair tensors
+    return i3d_leave(h, user);
+}
+
+int vf_i3d_debug_mixed(vf_i3d_t* h, int block, const void* x_pairs, int n, int T, void* out_pairs, void* stream) {
+    if (!h || !x_pairs || !out_pairs) return fail(VF_ERR_INVALID, "i3d_debug_mixed: null argument");
+    if (block < 0 || block > 8 || n < 1 || T < 1)
+        return fail(VF_ERR_INVALID, "i3d_debug_mixed: block %d, %d clips of %d frames", block, n, T);
+    const int S = block < 2 ? 28 : block < 7 ? 14 : 7;
+    const Vol v = bordered(n, T, S, S);
+    // bufA / bufB (2048 columns), t1 (192), t2 (64) and tp (1664) hold cap_rows2 rows of any block's widest operand
+    if (size_t(v.rows()) > h->cap_rows2)
+        return fail(VF_ERR_INVALID, "i3d_debug_mixed: %d clips of %d frames exceed the workspace", n, T);
+    const int* c = kMixed[block];
+    const int cin = c[0], ctot = c[1] + c[3] + c[5] + c[6];
+    cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
+    for (vf_i3d::StageRef& r : h->stages) r.p = nullptr;      // bufA / bufB no longer hold the last forward's stages
+    VF_TRY(i3d_enter(h, user));
+    VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, size_t(v.rows()) * 2 * cin * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    VF_TRY(mixed_block(h, block, h->bufA, v, h->bufB, s));
+    VF_CUDA(cudaMemcpyAsync(out_pairs, h->bufB, size_t(v.rows()) * 2 * ctot * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     return i3d_leave(h, user);
 }
 

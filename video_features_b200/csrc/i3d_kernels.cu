@@ -397,27 +397,44 @@ int launch_i3d_phase_pack_flow(const float* flow, int n, int T, int H, int W, in
     VF_CUDA(cudaGetLastError());
     return VF_OK;
 }
-int launch_maxpool3d_raw(const __half* in, const void* vi, __half* out, const void* vo, int C, int kt, int kh, int kw,
-                         int st, int sh, int sw, int pt, int ph, int pw, cudaStream_t s) {
-    if (C % 8) return fail(VF_ERR_INVALID, "maxpool3d: C=%d must be a multiple of 8", C);
+// Which kernel launch_maxpool3d_raw runs (VF_POOL_*):
+//   same3: a 3x3x3 / 1 pad 1 pool onto the input's own geometry with a border of at least 1 on every side;
+//   fast:  padding 0 before, the last window of every axis ends inside the input's zero border, and the window / stride
+//          is one the fast kernel is instantiated for;
+//   general: everything else.
+int maxpool3d_path_raw(const void* vi, const void* vo, int kt, int kh, int kw, int st, int sh, int sw, int pt, int ph,
+                       int pw) {
     const DVol a = to_dev(vi), b = to_dev(vo);
     const bool same_geom = a.n == b.n && a.Tp == b.Tp && a.Hp == b.Hp && a.Wp == b.Wp && a.t0 == b.t0 && a.t1 == b.t1 &&
                            a.h0 == b.h0 && a.h1 == b.h1 && a.w0 == b.w0 && a.w1 == b.w1;
     if (same_geom && kt == 3 && kh == 3 && kw == 3 && st == 1 && sh == 1 && sw == 1 && pt == 1 && ph == 1 && pw == 1 &&
-        a.t0 >= 1 && a.h0 >= 1 && a.w0 >= 1 && a.t1 < a.Tp && a.h1 < a.Hp && a.w1 < a.Wp) {
+        a.t0 >= 1 && a.h0 >= 1 && a.w0 >= 1 && a.t1 < a.Tp && a.h1 < a.Hp && a.w1 < a.Wp)
+        return VF_POOL_SAME3;
+    const int To = b.t1 - b.t0, Ho = b.h1 - b.h0, Wo = b.w1 - b.w0;
+    const bool fits = pt == 0 && ph == 0 && pw == 0 && To > 0 && Ho > 0 && Wo > 0 &&
+                      a.t0 + (To - 1) * st + kt <= a.Tp && a.h0 + (Ho - 1) * sh + kh <= a.Hp &&
+                      a.w0 + (Wo - 1) * sw + kw <= a.Wp;
+    const bool window = (kt == 1 && kh == 3 && kw == 3 && st == 1 && sh == 2 && sw == 2) ||
+                        (kt == 3 && kh == 3 && kw == 3 && st == 2 && sh == 2 && sw == 2) ||
+                        (kt == 2 && kh == 2 && kw == 2 && st == 2 && sh == 2 && sw == 2);
+    return fits && window ? VF_POOL_FAST : VF_POOL_GENERAL;
+}
+
+int launch_maxpool3d_raw(const __half* in, const void* vi, __half* out, const void* vo, int C, int kt, int kh, int kw,
+                         int st, int sh, int sw, int pt, int ph, int pw, cudaStream_t s) {
+    if (C % 8) return fail(VF_ERR_INVALID, "maxpool3d: C=%d must be a multiple of 8", C);
+    const DVol a = to_dev(vi), b = to_dev(vo);
+    const int path = maxpool3d_path_raw(vi, vo, kt, kh, kw, st, sh, sw, pt, ph, pw);
+    if (path == VF_POOL_SAME3) {
         const int64_t threads = int64_t(a.n) * a.Tp * a.Wp * (C / 8);
         maxpool3d_same3_kernel<<<nblocks(threads, 128), 128, 0, s>>>(in, a, out, C);
         VF_CUDA(cudaGetLastError());
         return VF_OK;
     }
     const int64_t total = int64_t(b.n) * b.Tp * b.Hp * b.Wp * (C / 8);
-    {   // fast path: padding 0 before, and the last window of every axis ends inside the input's zero border
-        const int To = b.t1 - b.t0, Ho = b.h1 - b.h0, Wo = b.w1 - b.w0;
-        const bool fits = pt == 0 && ph == 0 && pw == 0 && To > 0 && Ho > 0 && Wo > 0 &&
-                          a.t0 + (To - 1) * st + kt <= a.Tp && a.h0 + (Ho - 1) * sh + kh <= a.Hp &&
-                          a.w0 + (Wo - 1) * sw + kw <= a.Wp;
+    if (path == VF_POOL_FAST) {
 #define VF_POOL_CASE(KT, KH, KW, ST, SH, SW)                                                                      \
-        if (fits && kt == KT && kh == KH && kw == KW && st == ST && sh == SH && sw == SW) {                       \
+        if (kt == KT && kh == KH && kw == KW && st == ST && sh == SH && sw == SW) {                               \
             maxpool3d_fast_kernel<KT, KH, KW, ST, SH, SW><<<nblocks(total, 256), 256, 0, s>>>(in, a, out, b, C);   \
             VF_CUDA(cudaGetLastError());                                                                          \
             return VF_OK;                                                                                         \
@@ -426,6 +443,7 @@ int launch_maxpool3d_raw(const __half* in, const void* vi, __half* out, const vo
         VF_POOL_CASE(3, 3, 3, 2, 2, 2)
         VF_POOL_CASE(2, 2, 2, 2, 2, 2)
 #undef VF_POOL_CASE
+        return fail(VF_ERR_INVALID, "maxpool3d: no fast kernel for window %dx%dx%d / %dx%dx%d", kt, kh, kw, st, sh, sw);
     }
     maxpool3d_kernel<<<nblocks(total, 256), 256, 0, s>>>(in, a, out, b, C, kt, kh, kw, st, sh, sw, pt, ph, pw);
     VF_CUDA(cudaGetLastError());
@@ -448,3 +466,37 @@ int launch_unpack_ndhwc_raw(const __half* in, const void* vi, int C, int c_off, 
 }
 
 }  // namespace vf
+
+namespace {
+
+// a volume the pool / head kernels can index: positive extents, the valid region inside the padded one
+bool vol_ok(const int* v) {
+    return v[0] > 0 && v[1] > 0 && v[2] > 0 && v[3] > 0 && 0 <= v[4] && v[4] < v[5] && v[5] <= v[1] && 0 <= v[6] &&
+           v[6] < v[7] && v[7] <= v[2] && 0 <= v[8] && v[8] < v[9] && v[9] <= v[3];
+}
+
+}  // namespace
+
+extern "C" {
+
+int vf_debug_maxpool3d(const void* in, const int* vol_in, void* out, const int* vol_out, int C, const int* k,
+                       const int* s, const int* p, int* path, void* stream) {
+    if (!in || !vol_in || !out || !vol_out || !k || !s || !p || !path)
+        return vf::fail(VF_ERR_INVALID, "debug_maxpool3d: null argument");
+    if (!vol_ok(vol_in) || !vol_ok(vol_out) || vol_in[0] != vol_out[0] || C <= 0)
+        return vf::fail(VF_ERR_INVALID, "debug_maxpool3d: bad volume or C=%d", C);
+    for (int j = 0; j < 3; ++j)
+        if (k[j] < 1 || s[j] < 1 || p[j] < 0) return vf::fail(VF_ERR_INVALID, "debug_maxpool3d: bad window");
+    *path = vf::maxpool3d_path_raw(vol_in, vol_out, k[0], k[1], k[2], s[0], s[1], s[2], p[0], p[1], p[2]);
+    return vf::launch_maxpool3d_raw(static_cast<const __half*>(in), vol_in, static_cast<__half*>(out), vol_out, C, k[0],
+                                    k[1], k[2], s[0], s[1], s[2], p[0], p[1], p[2], static_cast<cudaStream_t>(stream));
+}
+
+int vf_debug_i3d_head(const void* in, const int* vol, int C, float* out, void* stream) {
+    if (!in || !vol || !out) return vf::fail(VF_ERR_INVALID, "debug_i3d_head: null argument");
+    if (!vol_ok(vol) || C <= 0 || vol[5] - vol[4] < 2 || vol[7] - vol[6] != 7 || vol[9] - vol[8] != 7)
+        return vf::fail(VF_ERR_INVALID, "debug_i3d_head: the valid region must be T3 >= 2 x 7 x 7 (C=%d)", C);
+    return vf::launch_i3d_head_raw(static_cast<const __half*>(in), vol, C, out, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -511,7 +511,8 @@ int vf_s3d_forward_u8(vf_s3d_t* h, const uint8_t* frames, int n_frames, int H, i
 }
 
 int vf_s3d_read_stage(vf_s3d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream) {
-    if (!h || !dims5 || h->last_m <= 0) return fail(VF_ERR_INVALID, "s3d_read_stage: no forward has run");
+    if (!h || !dims5 || h->last_m <= 0)
+        return fail(VF_ERR_INVALID, "s3d_read_stage: no forward has run (since the last vf_s3d_debug_mixed)");
     if (stage < 0 || stage > 4) return fail(VF_ERR_INVALID, "s3d_read_stage: unknown stage %d", stage);
     const S3Geom g = geom(h->last_m, h->last_T);
     const Vol3 vols[5] = {g.vt, g.v1, g.v2, g.v3, g.v4};
@@ -526,6 +527,34 @@ int vf_s3d_read_stage(vf_s3d_t* h, int stage, float* out, int64_t capacity, int*
     VF_CUDA(cudaSetDevice(h->device));
     VF_CUDA(cudaStreamSynchronize(h->cs));      // diagnostics only: the engine stream has finished the last call
     return launch_unpack_ndhwc_raw(srcs[stage], &v, C, 0, C, 2 * C, C, out, static_cast<cudaStream_t>(stream));
+}
+
+int vf_s3d_debug_mixed(vf_s3d_t* h, int block, const void* x_pairs, int n, int T, void* out_pairs, void* stream) {
+    if (!h || !x_pairs || !out_pairs) return fail(VF_ERR_INVALID, "s3d_debug_mixed: null argument");
+    if (block < 0 || block > 8 || n < 1 || T < 1)
+        return fail(VF_ERR_INVALID, "s3d_debug_mixed: block %d, %d clips of %d frames", block, n, T);
+    const int S = block < 2 ? 28 : block < 7 ? 14 : 7;
+    const Vol3 v{n, T + 2, S + 2, S + 2, 1, T + 1, 1, S + 1, 1, S + 1};
+    const S3Mixed& B = h->mixed[block];
+    const size_t r = size_t(v.rows());
+    const int* c = B.c;
+    // the buffers run_trunk gives a Mixed block: input bufA, output bufB, ta / tb the branch intermediates, tp the pool
+    if (r * 2 * B.cin > h->cap.mixA || r * 2 * B.ctot() > h->cap.mixA ||
+        r * 2 * std::max({c[1], c[2], c[3], c[4]}) > h->cap.mixT || r * 2 * B.cin > h->cap.mixP)
+        return fail(VF_ERR_INVALID, "s3d_debug_mixed: %d clips of %d frames exceed the workspace", n, T);
+    cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
+    VF_CUDA(cudaSetDevice(h->device));
+    // the retained stages (stem_out, c3, m3c, m4f, m5c) are not written here, but the block replaces bufA / bufB and
+    // the branch intermediates, so read_stage is refused until a forward has run again, as for I3D
+    h->last_m = 0;
+    VF_CUDA(cudaEventRecord(h->ev_in, user));
+    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, r * 2 * B.cin * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    VF_TRY(run_mixed(h, B, h->bufA, v, h->bufB, s));
+    VF_CUDA(cudaMemcpyAsync(out_pairs, h->bufB, r * 2 * B.ctot() * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    VF_CUDA(cudaEventRecord(h->ev_out, s));
+    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
+    return VF_OK;
 }
 
 int64_t vf_s3d_launch_count(const vf_s3d_t* h) { return h ? h->ch.launches : 0; }

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import ops  # noqa: F401  (registers torch.ops.vfeat.*)
-from ._lib import I3D_UNITS, I3DWeights, check, lib, read_split_conv
+from ._lib import I3D_UNITS, I3DWeights, check, debug_mixed, lib, read_split_conv
 from .class_head import I3D_KEYS, ClassHead
 
 _MIXED = ["mixed_3b", "mixed_3c", "mixed_4b", "mixed_4c", "mixed_4d", "mixed_4e", "mixed_4f", "mixed_5b", "mixed_5c"]
@@ -172,6 +172,12 @@ class I3DEngine:
         _lib.read_split_conv."""
         with torch.cuda.device(self.device):
             return read_split_conv(lib().vf_i3d_conv, self._h, index, self.device)
+
+    def debug_mixed(self, block: int, x: torch.Tensor) -> torch.Tensor:
+        """Diagnostics: Mixed block ``block`` (0 .. 8: mixed_3b .. mixed_5c) on the fp16 pair volume x
+        (n, T + 2, S + 2, S + 2, 2 cin), S = 28 / 14 / 7, zero border -> its concat pair volume (n, T + 2, S + 2, S + 2,
+        2 ctot) (include/vfeat.h vf_i3d_debug_mixed).  read_stage then fails until the next forward."""
+        return debug_mixed(lib().vf_i3d_debug_mixed, self._h, block, x, self.device)
 
     @property
     def launch_count(self) -> int:

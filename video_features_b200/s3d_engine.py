@@ -8,7 +8,7 @@ from typing import Dict, Sequence
 import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib, read_conv
+from ._lib import NamedTensor, check, debug_mixed, lib, read_conv
 
 OUT_DIM = 1024
 MIN_T = 13
@@ -86,6 +86,12 @@ class S3DEngine:
         """Diagnostics: conv ``index`` as uploaded, in execution order (include/vfeat.h vf_s3d_conv); see _lib.read_conv."""
         with torch.cuda.device(self.device):
             return read_conv(lib().vf_s3d_conv, self._h, index, self.device)
+
+    def debug_mixed(self, block: int, x: torch.Tensor) -> torch.Tensor:
+        """Diagnostics: Mixed block ``block`` (0 .. 8: features.5, 6, 8 .. 12, 14, 15) on the fp16 pair volume x
+        (n, T + 2, S + 2, S + 2, 2 cin), S = 28 / 14 / 7, zero border -> its concat pair volume (n, T + 2, S + 2, S + 2,
+        2 ctot) (include/vfeat.h vf_s3d_debug_mixed).  read_stage then fails until the next forward."""
+        return debug_mixed(lib().vf_s3d_debug_mixed, self._h, block, x, self.device)
 
     @property
     def launch_count(self) -> int:
