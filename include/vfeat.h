@@ -320,8 +320,8 @@ int64_t vf_resnet_launch_count(const vf_resnet_t* h);
  * DEVICE buffers filled when not NULL.  An index past the last conv is VF_ERR_INVALID. */
 int vf_resnet_conv(const vf_resnet_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 
-/* ---- R(2+1)D-18 clip features: replaces torchvision `r2plus1d_18(pretrained=True)` with `fc = Identity()` in eval mode,
- * and its clip transform ToFloatTensorInZeroOne -> Resize((128, 171)) -> Normalize -> CenterCrop(112)
+/* ---- R(2+1)D clip features: replaces torchvision `r2plus1d_18(pretrained=True)` with `fc = Identity()` in eval mode
+ * (and the IG65M R(2+1)D-34 models, vf_r21d_create2), and its clip transform ToFloatTensorInZeroOne -> Resize((128, 171)) -> Normalize -> CenterCrop(112)
  * (models/r21d/extract_r21d.py).  Weights: the torchvision state_dict by key (optionally with the "module." prefix),
  * HOST fp32; fc.* is ignored.  A missing / mis-sized tensor is VF_ERR_INVALID. */
 typedef struct vf_r21d vf_r21d_t;
@@ -329,6 +329,12 @@ typedef struct vf_r21d vf_r21d_t;
 /* Workspace holds max_clips clips of max_T frames (0 = 4 and 16); a call of T-frame clips runs in chunks of
  * max_clips * (max_T + 2) / (T + 2) clips (at most 256), so any T up to that holds with bounded device memory. */
 int vf_r21d_create(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips, int max_T);
+/* The same with BatchNorm eps bn_eps (vf_r21d_create: 1e-5, torchvision's; the IG65M R(2+1)D-34 models: 1e-3).  The
+ * network's depth comes from the state dict: blocks per stage (the layerL.B.conv1.0.0.weight keys), each
+ * Conv2Plus1D's mid width (conv{1,2}.0.0.weight, which may differ between conv1 and conv2 of a block) and the
+ * downsamples (required where a block changes stride or width, refused elsewhere). */
+int vf_r21d_create2(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips, int max_T,
+                    double bn_eps);
 int vf_r21d_destroy(vf_r21d_t* h);
 /* clips: n x 3 x T x 112 x 112 fp32 on the device, already transformed (the tensor the reference passes to the model)
  * -> out: n x 512 fp32. */
@@ -340,7 +346,7 @@ int vf_r21d_forward_f32(vf_r21d_t* h, const float* clips, int n, int T, float* o
 int vf_r21d_forward_u8(vf_r21d_t* h, const uint8_t* frames, int n_frames, int H, int W, const int* starts, int n, int T,
                        float* out, void* stream);
 /* Diagnostics: an activation of the last chunk of the last call as fp32 NCTHW: stage 0 stem (after the temporal
- * conv), 1..4 layer1..layer4.  dims5 receives (n, C, T, H, W); out == NULL only queries the shape. */
+ * conv), 1..4 the output of the last block of layer1..layer4.  dims5 receives (n, C, T, H, W); out == NULL only queries the shape. */
 int vf_r21d_read_stage(vf_r21d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream);
 int64_t vf_r21d_launch_count(const vf_r21d_t* h);
 /* Diagnostics: conv `index` as uploaded, in execution order (the stem's spatial and temporal convs, then per block

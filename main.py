@@ -4,7 +4,8 @@ refused -- the reference's CPU path is what ``bench.py --impl reference`` times,
 Beyond the reference: ``--gather_features`` (one all-gather of every GPU's features into one .npz) and the ``s3d``
 feature type (torchvision's S3D, the Kinetics-400 clip feature upstream video_features added later), the first choice
 outside the reference's list, and the ``CLIP-ViT-L/14`` / ``CLIP-ViT-L/14@336px`` feature types (openai's largest
-released ViT, 768-d features), which the reference does not offer either.
+released ViT, 768-d features), which the reference does not offer either; ``--model_name`` selects upstream's IG65M
+R(2+1)D-34 models for ``r21d_rgb``.
 """
 import argparse
 import functools
@@ -99,6 +100,12 @@ _FLAGS = [
     ('--output_direct', dict(action='store_true', help='save as <output_path>/<video stem>.npy')),
     ('--extraction_fps', dict(type=float, help='resample to this frame rate first (I3D)')),
     ('--extract_method', dict(type=str, help='frame sampler: uni_N or fix_N')),
+    # upstream video_features' model choice for r21d_rgb; None means r2plus1d_18_16_kinetics, so that sanity_check can
+    # refuse the flag for other feature types
+    ('--model_name', dict(choices=['r2plus1d_18_16_kinetics', 'r2plus1d_34_32_ig65m_ft_kinetics',
+                                   'r2plus1d_34_8_ig65m_ft_kinetics'], default=None,
+                          help='r21d_rgb network (default r2plus1d_18_16_kinetics; the R(2+1)D-34 IG65M models default '
+                               'to 32 / 32 and 8 / 8 frame stacks)')),
     ('--stack_size', dict(type=int, help='frames per I3D / R(2+1)D / S3D stack')),
     ('--step_size', dict(type=int, help='frames between I3D / R(2+1)D / S3D stacks')),
     ('--streams', dict(nargs='+', choices=['flow', 'rgb'], help='I3D streams (default: both)')),

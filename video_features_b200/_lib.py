@@ -133,6 +133,8 @@ SIGNATURES = {
     "vf_resnet_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                                  C.c_void_p, C.c_void_p]),
     "vf_r21d_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vf_r21d_create2": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int,
+                                  C.c_double]),
     "vf_r21d_destroy": (C.c_int, [C.c_void_p]),
     "vf_r21d_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_r21d_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int,

@@ -1,7 +1,9 @@
-// torchvision R(2+1)D-18 trunk (`r2plus1d_18`, fc = Identity) on the wgmma conv-GEMM.
+// torchvision R(2+1)D trunk (`VideoResNet` with `Conv2Plus1D` blocks, fc = Identity) on the wgmma conv-GEMM.
 // Replaces `r2plus1d_18(pretrained=True)` with `model.fc = Identity()` in eval mode (reference:
 // models/r21d/extract_r21d.py) together with its clip transform ToFloatTensorInZeroOne -> Resize((128, 171)) ->
-// Normalize -> CenterCrop(112).
+// Normalize -> CenterCrop(112).  The depth is read from the state dict: blocks per stage, each Conv2Plus1D's mid width
+// and the downsamples, so the IG65M R(2+1)D-34 models (layers 3, 4, 6, 3; conv1 and conv2 of a block with different
+// mid widths; BatchNorm eps 1e-3) run on the same code.
 //
 // Layout: every activation is a split-fp16 pair row [hi C | lo C] of a zero-bordered channels-last 3-D volume
 // [clip][T+2][Hp][Wp] (r21d_kernels.h Vol3), written by the GEMM epilogue's split output; BatchNorm is folded into the
@@ -49,7 +51,7 @@ struct R21Conv {
 };
 
 struct R21Block {
-    int cin = 0, mid = 0, cout = 0, stride = 1;     // mid: padded to a multiple of 8
+    int cin = 0, mid1 = 0, mid2 = 0, cout = 0, stride = 1;     // conv1's / conv2's mid width, padded to a multiple of 8
     bool down = false;
     R21Conv c1s, c1t, c2s, c2t, dn;
 };
@@ -61,8 +63,10 @@ using namespace vf;
 struct vf_r21d {
     int device = 0, max_clips = 0, max_T = 0, slots = 0;
     std::vector<void*> allocs;
+    double bn_eps = 1e-5;
     R21Conv stem_s, stem_t;
     std::vector<R21Block> blocks;
+    int nblocks[4] = {0, 0, 0, 0};   // blocks per stage, in the order of `blocks`
     // workspace, in frame slots (max_clips * (max_T + 2)); stage outputs are kept for vf_r21d_read_stage
     __half *s0 = nullptr, *pf = nullptr, *stem_mid = nullptr, *stem_out = nullptr;
     __half *stage_out[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -114,22 +118,36 @@ static int ralloc(vf_r21d* h, Tp** p, size_t count) {
 // torchvision state_dict lookup by key, with or without the "module." prefix of a DataParallel checkpoint
 struct R21Tensors {
     const vf_named_tensor* t; int n;
-    int get(const std::string& name, int64_t numel, const float** out) const {
+    const vf_named_tensor* find(const std::string& name) const {
         for (int i = 0; i < n; ++i) {
             const char* k = t[i].name;
-            if (!k || !(name == k || (strncmp(k, "module.", 7) == 0 && name == k + 7))) continue;
-            if (!t[i].data || t[i].numel != numel)
-                return fail(VF_ERR_INVALID, "r21d_create: tensor '%s' has %lld elements, expected %lld", name.c_str(),
-                            (long long)t[i].numel, (long long)numel);
-            *out = t[i].data;
-            return VF_OK;
+            if (k && (name == k || (strncmp(k, "module.", 7) == 0 && name == k + 7))) return &t[i];
         }
-        return fail(VF_ERR_INVALID, "r21d_create: missing tensor '%s'", name.c_str());
+        return nullptr;
+    }
+    int get(const std::string& name, int64_t numel, const float** out) const {
+        const vf_named_tensor* e = find(name);
+        if (!e) return fail(VF_ERR_INVALID, "r21d_create: missing tensor '%s'", name.c_str());
+        if (!e->data || e->numel != numel)
+            return fail(VF_ERR_INVALID, "r21d_create: tensor '%s' has %lld elements, expected %lld", name.c_str(),
+                        (long long)e->numel, (long long)numel);
+        *out = e->data;
+        return VF_OK;
+    }
+    // output channels of the (1,3,3) conv `name` over ci input channels: its weight is [co][ci][1][3][3]
+    int spatial_width(const std::string& name, int ci, int* co) const {
+        const vf_named_tensor* e = find(name);
+        if (!e) return fail(VF_ERR_INVALID, "r21d_create: missing tensor '%s'", name.c_str());
+        if (e->numel <= 0 || e->numel % (int64_t(9) * ci) != 0 || e->numel / (int64_t(9) * ci) > 65536)
+            return fail(VF_ERR_INVALID, "r21d_create: tensor '%s' has %lld elements, not a (co, %d, 1, 3, 3) weight",
+                        name.c_str(), (long long)e->numel, ci);
+        *co = int(e->numel / (int64_t(9) * ci));
+        return VF_OK;
     }
 };
 
-// Uploads conv `name` (weight [co][ci][kt][kh][kw], no bias) followed by BatchNorm3d `bn` (eval, eps 1e-5, folded in
-// double) as a hi + lo weight pair of co_pad rows; pad rows get zero weights, scale and bias.  col(kt, kh, kw, c) -> K
+// Uploads conv `name` (weight [co][ci][kt][kh][kw], no bias) followed by BatchNorm3d `bn` (eval, eps h->bn_eps, folded
+// in double) as a hi + lo weight pair of co_pad rows; pad rows get zero weights, scale and bias.  col(kt, kh, kw, c) -> K
 // column of the activation's hi half; its lo half sits lo_off columns further and gets the same weight.
 // cw.ntaps / k_per_tap and the tap shifts must be set.
 static int upload_conv(vf_r21d* h, R21Conv& cw, const R21Tensors& T, const std::string& name, const std::string& bn,
@@ -141,7 +159,7 @@ static int upload_conv(vf_r21d* h, R21Conv& cw, const R21Tensors& T, const std::
     VF_TRY(T.get(bn + ".running_mean", co, &m)); VF_TRY(T.get(bn + ".running_var", co, &v));
     std::vector<float> sc(co_pad, 0.f), sh(co_pad, 0.f);
     for (int i = 0; i < co; ++i) {
-        const double s = double(g[i]) / sqrt(double(v[i]) + 1e-5);
+        const double s = double(g[i]) / sqrt(double(v[i]) + h->bn_eps);
         sc[i] = float(s);
         sh[i] = float(double(b[i]) - double(m[i]) * s);
     }
@@ -271,20 +289,20 @@ static int run_conv(vf_r21d* h, const R21Conv& cw, const __half* X, int pitch, c
 // torchvision video BasicBlock with Conv2Plus1D: x (volume vi, cin channels) -> dst (vo, cout channels)
 static int run_block(vf_r21d* h, const R21Block& B, const __half* x, const Vol3& vi, const Vol3& vo, __half* dst,
                      cudaStream_t s) {
-    const int mid = B.mid, cout = B.cout;
+    const int mid1 = B.mid1, cout = B.cout;
     if (B.stride == 2) {
         const Vol3 vm = mix_vol(vi, vo);           // the spatial conv keeps the frames
         VF_TRY(raft_phase_repack(x, frames2d(vi), 2 * B.cin, h->ph, frames2d(vm), s));
         VF_TRY(run_conv(h, B.c1s, h->ph, 8 * B.cin, vm, h->t1, true, s));
-        VF_TRY(r21d_temporal_phase(h->t1, vm, 2 * mid, h->tph, vo, s));
-        VF_TRY(run_conv(h, B.c1t, h->tph, 4 * mid, vo, h->t2, true, s));
+        VF_TRY(r21d_temporal_phase(h->t1, vm, 2 * mid1, h->tph, vo, s));
+        VF_TRY(run_conv(h, B.c1t, h->tph, 4 * mid1, vo, h->t2, true, s));
         h->launches += 2;
     } else {
         VF_TRY(run_conv(h, B.c1s, x, 2 * B.cin, vi, h->t1, true, s));
-        VF_TRY(run_conv(h, B.c1t, h->t1, 2 * mid, vi, h->t2, true, s));
+        VF_TRY(run_conv(h, B.c1t, h->t1, 2 * mid1, vi, h->t2, true, s));
     }
     VF_TRY(run_conv(h, B.c2s, h->t2, 2 * cout, vo, h->t1, true, s));
-    VF_TRY(run_conv(h, B.c2t, h->t1, 2 * mid, vo, h->t3, false, s));
+    VF_TRY(run_conv(h, B.c2t, h->t1, 2 * B.mid2, vo, h->t3, false, s));
     const __half* res = x;
     if (B.down) {
         VF_TRY(r21d_subsample(x, vi, 2 * B.cin, h->sub, vo, s));
@@ -305,9 +323,10 @@ static int run_trunk(vf_r21d* h, int m, int T, cudaStream_t s) {
     VF_TRY(run_conv(h, h->stem_t, h->stem_mid, 96, v0, h->stem_out, true, s));
     const __half* x = h->stem_out;
     for (int L = 0, bi = 0; L < 4; ++L)
-        for (int b = 0; b < 2; ++b, ++bi) {
+        for (int b = 0; b < h->nblocks[L]; ++b, ++bi) {
             const Vol3 vo = stage_vol(m, T, L), vi = (b == 0 && L > 0) ? stage_vol(m, T, L - 1) : vo;
-            __half* dst = b == 1 ? h->stage_out[L] : (x == h->bufA ? h->bufB : h->bufA);
+            // the stage's last block writes the stage output vf_r21d_read_stage returns
+            __half* dst = b == h->nblocks[L] - 1 ? h->stage_out[L] : (x == h->bufA ? h->bufB : h->bufA);
             VF_TRY(run_block(h, h->blocks[bi], x, vi, vo, dst, s));
             x = dst;
         }
@@ -319,8 +338,14 @@ static int run_trunk(vf_r21d* h, int m, int T, cudaStream_t s) {
 extern "C" {
 
 int vf_r21d_create(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips, int max_T) {
+    return vf_r21d_create2(out, tensors, n_tensors, device, max_clips, max_T, 1e-5);
+}
+
+int vf_r21d_create2(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips, int max_T,
+                    double bn_eps) {
     if (!out || !tensors || n_tensors <= 0) return fail(VF_ERR_INVALID, "r21d_create: null argument");
     *out = nullptr;
+    if (!(bn_eps > 0.0 && bn_eps < 1.0)) return fail(VF_ERR_INVALID, "r21d_create: BatchNorm eps %g outside (0, 1)", bn_eps);
     if (max_clips <= 0) max_clips = 4;
     if (max_T <= 0) max_T = 16;
     VF_CUDA(cudaSetDevice(device));
@@ -330,7 +355,7 @@ int vf_r21d_create(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensor
     if (major != 9 || minor != 0)
         return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
     vf_r21d* h = new vf_r21d();
-    h->device = device; h->max_clips = max_clips; h->max_T = max_T;
+    h->device = device; h->max_clips = max_clips; h->max_T = max_T; h->bn_eps = bn_eps;
     h->slots = max_clips * (max_T + 2);
     const R21Tensors Tn{tensors, n_tensors};
     auto body = [&]() -> int {
@@ -343,31 +368,44 @@ int vf_r21d_create(vf_r21d_t** out, const vf_named_tensor* tensors, int n_tensor
         for (int L = 0; L < 4; ++L) {
             const int cout = kCout[L];
             const Vol3 vo = stage_vol(1, 1, L);
-            for (int b = 0; b < 2; ++b) {
+            // blocks layerL.0, layerL.1, ... as far as the state dict has them (r2plus1d_18: 2 per stage; R(2+1)D-34:
+            // 3, 4, 6, 3)
+            int nb = 0;
+            while (nb < 64 && Tn.find("layer" + std::to_string(L + 1) + "." + std::to_string(nb) + ".conv1.0.0.weight"))
+                ++nb;
+            if (nb == 0) return fail(VF_ERR_INVALID, "r21d_create: missing tensor 'layer%d.0.conv1.0.0.weight'", L + 1);
+            h->nblocks[L] = nb;
+            for (int b = 0; b < nb; ++b) {
                 R21Block B;
                 B.cin = b == 0 ? cin : cout; B.cout = cout;
                 B.stride = (b == 0 && L > 0) ? 2 : 1;
                 B.down = B.stride != 1 || B.cin != cout;
-                // torchvision BasicBlock: midplanes = (inplanes * planes * 27) // (inplanes * 9 + 3 * planes), shared by
-                // both Conv2Plus1D of the block
-                const int mid = (B.cin * cout * 27) / (B.cin * 9 + 3 * cout);
-                B.mid = pad8(mid);
                 const std::string p = "layer" + std::to_string(L + 1) + "." + std::to_string(b);
+                if (!B.down && Tn.find(p + ".downsample.0.weight"))
+                    return fail(VF_ERR_INVALID, "r21d_create: '%s.downsample.0.weight' on a stride-1 block of equal "
+                                "widths (%d -> %d); torchvision's VideoResNet has none there", p.c_str(), B.cin, cout);
+                // each Conv2Plus1D's mid width is its spatial conv's output width: torchvision's BasicBlock gives both
+                // (inplanes * planes * 27) // (inplanes * 9 + 3 * planes), IG65M's R(2+1)D-34 widens conv2's in the
+                // first block of layer2..4 (288, 576, 1152 instead of 230, 460, 921)
+                int mid1 = 0, mid2 = 0;
+                VF_TRY(Tn.spatial_width(p + ".conv1.0.0.weight", B.cin, &mid1));
+                VF_TRY(Tn.spatial_width(p + ".conv2.0.0.weight", cout, &mid2));
+                B.mid1 = pad8(mid1); B.mid2 = pad8(mid2);
                 if (B.stride == 2) {
-                    VF_TRY(prep_spatial2(h, B.c1s, Tn, p + ".conv1.0.0", p + ".conv1.0.1", mid, B.cin));
-                    VF_TRY(prep_temporal2(h, B.c1t, Tn, p + ".conv1.0.3", p + ".conv1.1", cout, mid, B.mid));
+                    VF_TRY(prep_spatial2(h, B.c1s, Tn, p + ".conv1.0.0", p + ".conv1.0.1", mid1, B.cin));
+                    VF_TRY(prep_temporal2(h, B.c1t, Tn, p + ".conv1.0.3", p + ".conv1.1", cout, mid1, B.mid1));
                     e_ph = std::max(e_ph, rows(vo) * 8 * B.cin);
-                    e_tph = std::max(e_tph, rows(vo) * 4 * B.mid);
+                    e_tph = std::max(e_tph, rows(vo) * 4 * B.mid1);
                     e_sub = std::max(e_sub, rows(vo) * 2 * B.cin);
                 } else {
-                    VF_TRY(prep_spatial(h, B.c1s, Tn, p + ".conv1.0.0", p + ".conv1.0.1", mid, B.cin, B.cin));
-                    VF_TRY(prep_temporal(h, B.c1t, Tn, p + ".conv1.0.3", p + ".conv1.1", cout, mid, B.mid));
+                    VF_TRY(prep_spatial(h, B.c1s, Tn, p + ".conv1.0.0", p + ".conv1.0.1", mid1, B.cin, B.cin));
+                    VF_TRY(prep_temporal(h, B.c1t, Tn, p + ".conv1.0.3", p + ".conv1.1", cout, mid1, B.mid1));
                 }
-                // conv2 is Conv2Plus1D(planes, planes, midplanes) with the block's midplanes
-                VF_TRY(prep_spatial(h, B.c2s, Tn, p + ".conv2.0.0", p + ".conv2.0.1", mid, cout, cout));
-                VF_TRY(prep_temporal(h, B.c2t, Tn, p + ".conv2.0.3", p + ".conv2.1", cout, mid, B.mid));
+                VF_TRY(prep_spatial(h, B.c2s, Tn, p + ".conv2.0.0", p + ".conv2.0.1", mid2, cout, cout));
+                VF_TRY(prep_temporal(h, B.c2t, Tn, p + ".conv2.0.3", p + ".conv2.1", cout, mid2, B.mid2));
                 if (B.down) VF_TRY(prep_point(h, B.dn, Tn, p + ".downsample.0", p + ".downsample.1", cout, B.cin));
-                e_mid = std::max(e_mid, rows(vo) * 2 * B.mid);
+                // t1 holds both spatial convs' outputs
+                e_mid = std::max(e_mid, rows(vo) * 2 * std::max(B.mid1, B.mid2));
                 e_act = std::max(e_act, rows(vo) * 2 * cout);
                 h->blocks.push_back(B);
             }

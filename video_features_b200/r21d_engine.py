@@ -1,5 +1,6 @@
-"""R(2+1)D-18 clip-feature handle: stands where the reference keeps torchvision ``r2plus1d_18(pretrained=True)`` with
-``fc = Identity()`` in eval mode (models/r21d/extract_r21d.py)."""
+"""R(2+1)D clip-feature handle: stands where the reference keeps torchvision ``r2plus1d_18(pretrained=True)`` with
+``fc = Identity()`` in eval mode (models/r21d/extract_r21d.py), and runs the IG65M R(2+1)D-34 models on the same
+engine."""
 from __future__ import annotations
 
 import ctypes as C
@@ -14,11 +15,14 @@ OUT_DIM = 512
 
 
 class R21DEngine:
-    """``state_dict``: torchvision's r2plus1d_18 keys (with or without the ``module.`` prefix), any float dtype.
+    """``state_dict``: torchvision's VideoResNet keys (with or without the ``module.`` prefix), any float dtype; the
+    depth, the mid widths and the downsamples are read from it (r2plus1d_18, or R(2+1)D-34 with 3, 4, 6, 3 blocks).
+    ``bn_eps``: every BatchNorm's eps (1e-5 for r2plus1d_18, 1e-3 for the IG65M R(2+1)D-34 models).
     ``max_clips`` x ``max_T``: the workspace; a call of T-frame clips runs in chunks of
     max_clips * (max_T + 2) // (T + 2) clips inside the call."""
 
-    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, max_clips: int = 4, max_T: int = 16):
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device: int = 0, max_clips: int = 4, max_T: int = 16,
+                 bn_eps: float = 1e-5):
         if not torch.cuda.is_available():
             raise RuntimeError("R21DEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
@@ -34,7 +38,7 @@ class R21DEngine:
             arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
             arr[i].numel = a.size
         h = C.c_void_p()
-        check(lib().vf_r21d_create(C.byref(h), arr, len(items), device, max_clips, max_T))
+        check(lib().vf_r21d_create2(C.byref(h), arr, len(items), device, max_clips, max_T, float(bn_eps)))
         self._h = h
         del keep
 

@@ -274,6 +274,8 @@ def sanity_check(args: argparse.Namespace):
         args.device_ids = args.device_ids[:1]
     if args.feature_type == 'i3d' and args.stack_size is not None and args.stack_size < 10:
         raise AssertionError(f'I3D model does not support inputs shorter than 10 timestamps. You have: {args.stack_size}')
+    if getattr(args, 'model_name', None) is not None and args.feature_type != 'r21d_rgb':
+        raise AssertionError(f'--model_name selects the r21d_rgb network; it does not apply to {args.feature_type}')
 
 
 def _paired(videos, flows):
