@@ -377,11 +377,35 @@ int vf_clip_rn_encode_u8(vf_clip_rn_t* h, const uint8_t* frames, int n, int H, i
  * 6 the attention output before c_proj (n, E, 1, 1).  dims4 receives the shape; out == NULL only queries it. */
 int vf_clip_rn_read_stage(vf_clip_rn_t* h, int stage, float* out, int64_t capacity, int* dims4, void* stream);
 int64_t vf_clip_rn_launch_count(const vf_clip_rn_t* h);
+/* Diagnostics: stage 0 .. 4 of vf_clip_rn_read_stage as the engine holds it, the raw zero-bordered pair volume
+ * (n, S+2, S+2, 2C) fp16 with its border rows; capacity: halves of out. */
+int vf_clip_rn_read_pairs(vf_clip_rn_t* h, int stage, void* out, int64_t capacity, void* stream);
 /* Diagnostics: conv `index` as uploaded, in execution order: the stem's conv1, conv2, conv3, then per block conv1,
  * conv2, conv3, the downsample if any, then the attention pool's q_proj, k|v (one projection of 2E outputs) and c_proj
  * (linears: one tap, scale 1, the bias).  Same contract as vf_resnet_conv; a pooled 1x1 conv carries its weight in all
  * four phase slots and 1/4 in its scale. */
 int vf_clip_rn_conv(const vf_clip_rn_t* h, int index, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
+/* Diagnostics: Bottleneck `block` (0 .. sum of the layers - 1, execution order) once, through the trunk's own kernels
+ * and buffers, on n (1 .. max_frames) frames.  x_pairs: zero-bordered channels-last pair volume (n, S_in+2, S_in+2,
+ * 2 cin) on the device -- block 0 takes the UNPOOLED stem output (S_in = n_px/2; layer1.0's AvgPool2d(2) is fused into
+ * its convs), the first block of layer L > 1 layer L-1's output, every other block its own layer's.  out_pairs: the
+ * block output (n, S_out+2, S_out+2, 2 cout), border rows included; branch_out: bn3's output before the residual add,
+ * shortcut_out (NULL to skip; untouched by a block without a downsample): the downsample's output, both pair volumes of
+ * the output's geometry.  Afterwards vf_clip_rn_read_stage is VF_ERR_INVALID until the next encode. */
+int vf_clip_rn_debug_block(vf_clip_rn_t* h, int block, const void* x_pairs, int n, void* out_pairs, void* branch_out,
+                           void* shortcut_out, void* stream);
+/* Diagnostics: AttentionPool2d as the encode runs it (tokens -> K|V -> Q -> attention -> c_proj) on a layer4 pair
+ * volume x_pairs (n, S4+2, S4+2, 2E), n = 1 .. max_frames -> features n x out_dim fp32.  Then read_stage is
+ * VF_ERR_INVALID until the next encode, and vf_clip_rn_debug_attnpool_read returns the intermediates. */
+int vf_clip_rn_debug_attnpool(vf_clip_rn_t* h, const void* x_pairs, int n, float* features, void* stream);
+/* An intermediate of the last vf_clip_rn_debug_attnpool (until the next encode or debug call), copied raw: what 0 the
+ * tokens (n T rows of [hi E | lo E] fp16), 1 K|V (n T rows of [k E | v E] fp32, biases added), 2 Q (n rows of E fp32,
+ * bias added, unscaled), 3 the attention output (n rows of [hi E | lo E] fp16).  capacity: elements of out. */
+int vf_clip_rn_debug_attnpool_read(vf_clip_rn_t* h, int what, void* out, int64_t capacity, void* stream);
+/* Diagnostics, stateless: the towers' attention kernel on caller-supplied fp32 K|V (n T rows of [k E | v E]) and Q (n
+ * rows of E) -> out_pairs (n rows of [hi E | lo E] fp16): per (frame, head of 64) softmax((q / 8) . k) v.  E must be a
+ * multiple of 64, and the T scores must fit the kernel's dynamic shared memory (VF_ERR_INVALID otherwise). */
+int vf_debug_clip_rn_attention(const float* kv, const float* q, int n, int T, int E, void* out_pairs, void* stream);
 
 /* ---- CLIP ViT-L/14 image towers (224 px, 257 tokens; 336 px, 577 tokens): replace `clip.load("ViT-L/14" |
  * "ViT-L/14@336px")` and `model.encode_image(preprocess(frame))` with its transform Resize(n_px, bicubic) ->

@@ -86,6 +86,7 @@ def _bn(sd, p, x, calib=None):
 
 
 def _block(sd, p, x, stride, calib=None):
+    """One Bottleneck -> (output, branch = bn3's output before the add, shortcut = the downsample's output or x)."""
     y = F.relu(_bn(sd, p + ".bn1", F.conv2d(x, sd[p + ".conv1.weight"]), calib))
     y = F.relu(_bn(sd, p + ".bn2", F.conv2d(y, sd[p + ".conv2.weight"], padding=1), calib))
     if stride > 1:
@@ -95,20 +96,47 @@ def _block(sd, p, x, stride, calib=None):
         if stride > 1:
             x = F.avg_pool2d(x, stride)
         x = _bn(sd, p + ".downsample.1", F.conv2d(x, sd[p + ".downsample.0.weight"]), calib)
-    return F.relu(x + y)
+    return F.relu(x + y), y, x
+
+
+def blocks(cfg):
+    """Every Bottleneck in execution order: (key prefix, stride, layer index)."""
+    return [(f"visual.layer{L + 1}.{b}", 2 if (b == 0 and L > 0) else 1, L)
+            for L, nb in enumerate(cfg["layers"]) for b in range(nb)]
+
+
+def _stem(sd, x, calib=None):
+    x = F.relu(_bn(sd, "visual.bn1", F.conv2d(x, sd["visual.conv1.weight"], stride=2, padding=1), calib))
+    x = F.relu(_bn(sd, "visual.bn2", F.conv2d(x, sd["visual.conv2.weight"], padding=1), calib))
+    return F.relu(_bn(sd, "visual.bn3", F.conv2d(x, sd["visual.conv3.weight"], padding=1), calib))
+
+
+def block(sd, cfg, i, x):
+    """Bottleneck i (execution order) on its input as the engine takes it -- block 0 the UNPOOLED stem output, whose
+    AvgPool2d(2) the engine fuses into layer1.0's convs -> (output, branch, shortcut)."""
+    p, stride, _ = blocks(cfg)[i]
+    return _block(sd, p, F.avg_pool2d(x, 2) if i == 0 else x, stride)
+
+
+def block_inputs(sd, x, cfg):
+    """The trunk's input to every block, in execution order, as ``block`` takes it (block 0: the stem output)."""
+    y = _stem(sd, x)
+    ins = []
+    for i in range(len(blocks(cfg))):
+        ins.append(y)
+        y = block(sd, cfg, i, y)[0]
+    return ins
 
 
 def trunk(sd, x, cfg, calib=None):
     """stem .. layer4 -> (layer4, {stage: activation})."""
     st = {}
-    x = F.relu(_bn(sd, "visual.bn1", F.conv2d(x, sd["visual.conv1.weight"], stride=2, padding=1), calib))
-    x = F.relu(_bn(sd, "visual.bn2", F.conv2d(x, sd["visual.conv2.weight"], padding=1), calib))
-    x = F.relu(_bn(sd, "visual.bn3", F.conv2d(x, sd["visual.conv3.weight"], padding=1), calib))
+    x = _stem(sd, x, calib)
     st["stem"] = x
     x = F.avg_pool2d(x, 2)
     for L, nb in enumerate(cfg["layers"]):
         for b in range(nb):
-            x = _block(sd, f"visual.layer{L + 1}.{b}", x, 2 if (b == 0 and L > 0) else 1, calib)
+            x = _block(sd, f"visual.layer{L + 1}.{b}", x, 2 if (b == 0 and L > 0) else 1, calib)[0]
         st[f"layer{L + 1}"] = x
     return x, st
 

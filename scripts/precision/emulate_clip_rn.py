@@ -3,10 +3,12 @@
     python scripts/precision/emulate_clip_rn.py [--towers RN50 RN101 RN50x4 RN50x16] [--frames 2] [--tiny]
 
 For each tower's calibrated stand-in (oracle/clip_resnet.py) and one operand class at a time, the forward in float64
-with that class rounded to fp16 and every other operand rounded to fp32 (the engine's split pairs carry ~fp32), against
-the same forward with nothing rounded.  Classes: the stem input, the inputs of the 1x1 convs, of the 3x3 convs, of the
+with that class rounded to fp16 and every other operand stored as the engine's split pair, modelled exactly: hi =
+fp16(v), lo = fp16(v - hi), subnormal lo halves included (for |v| < 0.125 lo is an fp16 subnormal with a spacing of
+2^-24, so a pair of a small weight keeps about 19 bits, not fp32's 24), against the same forward with nothing rounded.  Classes: the stem input, the inputs of the 1x1 convs, of the 3x3 convs, of the
 downsample convs, the residual stream (block outputs), all conv weights, the attention-pool tokens and their K / V, and
-the attention output (c_proj's input).  Reports the worst row's rel-L2 / max-abs÷max of the features; the project's
+the attention output (c_proj's input); "pairs" rounds no class to fp16, so it is the cost of the pair representation
+alone.  Reports the worst row's rel-L2 / max-abs÷max of the features; the project's
 bar is 1e-3 against the fp32 oracle.  --tiny runs a one-block-per-stage tower of width 16 at 64 px (a smoke run).
 """
 import argparse
@@ -21,7 +23,7 @@ sys.path.insert(0, ROOT)
 
 from oracle import clip_resnet  # noqa: E402
 
-CLASSES = ("none", "stem_in", "1x1_in", "3x3_in", "down_in", "residual", "weights", "tokens_kv", "attn_out")
+CLASSES = ("none", "pairs", "stem_in", "1x1_in", "3x3_in", "down_in", "residual", "weights", "tokens_kv", "attn_out")
 
 
 def forward(sd, x, cfg, cls):
@@ -29,7 +31,10 @@ def forward(sd, x, cfg, cls):
     def r(c, t):
         if cls == "none":
             return t
-        return t.half().double() if c == cls else t.float().double()
+        if c == cls:
+            return t.half().double()
+        hi = t.half()
+        return hi.double() + (t - hi.double()).half().double()
 
     def conv(t, p, c, **kw):
         return F.conv2d(r(c, t), r("weights", sd[p + ".weight"]), **kw)

@@ -46,6 +46,28 @@ def test_attention_pool_equals_multihead_attention(T):
     torch.testing.assert_close(F.linear(pre, sd[a + "c_proj.weight"], sd[a + "c_proj.bias"]), got, rtol=1e-12, atol=1e-12)
 
 
+def test_chained_blocks_reproduce_trunk_and_forward():
+    """block_inputs + block, chained, give the float64 trunk's layer outputs and the features bit for bit: the block
+    tests compare the engine's blocks against exactly the computation the tower tests compare its stages against."""
+    sd = {k: v.double() for k, v in clip_resnet.stand_in_state_dict("RN50").items()}
+    cfg = clip_resnet.config(sd)
+    x = clip_resnet.calibration_images(cfg["n_px"], seed=7, n=1).double()
+    with torch.no_grad():
+        ref, taps = clip_resnet.forward(sd, x, taps=True)
+        ins = clip_resnet.block_inputs(sd, x, cfg)
+        assert len(ins) == sum(cfg["layers"]) and torch.equal(ins[0], taps["stem"])
+        y = ins[0]
+        for i, (p, stride, L) in enumerate(clip_resnet.blocks(cfg)):
+            assert torch.equal(y, ins[i]), p
+            out, branch, short = clip_resnet.block(sd, cfg, i, y)
+            assert torch.equal(out, torch.relu(short + branch)), p
+            if i + 1 == len(ins) or clip_resnet.blocks(cfg)[i + 1][2] != L:
+                assert torch.equal(out, taps[f"layer{L + 1}"]), p
+            y = out
+        feats = clip_resnet.attention_pool(sd, clip_resnet.pool_tokens(sd, y), cfg["heads"])
+    assert torch.equal(feats, ref)
+
+
 def _eff(t):
     hi, lo = lay.split(t)
     return hi.double() + lo.double()

@@ -166,6 +166,13 @@ SIGNATURES = {
     "vf_clip_rn_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_clip_rn_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                                   C.c_void_p, C.c_void_p]),
+    "vf_clip_rn_read_pairs": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
+    "vf_clip_rn_debug_block": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
+    "vf_clip_rn_debug_attnpool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_rn_debug_attnpool_read": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
+    "vf_debug_clip_rn_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                             C.c_void_p]),
     "vf_clip_vitl_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
     "vf_clip_vitl_destroy": (C.c_int, [C.c_void_p]),
     "vf_clip_vitl_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
@@ -301,6 +308,25 @@ def debug_i3d_head(x, vol, channels: int):
     with torch.cuda.device(x.device):
         check(lib().vf_debug_i3d_head(x.data_ptr(), (C.c_int * 10)(*vol), channels, out.data_ptr(),
                                       torch.cuda.current_stream().cuda_stream))
+    return out
+
+
+def debug_clip_rn_attention(kv, q):
+    """Diagnostics: vf_debug_clip_rn_attention, the CLIP ResNet towers' attention kernel on fp32 K|V (n, T, 2E) and Q
+    (n, E) on one device -> (n, 2E) fp16 pairs [hi E | lo E] of softmax((q / 8) . k) v per head of 64."""
+    import torch
+    if kv.dtype != torch.float32 or q.dtype != torch.float32 or kv.dim() != 3 or q.dim() != 2:
+        raise ValueError(f"kv (n, T, 2E) and q (n, E) fp32; got {kv.dtype} {tuple(kv.shape)}, {q.dtype} {tuple(q.shape)}")
+    n, T, E2 = kv.shape
+    if E2 % 2 or tuple(q.shape) != (n, E2 // 2):
+        raise ValueError(f"kv {tuple(kv.shape)} and q {tuple(q.shape)} do not agree on (n, E)")
+    if not kv.is_cuda or q.device != kv.device:
+        raise ValueError(f"kv on {kv.device}, q on {q.device}: both must be on one CUDA device")
+    kv, q = kv.contiguous(), q.contiguous()
+    out = torch.empty((n, E2), dtype=torch.float16, device=kv.device)
+    with torch.cuda.device(kv.device):
+        check(lib().vf_debug_clip_rn_attention(kv.data_ptr(), q.data_ptr(), n, T, E2 // 2, out.data_ptr(),
+                                               torch.cuda.current_stream().cuda_stream))
     return out
 
 

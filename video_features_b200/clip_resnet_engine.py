@@ -130,10 +130,84 @@ class ClipResNetEngine:
             return out[:, :, 0, 0]
         return out
 
+    def read_pairs(self, stage: int) -> torch.Tensor:
+        """Diagnostics: stage 0 .. 4 of read_stage as held, the pair volume (n, S + 2, S + 2, 2C) fp16, border
+        included (the form debug_block takes)."""
+        dims = (C.c_int * 4)()
+        check(lib().vf_clip_rn_read_stage(self._h, stage, None, 0, dims, None))
+        if not 0 <= stage <= 4:
+            raise ValueError(f"stage {stage}: read_pairs takes 0 .. 4")
+        n, c, s, _ = dims
+        out = torch.empty((n, s + 2, s + 2, 2 * c), dtype=torch.float16, device=self.device)
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_rn_read_pairs(self._h, stage, out.data_ptr(), out.numel(), self._stream()))
+        return out
+
     def conv(self, index: int) -> dict:
         """Diagnostics: conv ``index`` as uploaded, in execution order (include/vfeat.h vf_clip_rn_conv)."""
         with torch.cuda.device(self.device):
             return read_conv(lib().vf_clip_rn_conv, self._h, index, self.device)
+
+    def block_geometry(self, block: int):
+        """(side of the input, cin, side of the output, cout) of Bottleneck ``block`` as debug_block takes it."""
+        if not 0 <= block < sum(self.layers):
+            raise ValueError(f"block {block} outside 0 .. {sum(self.layers) - 1}")
+        L, b = 0, block
+        while b >= self.layers[L]:
+            b -= self.layers[L]
+            L += 1
+        s_out, cout = self.n_px // (4 << L), 4 * (self.width << L)
+        if b > 0:
+            return s_out, cout, s_out, cout
+        if L == 0:
+            return self.n_px // 2, self.width, s_out, cout
+        return 2 * s_out, cout // 2, s_out, cout
+
+    def _check_pairs(self, x: torch.Tensor, side: int, c: int, what: str) -> torch.Tensor:
+        # the entries copy n (side + 2)^2 rows of 2c halves from x: a wrong shape must not reach them
+        if x.dtype != torch.float16 or x.dim() != 4 or tuple(x.shape[1:]) != (side + 2, side + 2, 2 * c):
+            raise ValueError(f"{what} takes an fp16 pair volume (n, {side + 2}, {side + 2}, {2 * c}); "
+                             f"got {x.dtype} {tuple(x.shape)}")
+        if x.device != self.device:
+            raise ValueError(f"the volume is on {x.device}, the engine on {self.device}")
+        if not 1 <= x.shape[0] <= self.max_frames:
+            raise ValueError(f"{x.shape[0]} frames; {what} takes 1 .. {self.max_frames}")
+        return x.contiguous()
+
+    def debug_block(self, block: int, x: torch.Tensor):
+        """Diagnostics: Bottleneck ``block`` (execution order) once through the trunk's kernels (include/vfeat.h
+        vf_clip_rn_debug_block).  x: zero-bordered pair volume (n, S_in + 2, S_in + 2, 2 cin) on the device (block 0:
+        the unpooled stem output).  Returns (output, branch, shortcut or None) pair volumes (n, S_out + 2, S_out + 2,
+        2 cout), border rows included.  read_stage then fails until the next encode."""
+        s_in, cin, s_out, cout = self.block_geometry(block)
+        x = self._check_pairs(x, s_in, cin, f"block {block}")
+        shape = (x.shape[0], s_out + 2, s_out + 2, 2 * cout)
+        out, branch, short = (torch.empty(shape, dtype=torch.float16, device=self.device) for _ in range(3))
+        has_down = block in {sum(self.layers[:L]) for L in range(4)}
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_rn_debug_block(self._h, block, x.data_ptr(), x.shape[0], out.data_ptr(),
+                                               branch.data_ptr(), short.data_ptr() if has_down else None,
+                                               self._stream()))
+        return out, branch, (short if has_down else None)
+
+    def debug_attnpool(self, x: torch.Tensor):
+        """Diagnostics: the attention pool as the encode runs it on a layer4 pair volume x (n, S4 + 2, S4 + 2, 2E)
+        (include/vfeat.h vf_clip_rn_debug_attnpool).  Returns dict features (n, out_dim) fp32, tokens (n, T, 2E) fp16
+        pairs, kv (n, T, 2E) fp32 ([k | v]), q (n, E) fp32 (unscaled), att (n, 2E) fp16 pairs."""
+        s4 = self.n_px // 32
+        x = self._check_pairs(x, s4, self.embed, "the attention pool")
+        n, T, E = x.shape[0], self.tokens, self.embed
+        feats = torch.empty((n, self.out_dim), dtype=torch.float32, device=self.device)
+        out = dict(features=feats, tokens=torch.empty((n, T, 2 * E), dtype=torch.float16, device=self.device),
+                   kv=torch.empty((n, T, 2 * E), dtype=torch.float32, device=self.device),
+                   q=torch.empty((n, E), dtype=torch.float32, device=self.device),
+                   att=torch.empty((n, 2 * E), dtype=torch.float16, device=self.device))
+        with torch.cuda.device(self.device):
+            check(lib().vf_clip_rn_debug_attnpool(self._h, x.data_ptr(), n, feats.data_ptr(), self._stream()))
+            for what, key in enumerate(("tokens", "kv", "q", "att")):
+                t = out[key]
+                check(lib().vf_clip_rn_debug_attnpool_read(self._h, what, t.data_ptr(), t.numel(), self._stream()))
+        return out
 
     @property
     def launch_count(self) -> int:

@@ -65,6 +65,7 @@ struct vf_clip_rn : vf::ConvHost {
     bool use_graph = true;
     std::map<int, std::pair<cudaGraphExec_t, int64_t>> graphs;     // frames -> (trunk graph, launches in it)
     int last_n = 0;
+    int attn_n = 0;           // frames of the last vf_clip_rn_debug_attnpool (its intermediates stay readable)
 };
 
 namespace vf {
@@ -158,10 +159,28 @@ static int run_block(vf_clip_rn* h, const RnBlock& B, const __half* x, const Vol
     return VF_OK;
 }
 
+// AttentionPool2d up to c_proj's input, on m frames of the layer4 pair volume x4: tokens (h->tok), K|V (h->kvo), Q
+// (h->qo: token 0 of every frame, read in place with a pitch of T tokens), attention (h->att).  The trunk graph and
+// vf_clip_rn_debug_attnpool run it; run_cproj follows outside the graph, since it writes the caller's rows.
+static int run_attention(vf_clip_rn* h, const __half* x4, int m, cudaStream_t s) {
+    const int E = h->embed, T = h->tokens;
+    VF_TRY(clip_rn_tokens(x4, stage_vol(h, m, 3), E, h->pos, h->tok, s));
+    VF_TRY(run_linear(h, h->kv, h->tok, 2 * E, m * T, h->kvo, 2 * E, s));
+    VF_TRY(run_linear(h, h->q, h->tok, T * 2 * E, m, h->qo, E, s));
+    VF_TRY(clip_rn_attention(h->kvo, h->qo, m, T, E, h->att, s));
+    h->launches += 2;
+    return VF_OK;
+}
+
+// c_proj of the m attention rows in h->att -> m fp32 rows of out_dim
+static int run_cproj(vf_clip_rn* h, int m, float* out, cudaStream_t s) {
+    return run_linear(h, h->cproj, h->att, 2 * h->embed, m, out, h->out_dim, s);
+}
+
 // stem conv1 .. attention on m frames whose stem phase volume is in h->s0
 static int run_trunk(vf_clip_rn* h, int m, cudaStream_t s) {
     const Vol2 sv = stem_vol(h, m);
-    const int w = h->width, E = h->embed, T = h->tokens;
+    const int w = h->width;
     VF_TRY(run_conv(h, h->stem[0], h->s0, 32, sv, h->t1, true, s));
     VF_TRY(run_conv(h, h->stem[1], h->t1, w, sv, h->t2, true, s));
     VF_TRY(run_conv(h, h->stem[2], h->t2, w, sv, h->stem_out, true, s));
@@ -174,12 +193,7 @@ static int run_trunk(vf_clip_rn* h, int m, cudaStream_t s) {
             VF_TRY(run_block(h, h->blocks[bi], x, vi, vo, dst, s));
             x = dst;
         }
-    VF_TRY(clip_rn_tokens(h->stage_out[3], stage_vol(h, m, 3), E, h->pos, h->tok, s));
-    VF_TRY(run_linear(h, h->kv, h->tok, 2 * E, m * T, h->kvo, 2 * E, s));
-    VF_TRY(run_linear(h, h->q, h->tok, T * 2 * E, m, h->qo, E, s));      // token 0 of every frame, read in place
-    VF_TRY(clip_rn_attention(h->kvo, h->qo, m, T, E, h->att, s));
-    h->launches += 2;
-    return VF_OK;
+    return run_attention(h, h->stage_out[3], m, s);
 }
 
 static int trunk_graph(vf_clip_rn* h, int m, cudaStream_t s) {
@@ -258,9 +272,10 @@ static int clip_rn_encode(vf_clip_rn* h, const void* frames, int is_u8, int n, i
         }
         VF_TRY(clip_rn_input_pack(src, is_u8, m, rh, rw, cy, cx, npx, h->s0, s));
         VF_TRY(trunk_graph(h, m, s));
-        VF_TRY(run_linear(h, h->cproj, h->att, 2 * h->embed, m, out + size_t(off) * h->out_dim, h->out_dim, s));
-        h->launches += 1;
+        VF_TRY(run_cproj(h, m, out + size_t(off) * h->out_dim, s));
+        h->launches += 1;       // the input pack
         h->last_n = m;
+        h->attn_n = 0;
     }
     VF_CUDA(cudaEventRecord(h->ev_out, s));
     VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
@@ -426,7 +441,8 @@ int vf_clip_rn_encode_u8(vf_clip_rn_t* h, const uint8_t* frames, int n, int H, i
 }
 
 int vf_clip_rn_read_stage(vf_clip_rn_t* h, int stage, float* out, int64_t capacity, int* dims4, void* stream) {
-    if (!h || !dims4 || h->last_n <= 0) return fail(VF_ERR_INVALID, "clip_rn_read_stage: no encode has run");
+    if (!h || !dims4 || h->last_n <= 0)
+        return fail(VF_ERR_INVALID, "clip_rn_read_stage: no encode has run (since the last debug call)");
     if (stage < 0 || stage > 6) return fail(VF_ERR_INVALID, "clip_rn_read_stage: unknown stage %d", stage);
     const int n = h->last_n, E = h->embed;
     Vol2 v;
@@ -442,6 +458,100 @@ int vf_clip_rn_read_stage(vf_clip_rn_t* h, int stage, float* out, int64_t capaci
     VF_CUDA(cudaSetDevice(h->device));
     VF_CUDA(cudaStreamSynchronize(h->cs));      // diagnostics only: the engine stream has finished the last call
     return raft_unpack2d(src, v, ld, 0, C, C, out, static_cast<cudaStream_t>(stream));
+}
+
+int vf_clip_rn_debug_block(vf_clip_rn_t* h, int block, const void* x_pairs, int n, void* out_pairs, void* branch_out,
+                           void* shortcut_out, void* stream) {
+    if (!h || !x_pairs || !out_pairs || !branch_out) return fail(VF_ERR_INVALID, "clip_rn_debug_block: null argument");
+    if (block < 0 || block >= int(h->blocks.size()) || n <= 0 || n > h->max_frames)
+        return fail(VF_ERR_INVALID, "clip_rn_debug_block: block %d of %d, %d frames (max_frames %d)", block,
+                    int(h->blocks.size()), n, h->max_frames);
+    int L = 0, b = block;
+    while (b >= h->layers[L]) b -= h->layers[L++];
+    const RnBlock& B = h->blocks[size_t(block)];
+    const Vol2 vo = stage_vol(h, n, L), vi = b > 0 ? vo : L == 0 ? stem_vol(h, n) : stage_vol(h, n, L - 1);
+    cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
+    VF_CUDA(cudaSetDevice(h->device));
+    // the trunk's own buffers: bufA holds every block input (the workspace sizes it for the stem volume too), bufB the
+    // output; run_block leaves bn3's output in t1 and the downsample's in ds.  The retained stages are not written,
+    // but read_stage is refused until the next encode, as for I3D and S3D.
+    h->last_n = 0;
+    h->attn_n = 0;
+    const size_t in_h = size_t(vi.rows()) * 2 * B.cin, out_h = size_t(vo.rows()) * 2 * B.cout;
+    VF_CUDA(cudaEventRecord(h->ev_in, user));
+    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, in_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    VF_TRY(run_block(h, B, h->bufA, vi, vo, h->bufB, s));
+    VF_CUDA(cudaMemcpyAsync(out_pairs, h->bufB, out_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    VF_CUDA(cudaMemcpyAsync(branch_out, h->t1, out_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    if (B.down && shortcut_out)
+        VF_CUDA(cudaMemcpyAsync(shortcut_out, h->ds, out_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
+    VF_CUDA(cudaEventRecord(h->ev_out, s));
+    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
+    return VF_OK;
+}
+
+int vf_clip_rn_debug_attnpool(vf_clip_rn_t* h, const void* x_pairs, int n, float* features, void* stream) {
+    if (!h || !x_pairs || !features) return fail(VF_ERR_INVALID, "clip_rn_debug_attnpool: null argument");
+    if (n <= 0 || n > h->max_frames)
+        return fail(VF_ERR_INVALID, "clip_rn_debug_attnpool: %d frames (max_frames %d)", n, h->max_frames);
+    const Vol2 v4 = stage_vol(h, n, 3);
+    cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
+    VF_CUDA(cudaSetDevice(h->device));
+    h->last_n = 0;
+    VF_CUDA(cudaEventRecord(h->ev_in, user));
+    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, size_t(v4.rows()) * 2 * h->embed * sizeof(__half),
+                            cudaMemcpyDeviceToDevice, s));
+    VF_TRY(run_attention(h, h->bufA, n, s));
+    VF_TRY(run_cproj(h, n, features, s));
+    VF_CUDA(cudaEventRecord(h->ev_out, s));
+    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
+    h->attn_n = n;
+    return VF_OK;
+}
+
+int vf_clip_rn_debug_attnpool_read(vf_clip_rn_t* h, int what, void* out, int64_t capacity, void* stream) {
+    if (!h || !out) return fail(VF_ERR_INVALID, "clip_rn_debug_attnpool_read: null argument");
+    if (h->attn_n <= 0) return fail(VF_ERR_INVALID, "clip_rn_debug_attnpool_read: no vf_clip_rn_debug_attnpool has run");
+    const int64_t n = h->attn_n, T = h->tokens, E = h->embed;
+    const void* src;
+    int64_t count, size;
+    switch (what) {
+        case 0: src = h->tok; count = n * T * 2 * E; size = sizeof(__half); break;
+        case 1: src = h->kvo; count = n * T * 2 * E; size = sizeof(float); break;
+        case 2: src = h->qo; count = n * E; size = sizeof(float); break;
+        case 3: src = h->att; count = n * 2 * E; size = sizeof(__half); break;
+        default: return fail(VF_ERR_INVALID, "clip_rn_debug_attnpool_read: unknown intermediate %d", what);
+    }
+    if (capacity < count) return fail(VF_ERR_INVALID, "clip_rn_debug_attnpool_read: capacity too small");
+    VF_CUDA(cudaSetDevice(h->device));
+    VF_CUDA(cudaStreamSynchronize(h->cs));
+    VF_CUDA(cudaMemcpyAsync(out, src, size_t(count * size), cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+    return VF_OK;
+}
+
+int vf_debug_clip_rn_attention(const float* kv, const float* q, int n, int T, int E, void* out_pairs, void* stream) {
+    if (!kv || !q || !out_pairs) return fail(VF_ERR_INVALID, "debug_clip_rn_attention: null argument");
+    if (n <= 0 || n > 65535 || E <= 0 || E % 64 || E / 64 > 65535)
+        return fail(VF_ERR_INVALID, "debug_clip_rn_attention: %d frames, E %d (a multiple of 64)", n, E);
+    return clip_rn_attention(kv, q, n, T, E, static_cast<__half*>(out_pairs), static_cast<cudaStream_t>(stream));
+}
+
+int vf_clip_rn_read_pairs(vf_clip_rn_t* h, int stage, void* out, int64_t capacity, void* stream) {
+    if (!h || !out || h->last_n <= 0)
+        return fail(VF_ERR_INVALID, "clip_rn_read_pairs: no encode has run (since the last debug call)");
+    if (stage < 0 || stage > 4) return fail(VF_ERR_INVALID, "clip_rn_read_pairs: unknown stage %d", stage);
+    const int n = h->last_n;
+    const Vol2 v = stage == 0 ? stem_vol(h, n) : stage_vol(h, n, stage - 1);
+    const int C = stage == 0 ? h->width : 4 * (h->width << (stage - 1));
+    const int64_t count = int64_t(v.rows()) * 2 * C;
+    if (capacity < count) return fail(VF_ERR_INVALID, "clip_rn_read_pairs: capacity too small");
+    VF_CUDA(cudaSetDevice(h->device));
+    VF_CUDA(cudaStreamSynchronize(h->cs));
+    VF_CUDA(cudaMemcpyAsync(out, stage == 0 ? h->stem_out : h->stage_out[stage - 1], size_t(count) * sizeof(__half),
+                            cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+    return VF_OK;
 }
 
 int64_t vf_clip_rn_launch_count(const vf_clip_rn_t* h) { return h ? h->launches : 0; }

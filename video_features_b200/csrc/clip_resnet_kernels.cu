@@ -150,6 +150,17 @@ int clip_rn_tokens(const __half* in, const Vol2& v, int E, const float* pos, __h
     LAUNCH_CHECK();
 }
 int clip_rn_attention(const float* kv, const float* q, int n, int T, int E, __half* out, cudaStream_t s) {
+    // the T scores sit in dynamic shared memory beside the kernel's static arrays, within the 48 KB a launch gets
+    // without opting in
+    static size_t static_bytes = 0;
+    if (!static_bytes) {
+        cudaFuncAttributes fa;
+        VF_CUDA(cudaFuncGetAttributes(&fa, attention_kernel));
+        static_bytes = fa.sharedSizeBytes;
+    }
+    if (T < 1 || static_bytes + size_t(T) * sizeof(float) > 48 * 1024)
+        return fail(VF_ERR_INVALID, "clip_rn_attention: %d tokens; the scores fit %zu", T,
+                    (48 * 1024 - static_bytes) / sizeof(float));
     attention_kernel<<<dim3(E / 64, n), 128, size_t(T) * sizeof(float), s>>>(kv, q, T, E, out);
     LAUNCH_CHECK();
 }
