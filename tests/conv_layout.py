@@ -411,11 +411,11 @@ def _stem_col(kt, kh, kw, c):
 
 
 ENGINE_FILTERS = {
-    # prep_same / prep_spatial: k kernel rows, each a run of k * 2ci_p; k = 1 is also the stride-2 downsample, which
+    # prep_same: k kernel rows, each a run of k * 2ci_p; k = 1 is also the stride-2 downsample, which
     # reads phase (0, 0), the first 2ci columns of a phase row
     "same": lambda k, ci, ci_p: (k, 2 * k * ci_p, [(0, a - k // 2, -(k // 2)) for a in range(k)],
                                  lambda kt, kh, kw, c: kh * 2 * k * ci_p + kw * 2 * ci_p + c, ci_p),
-    # prep_stride2 / prep_spatial2: tap (a, b) reads phase row (q + a - 1, q' + b - 1); kh = 2a + ph - 1
+    # prep_stride2: tap (a, b) reads phase row (q + a - 1, q' + b - 1); kh = 2a + ph - 1
     "stride2": lambda k, ci, ci_p: (4, 8 * ci, [(0, t // 2 - 1, t % 2 - 1) for t in range(4)],
                                     _stride2_col(8 * ci, 2 * ci), ci),
     # prep_stem (both engines): 4 taps of kernel row pairs, each 4 phase positions x 32 columns
@@ -427,7 +427,7 @@ ENGINE_FILTERS = {
     "temporal2": lambda k, ci, ci_p: (2, 4 * ci_p, [(-1, 0, 0), (0, 0, 0)],
                                       lambda kt, kh, kw, c: 2 * ci_p + c if kt == 0 else 4 * ci_p + (kt - 1) * 2 * ci_p + c,
                                       ci_p),
-    # prep_point: 1x1x1 over the subsampled block input
+    # prep_same (k = 1): 1x1x1 over the subsampled block input
     "point": lambda k, ci, ci_p: (1, 2 * ci, [(0, 0, 0)], lambda kt, kh, kw, c: c, ci),
 }
 

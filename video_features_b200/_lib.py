@@ -53,6 +53,26 @@ class NamedTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.POINTER(C.c_float)), ("numel", C.c_int64)]
 
 
+def named_tensors(state_dict):
+    """The floating-point tensors of ``state_dict`` (a mapping, or (name, tensor) pairs) as a ``NamedTensor`` array of
+    fp32 host copies: returns (array, count, keep).  ``keep`` holds the copies and names the array points into; it must
+    stay alive until the create call that reads the array returns."""
+    import numpy as np
+    import torch
+    items = state_dict.items() if hasattr(state_dict, "items") else state_dict
+    items = [(k, v) for k, v in items if torch.is_tensor(v) and v.dtype.is_floating_point]
+    keep = []
+    arr = (NamedTensor * max(len(items), 1))()
+    for i, (k, v) in enumerate(items):
+        a = np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
+        nm = k.encode()
+        keep.append((a, nm))
+        arr[i].name = nm
+        arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
+        arr[i].numel = a.size
+    return arr, len(items), keep
+
+
 _lock = threading.Lock()
 _lib = None
 

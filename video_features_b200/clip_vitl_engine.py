@@ -9,7 +9,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib
+from ._lib import check, lib, named_tensors
 
 LAYERS = 24
 
@@ -23,19 +23,9 @@ class ClipViTLEngine:
         if not torch.cuda.is_available():
             raise RuntimeError("ClipViTLEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
-        keep = []
-        items = [(k, v) for k, v in state_dict.items()
-                 if k.startswith("visual.") and torch.is_tensor(v) and v.dtype.is_floating_point]
-        arr = (NamedTensor * max(len(items), 1))()
-        for i, (k, v) in enumerate(items):
-            a = np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
-            nm = k.encode()
-            keep.append((a, nm))
-            arr[i].name = nm
-            arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
-            arr[i].numel = a.size
+        arr, n, keep = named_tensors({k: v for k, v in state_dict.items() if k.startswith("visual.")})
         h = C.c_void_p()
-        check(lib().vf_clip_vitl_create(C.byref(h), arr, len(items), device, max_frames))
+        check(lib().vf_clip_vitl_create(C.byref(h), arr, n, device, max_frames))
         self._h = h
         del keep
         info = (C.c_int * 8)()

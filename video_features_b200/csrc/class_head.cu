@@ -15,8 +15,8 @@
 
 #include "internal.h"
 
-struct vf_head {
-    int device = 0, C = 0, K = 0;
+struct vf_head : vf::EngineCore {
+    int C = 0, K = 0;
     float* w = nullptr;       // [C][K]
     float* b = nullptr;       // [C]
 };
@@ -147,10 +147,7 @@ extern "C" {
 
 int vf_head_destroy(vf_head_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    cudaFree(h->w);
-    cudaFree(h->b);
+    release(h);
     delete h;
     return VF_OK;
 }
@@ -160,18 +157,14 @@ int vf_head_create(vf_head_t** out, const float* weight, const float* bias, int 
     *out = nullptr;
     if (n_classes < 1 || n_features < 1)
         return fail(VF_ERR_INVALID, "head_create: %d classes x %d features", n_classes, n_features);
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_head* h = new vf_head();
+    h->who = "head_create";
     h->device = device; h->C = n_classes; h->K = n_features;
     const size_t wn = size_t(n_classes) * n_features;
     auto body = [&]() -> int {
-        VF_CUDA(cudaMalloc(&h->w, wn * sizeof(float)));
-        VF_CUDA(cudaMalloc(&h->b, size_t(n_classes) * sizeof(float)));
+        VF_TRY(ralloc(h, &h->w, wn));
+        VF_TRY(ralloc(h, &h->b, size_t(n_classes)));
         VF_CUDA(cudaMemcpy(h->w, weight, wn * sizeof(float), cudaMemcpyHostToDevice));
         VF_CUDA(cudaMemcpy(h->b, bias, size_t(n_classes) * sizeof(float), cudaMemcpyHostToDevice));
         return VF_OK;

@@ -29,12 +29,9 @@ struct ClipLayerDev {
 
 }  // namespace vf
 
-struct vf_clip {
-    int device = 0;
+struct vf_clip : vf::EngineCore {
     int chunk = 0;
     int patch = 32, T = 50, P = 49, PK = 3072;   // patch size, tokens (P + 1), patches per frame, patch-matrix columns
-    int64_t launches = 0;
-    std::vector<void*> allocs;
     // weights
     __half* w_patch = nullptr;   // [768, PK]
     __half* w_proj = nullptr;    // [512, 768]  (proj^T)
@@ -73,13 +70,10 @@ struct vf_clip {
         size_t resized_cap = 0, tmp_cap = 0;
         cudaStream_t cs = nullptr;
         cudaEvent_t ev_out = nullptr;
-        std::map<int, cudaGraphExec_t> graphs;   // frames in chunk -> instantiated tower graph (writes feat)
+        std::map<int, vf::CachedGraph> graphs;   // frames in chunk -> instantiated tower graph (writes feat)
         std::map<int, int> seen;                 // frames in chunk -> times this size has been run without a graph
     } lanes[2];
-    int n_lanes = 2, cur = 0;
-    cudaStream_t cs = nullptr;                // stream of the active lane
-    cudaEvent_t ev_in = nullptr;
-    bool use_graph = true;
+    int n_lanes = 2, cur = 0;                 // the lane streams stand in for EngineCore::cs, which stays null
     bool acc_o = true, acc_m = true;          // residual adds in the GEMM epilogue (fp32 reductions) instead of an fp16 y
     bool fused_attn = true;                   // QKV projection + attention in one kernel (VF_CLIP_ATTN=split: GEMM + kernel)
     float* feat = nullptr;                    // [chunk, 512] tower output of the active lane
@@ -93,18 +87,9 @@ struct vf_clip {
 
 namespace vf {
 
-template <typename Tp>
-static int dev_alloc(vf_clip* h, Tp** p, size_t count) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(Tp));
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "cudaMalloc(%zu bytes): %s", count * sizeof(Tp), cudaGetErrorString(e));
-    h->allocs.push_back(q);
-    *p = static_cast<Tp*>(q);
-    return VF_OK;
-}
 static int upload_f32(vf_clip* h, float** dst, const float* src, size_t count) {
     if (!src) return fail(VF_ERR_INVALID, "clip_create: missing weight tensor");
-    VF_TRY(dev_alloc(h, dst, count));
+    VF_TRY(ralloc(h, dst, count));
     VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
     return VF_OK;
 }
@@ -118,7 +103,7 @@ static int upload_f16(vf_clip* h, __half** dst, const float* src, size_t rows, s
         for (size_t r = 0; r < rows; ++r)
             for (size_t c = 0; c < cols; ++c) tmp[c * rows + r] = __float2half_rn(src[r * cols + c]);
     }
-    VF_TRY(dev_alloc(h, dst, rows * cols));
+    VF_TRY(ralloc(h, dst, rows * cols));
     VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
     return VF_OK;
 }
@@ -262,7 +247,6 @@ static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
     return tower_head(h, c, h->acc_m ? nullptr : h->y, out, s);
 }
 
-constexpr int TOWER_LAUNCHES_SPLIT = 2 + 7 * L + 2, TOWER_LAUNCHES_FUSED = 2 + 6 * L + 2;
 constexpr size_t kMaxTowerGraphs = 32;    // per lane; further sizes run eagerly
 
 // Tower on one chunk: replay (capturing on first use) the CUDA graph for this chunk size, then copy the features out.
@@ -277,23 +261,13 @@ static int clip_tower_chunk(vf_clip* h, int c, float* out, cudaStream_t s) {
         auto& seen = h->lanes[h->cur].seen;
         if (seen.size() > 4096) seen.clear();
         if (++seen[c] < 2 || graphs.size() >= kMaxTowerGraphs) return clip_tower_eager(h, c, out, s);
-        const int64_t before = h->launches;
-        cudaGraph_t graph = nullptr;
-        VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-        const int st = clip_tower_eager(h, c, h->feat, s);
-        const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-        h->launches = before;
-        if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-        if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-        cudaGraphExec_t exec = nullptr;
-        const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-        it = graphs.emplace(c, exec).first;
+        CachedGraph g;
+        VF_TRY(capture_graph(h, s, [&] { return clip_tower_eager(h, c, h->feat, s); }, &g));
+        it = graphs.emplace(c, g).first;
     }
-    VF_CUDA(cudaGraphLaunch(it->second, s));
+    VF_CUDA(cudaGraphLaunch(it->second.exec, s));
     VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(c) * E * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    h->launches += h->fused_attn ? TOWER_LAUNCHES_FUSED : TOWER_LAUNCHES_SPLIT;
+    h->launches += it->second.launches;
     return VF_OK;
 }
 
@@ -311,7 +285,6 @@ static cudaStream_t activate(vf_clip* h, int l) {
     h->patches = L.patches; h->h = L.h; h->qkv = L.qkv; h->att = L.att; h->mlp = L.mlp; h->cls = L.cls; h->y = L.y;
     h->x = L.x; h->emb = L.emb; h->feat = L.feat;
     h->resized = L.resized; h->resize_tmp = L.resize_tmp; h->resized_cap = L.resized_cap; h->tmp_cap = L.tmp_cap;
-    h->cs = L.cs;
     return L.cs;
 }
 static void deactivate(vf_clip* h) {      // keep the (possibly grown) resize scratch with its lane
@@ -391,13 +364,9 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
     // frames/s -- larger chunks gain no GEMM efficiency and lose overlap of the copies with the tower.
     if (chunk_frames <= 0) chunk_frames = patch_size == 32 ? 256 : 126;
     if (chunk_frames > 4096) return fail(VF_ERR_INVALID, "clip_create: chunk_frames %d too large", chunk_frames);
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_clip* h = new vf_clip();
+    h->who = "clip_create";
     h->device = device;
     h->chunk = chunk_frames;
     h->patch = patch_size;
@@ -458,23 +427,21 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
         }
         for (int l = 0; l < h->n_lanes; ++l) {
             vf_clip::Lane& L = h->lanes[l];
-            VF_TRY(dev_alloc(h, &L.patches, C * P * PK));
-            VF_TRY(dev_alloc(h, &L.x, C * T * W));
-            VF_TRY(dev_alloc(h, &L.y, C * T * W));
-            VF_TRY(dev_alloc(h, &L.emb, C * P * W));
-            VF_TRY(dev_alloc(h, &L.h, C * T * W));
-            VF_TRY(dev_alloc(h, &L.qkv, C * T * 3 * W));
-            VF_TRY(dev_alloc(h, &L.att, C * T * W));
-            VF_TRY(dev_alloc(h, &L.mlp, C * T * MLPW));
-            VF_TRY(dev_alloc(h, &L.cls, C * W));
-            VF_TRY(dev_alloc(h, &L.feat, C * E));
+            VF_TRY(ralloc(h, &L.patches, C * P * PK));
+            VF_TRY(ralloc(h, &L.x, C * T * W));
+            VF_TRY(ralloc(h, &L.y, C * T * W));
+            VF_TRY(ralloc(h, &L.emb, C * P * W));
+            VF_TRY(ralloc(h, &L.h, C * T * W));
+            VF_TRY(ralloc(h, &L.qkv, C * T * 3 * W));
+            VF_TRY(ralloc(h, &L.att, C * T * W));
+            VF_TRY(ralloc(h, &L.mlp, C * T * MLPW));
+            VF_TRY(ralloc(h, &L.cls, C * W));
+            VF_TRY(ralloc(h, &L.feat, C * E));
             VF_CUDA(cudaStreamCreateWithFlags(&L.cs, cudaStreamNonBlocking));
             VF_CUDA(cudaEventCreateWithFlags(&L.ev_out, cudaEventDisableTiming));
         }
         VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
         {
-            const char* e = getenv("VF_NO_GRAPH");
-            h->use_graph = !(e && e[0] == '1');
             const char* r = getenv("VF_CLIP_RESID");     // acc (default) | y | mix (reduction for the MLP only)
             h->acc_o = !(r && (r[0] == 'y' || r[0] == 'm'));
             h->acc_m = !(r && r[0] == 'y');
@@ -499,23 +466,20 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
 
 int vf_clip_destroy(vf_clip_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
+    release(h);
     if (h->stage_u8) cudaFree(h->stage_u8);
     if (h->out_dev) cudaFree(h->out_dev);
     for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
     deactivate(h);
     for (int l = 0; l < 2; ++l) {
         vf_clip::Lane& L = h->lanes[l];
-        for (auto& kv : L.graphs) cudaGraphExecDestroy(kv.second);
+        for (auto& kv : L.graphs) cudaGraphExecDestroy(kv.second.exec);
         if (L.cs) cudaStreamDestroy(L.cs);
         if (L.ev_out) cudaEventDestroy(L.ev_out);
         if (L.resized) cudaFree(L.resized);
         if (L.resize_tmp) cudaFree(L.resize_tmp);
     }
     h->resized = nullptr; h->resize_tmp = nullptr;
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
     for (int i = 0; i < 2; ++i) {
         if (h->ev_copy[i]) cudaEventDestroy(h->ev_copy[i]);

@@ -25,7 +25,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -46,8 +45,8 @@ struct RnBlock {
 
 using namespace vf;
 
-struct vf_clip_rn : vf::ConvHost {
-    int device = 0, max_frames = 0, npx = 0, width = 0, embed = 0, heads = 0, out_dim = 0, tokens = 0;
+struct vf_clip_rn : vf::EngineCore {
+    int max_frames = 0, npx = 0, width = 0, embed = 0, heads = 0, out_dim = 0, tokens = 0;
     int layers[4] = {0, 0, 0, 0};
     ResConv stem[3];
     std::vector<RnBlock> blocks;
@@ -60,15 +59,13 @@ struct vf_clip_rn : vf::ConvHost {
     float *kvo = nullptr, *qo = nullptr;
     uint8_t *resized = nullptr, *resize_tmp = nullptr;        // grown on demand for the u8 entry's resize
     size_t resized_cap = 0, tmp_cap = 0;
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    bool use_graph = true;
-    std::map<int, std::pair<cudaGraphExec_t, int64_t>> graphs;     // frames -> (trunk graph, launches in it)
     int last_n = 0;
     int attn_n = 0;           // frames of the last vf_clip_rn_debug_attnpool (its intermediates stay readable)
 };
 
 namespace vf {
+
+static const double kEps = 1e-5;                                // BatchNorm2d
 
 static Vol2 stem_vol(const vf_clip_rn* h, int n) {
     const int S = h->npx / 2;
@@ -90,7 +87,7 @@ static int64_t numel_of(const ResTensors& T, const std::string& name) {
 static int prep_stem1(vf_clip_rn* h, ResConv& cw, const ResTensors& T, int co) {
     cw.ntaps = 2; cw.k_per_tap = 64;
     for (int a = 0; a < 2; ++a) { cw.dh[a] = a - 1; cw.dw[a] = -1; }
-    return upload_conv(h, cw, T, "visual.conv1", "visual.bn1", co, 3, 3, 16, [](int kh, int kw, int c) {
+    return upload_conv(h, cw, T, "visual.conv1", "visual.bn1", kEps, {co, 3, 1, 3, 3}, 16, [](int, int kh, int kw, int c) {
         const int a = (kh + 1) / 2, ph = (kh + 1) % 2, b = (kw + 1) / 2, pw = (kw + 1) % 2;
         return a * 64 + b * 32 + (ph * 2 + pw) * 4 + c;
     });
@@ -101,14 +98,15 @@ static int prep_stem1(vf_clip_rn* h, ResConv& cw, const ResTensors& T, int co) {
 static int prep_pooled(vf_clip_rn* h, ResConv& cw, const ResTensors& T, const std::string& name, const std::string& bn,
                        int co, int ci) {
     cw.ntaps = 1; cw.k_per_tap = 8 * ci;
-    return upload_conv(h, cw, T, name, bn, co, ci, 1, ci, [](int, int, int c) { return c; }, 4, 2 * ci, 0.25f);
+    return upload_conv(h, cw, T, name, bn, kEps, {co, ci, 1, 1, 1}, ci, [](int, int, int, int c) { return c; }, 0, 4, 2 * ci,
+                       0.25f);
 }
 
 // nn.Linear (weight [co][ci], bias [co]) on split rows of 2*ci; w / b are host pointers already checked
 static int prep_linear(vf_clip_rn* h, ResConv& cw, const float* w, const float* b, int co, int ci) {
     cw.ntaps = 1; cw.k_per_tap = 2 * ci;
     const std::vector<float> sc(size_t(co), 1.f), sh(b, b + co);
-    return upload_weights(h, cw, w, co, ci, 1, ci, [](int, int, int c) { return c; }, sc, sh);
+    return upload_weights(h, cw, w, {co, ci, 1, 1, 1}, ci, [](int, int, int, int c) { return c; }, sc, sh);
 }
 
 // one linear on M rows of X (row pitch `pitch` elements) -> fp32 rows of ldo
@@ -196,35 +194,6 @@ static int run_trunk(vf_clip_rn* h, int m, cudaStream_t s) {
     return run_attention(h, h->stage_out[3], m, s);
 }
 
-static int trunk_graph(vf_clip_rn* h, int m, cudaStream_t s) {
-    if (!h->use_graph || gemm_profile_on()) return run_trunk(h, m, s);
-    auto it = h->graphs.find(m);
-    if (it == h->graphs.end()) {
-        const int64_t before = h->launches;
-        cudaGraph_t graph = nullptr;
-        VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-        const int st = run_trunk(h, m, s);
-        const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-        const int64_t n_launch = h->launches - before;
-        h->launches = before;
-        if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-        if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-        cudaGraphExec_t exec = nullptr;
-        const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-        // bounded cache: ragged last chunks of many videos must not pile up executable graphs
-        if (h->graphs.size() >= 16) {
-            cudaGraphExecDestroy(h->graphs.begin()->second.first);
-            h->graphs.erase(h->graphs.begin());
-        }
-        it = h->graphs.emplace(m, std::make_pair(exec, n_launch)).first;
-    }
-    VF_CUDA(cudaGraphLaunch(it->second.first, s));
-    h->launches += it->second.second;
-    return VF_OK;
-}
-
 // a resize buffer of at least `need` bytes; the engine stream is drained before an old one is freed
 static int grow(vf_clip_rn* h, uint8_t** p, size_t* cap, size_t need) {
     if (need <= *cap) return VF_OK;
@@ -258,8 +227,7 @@ static int clip_rn_encode(vf_clip_rn* h, const void* frames, int is_u8, int n, i
         VF_TRY(grow(h, &h->resized, &h->resized_cap, size_t(h->max_frames) * rh * rw * 3));
         VF_TRY(grow(h, &h->resize_tmp, &h->tmp_cap, size_t(h->max_frames) * H * rw * 3));
     }
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     for (int off = 0; off < n; off += h->max_frames) {      // calls beyond the workspace run in chunks
         const int m = std::min(h->max_frames, n - off);
         const void* src = is_u8 ? static_cast<const void*>(static_cast<const uint8_t*>(frames) + off * frame_elems)
@@ -271,15 +239,13 @@ static int clip_rn_encode(vf_clip_rn* h, const void* frames, int is_u8, int n, i
             src = h->resized;
         }
         VF_TRY(clip_rn_input_pack(src, is_u8, m, rh, rw, cy, cx, npx, h->s0, s));
-        VF_TRY(trunk_graph(h, m, s));
+        VF_TRY(run_graphed(h, {m, 0, 0, 0}, [&] { return run_trunk(h, m, s); }));
         VF_TRY(run_cproj(h, m, out + size_t(off) * h->out_dim, s));
         h->launches += 1;       // the input pack
         h->last_n = m;
         h->attn_n = 0;
     }
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
-    return VF_OK;
+    return leave(h, user);
 }
 
 }  // namespace vf
@@ -288,15 +254,9 @@ extern "C" {
 
 int vf_clip_rn_destroy(vf_clip_rn_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
+    release(h);
     if (h->resized) cudaFree(h->resized);
     if (h->resize_tmp) cudaFree(h->resize_tmp);
-    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second.first);
-    if (h->cs) cudaStreamDestroy(h->cs);
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
-    if (h->ev_out) cudaEventDestroy(h->ev_out);
     delete h;
     return VF_OK;
 }
@@ -331,12 +291,7 @@ int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_
                     "multiple of 8 x %d", (long long)n_cp, E);
     const int npx = 32 * side;
     if (max_frames <= 0) max_frames = npx <= 224 ? 64 : npx <= 288 ? 32 : 16;
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_clip_rn* h = new vf_clip_rn();
     h->who = "clip_rn_create";
     h->device = device; h->max_frames = max_frames; h->npx = npx; h->width = width; h->embed = E;
@@ -346,8 +301,8 @@ int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_
         auto rows = [](const Vol2& v) { return size_t(v.rows()); };
         const Vol2 sv = stem_vol(h, 1);
         VF_TRY(prep_stem1(h, h->stem[0], T, width / 2));
-        VF_TRY(prep_same(h, h->stem[1], T, "visual.conv2", "visual.bn2", width / 2, width / 2, 3));
-        VF_TRY(prep_same(h, h->stem[2], T, "visual.conv3", "visual.bn3", width, width / 2, 3));
+        VF_TRY(prep_same(h, h->stem[1], T, "visual.conv2", "visual.bn2", kEps, width / 2, width / 2, 3));
+        VF_TRY(prep_same(h, h->stem[2], T, "visual.conv3", "visual.bn3", kEps, width, width / 2, 3));
         // per-frame element counts of the working buffers, found while walking the blocks
         size_t e_act = rows(sv) * 2 * width, e_ph = 8;
         int cin = width;
@@ -364,15 +319,15 @@ int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_
                 const Vol2& vc = B.pool_in ? vo : vi;
                 const std::string p = "visual.layer" + std::to_string(L + 1) + "." + std::to_string(b);
                 if (B.pool_in) VF_TRY(prep_pooled(h, B.c1, T, p + ".conv1", p + ".bn1", planes, B.cin));
-                else           VF_TRY(prep_same(h, B.c1, T, p + ".conv1", p + ".bn1", planes, B.cin, 1));
-                VF_TRY(prep_same(h, B.c2, T, p + ".conv2", p + ".bn2", planes, planes, 3));
+                else           VF_TRY(prep_same(h, B.c1, T, p + ".conv1", p + ".bn1", kEps, planes, B.cin, 1));
+                VF_TRY(prep_same(h, B.c2, T, p + ".conv2", p + ".bn2", kEps, planes, planes, 3));
                 if (B.stride == 2) VF_TRY(prep_pooled(h, B.c3, T, p + ".conv3", p + ".bn3", cout, planes));
-                else               VF_TRY(prep_same(h, B.c3, T, p + ".conv3", p + ".bn3", cout, planes, 1));
+                else               VF_TRY(prep_same(h, B.c3, T, p + ".conv3", p + ".bn3", kEps, cout, planes, 1));
                 if (B.down) {
                     if (B.stride == 2 || B.pool_in)
                         VF_TRY(prep_pooled(h, B.dn, T, p + ".downsample.0", p + ".downsample.1", cout, B.cin));
                     else
-                        VF_TRY(prep_same(h, B.dn, T, p + ".downsample.0", p + ".downsample.1", cout, B.cin, 1));
+                        VF_TRY(prep_same(h, B.dn, T, p + ".downsample.0", p + ".downsample.1", kEps, cout, B.cin, 1));
                 }
                 e_act = std::max({e_act, rows(vc) * 2 * planes, rows(vo) * 2 * cout});
                 if (B.stride == 2) e_ph = std::max(e_ph, rows(vo) * 8 * planes);
@@ -411,12 +366,7 @@ int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_
         VF_TRY(ralloc(h, &h->kvo, F * TE));
         VF_TRY(ralloc(h, &h->qo, F * E));
         VF_TRY(ralloc(h, &h->att, F * 2 * E));
-        VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-        const char* e = getenv("VF_NO_GRAPH");
-        h->use_graph = !(e && e[0] == '1');
-        return VF_OK;
+        return open_stream(h);
     };
     const int st = body();
     if (st != VF_OK) { vf_clip_rn_destroy(h); return st; }
@@ -478,17 +428,14 @@ int vf_clip_rn_debug_block(vf_clip_rn_t* h, int block, const void* x_pairs, int 
     h->last_n = 0;
     h->attn_n = 0;
     const size_t in_h = size_t(vi.rows()) * 2 * B.cin, out_h = size_t(vo.rows()) * 2 * B.cout;
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, in_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     VF_TRY(run_block(h, B, h->bufA, vi, vo, h->bufB, s));
     VF_CUDA(cudaMemcpyAsync(out_pairs, h->bufB, out_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     VF_CUDA(cudaMemcpyAsync(branch_out, h->t1, out_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     if (B.down && shortcut_out)
         VF_CUDA(cudaMemcpyAsync(shortcut_out, h->ds, out_h * sizeof(__half), cudaMemcpyDeviceToDevice, s));
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
-    return VF_OK;
+    return leave(h, user);
 }
 
 int vf_clip_rn_debug_attnpool(vf_clip_rn_t* h, const void* x_pairs, int n, float* features, void* stream) {
@@ -499,14 +446,12 @@ int vf_clip_rn_debug_attnpool(vf_clip_rn_t* h, const void* x_pairs, int n, float
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
     VF_CUDA(cudaSetDevice(h->device));
     h->last_n = 0;
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, size_t(v4.rows()) * 2 * h->embed * sizeof(__half),
                             cudaMemcpyDeviceToDevice, s));
     VF_TRY(run_attention(h, h->bufA, n, s));
     VF_TRY(run_cproj(h, n, features, s));
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
+    VF_TRY(leave(h, user));
     h->attn_n = n;
     return VF_OK;
 }

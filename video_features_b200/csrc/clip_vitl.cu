@@ -35,10 +35,8 @@ struct VitlLayer {
 
 using namespace vf;
 
-struct vf_clip_vitl {
-    int device = 0, max_frames = 0, npx = 0, tokens = 0, patches_per_frame = 0;
-    int64_t launches = 0;
-    std::vector<void*> allocs;
+struct vf_clip_vitl : vf::EngineCore {
+    int max_frames = 0, npx = 0, tokens = 0, patches_per_frame = 0;
     // weights
     __half* w_patch = nullptr;      // [1024, VITL_PK] (conv1, zero columns 588..591)
     __half* w_proj = nullptr;       // [768, 1024] (proj^T)
@@ -50,30 +48,15 @@ struct vf_clip_vitl {
     float *x = nullptr, *emb = nullptr, *feat = nullptr;
     uint8_t *resized = nullptr, *resize_tmp = nullptr;        // grown on demand for the u8 entry's resize
     size_t resized_cap = 0, tmp_cap = 0;
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    bool use_graph = true;
-    std::map<int, cudaGraphExec_t> graphs;      // frames in chunk -> instantiated tower graph (writes feat)
     std::map<int, int> seen;                    // frames in chunk -> times run without a graph
 };
 
 namespace vf {
 
 constexpr size_t kVitlMaxGraphs = 16;
-constexpr int VL_TOWER_LAUNCHES = 2 + 6 * VL_LAYERS + 2;
 
-template <typename Tp>
-static int vl_alloc(vf_clip_vitl* h, Tp** p, size_t count) {
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, count * sizeof(Tp));
-    if (e != cudaSuccess)
-        return fail(VF_ERR_NOMEM, "clip_vitl_create: cudaMalloc(%zu bytes): %s", count * sizeof(Tp), cudaGetErrorString(e));
-    h->allocs.push_back(q);
-    *p = static_cast<Tp*>(q);
-    return VF_OK;
-}
 static int vl_upload_f32(vf_clip_vitl* h, float** dst, const float* src, size_t count) {
-    VF_TRY(vl_alloc(h, dst, count));
+    VF_TRY(ralloc(h, dst, count));
     VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
     return VF_OK;
 }
@@ -84,7 +67,7 @@ static int vl_upload_f16(vf_clip_vitl* h, __half** dst, const float* src, size_t
     std::vector<__half> tmp(rows * ld, __float2half_rn(0.f));
     for (size_t r = 0; r < rows; ++r)
         for (size_t c = 0; c < cols; ++c) tmp[r * ld + c] = __float2half_rn(transpose ? src[c * rows + r] : src[r * cols + c]);
-    VF_TRY(vl_alloc(h, dst, rows * ld));
+    VF_TRY(ralloc(h, dst, rows * ld));
     VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
     return VF_OK;
 }
@@ -150,27 +133,18 @@ static int vl_tower_eager(vf_clip_vitl* h, int c, float* out, cudaStream_t s) {
 // it the second time the size is seen (one-off sizes run eagerly); at most kVitlMaxGraphs graphs are kept
 static int vl_tower_chunk(vf_clip_vitl* h, int c, float* out, cudaStream_t s) {
     if (!h->use_graph || gemm_profile_on()) return vl_tower_eager(h, c, out, s);
-    auto it = h->graphs.find(c);
+    const GraphKey key{c, 0, 0, 0};
+    auto it = h->graphs.find(key);
     if (it == h->graphs.end()) {
         if (h->seen.size() > 4096) h->seen.clear();
         if (++h->seen[c] < 2 || h->graphs.size() >= kVitlMaxGraphs) return vl_tower_eager(h, c, out, s);
-        const int64_t before = h->launches;
-        cudaGraph_t graph = nullptr;
-        VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-        const int st = vl_tower_eager(h, c, h->feat, s);
-        const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-        h->launches = before;
-        if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-        if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-        cudaGraphExec_t exec = nullptr;
-        const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-        it = h->graphs.emplace(c, exec).first;
+        CachedGraph g;
+        VF_TRY(capture_graph(h, s, [&] { return vl_tower_eager(h, c, h->feat, s); }, &g));
+        it = h->graphs.emplace(key, g).first;
     }
-    VF_CUDA(cudaGraphLaunch(it->second, s));
+    VF_CUDA(cudaGraphLaunch(it->second.exec, s));
     VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(c) * VL_EMBED * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    h->launches += VL_TOWER_LAUNCHES;
+    h->launches += it->second.launches;
     return VF_OK;
 }
 
@@ -231,9 +205,7 @@ static int vl_encode(vf_clip_vitl* h, const void* frames, int is_u8, int n, int 
     if (is_u8) VF_TRY(vl_geometry(h, H, W, &g));
     const size_t frame_elems = is_u8 ? size_t(H) * W * 3 : size_t(3) * h->npx * h->npx;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_CUDA(cudaSetDevice(h->device));
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     const int step = vl_step(h, n);
     for (int off = 0; off < n; off += step) {
         const int c = n - off < step ? n - off : step;
@@ -245,9 +217,7 @@ static int vl_encode(vf_clip_vitl* h, const void* frames, int is_u8, int n, int 
         }
         VF_TRY(vl_tower_chunk(h, c, out + size_t(off) * VL_EMBED, s));
     }
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
-    return VF_OK;
+    return leave(h, user);
 }
 
 static int vl_debug_args(vf_clip_vitl* h, const void* a, const void* b, int n, const char* what) {
@@ -264,15 +234,9 @@ extern "C" {
 
 int vf_clip_vitl_destroy(vf_clip_vitl_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
+    release(h);
     if (h->resized) cudaFree(h->resized);
     if (h->resize_tmp) cudaFree(h->resize_tmp);
-    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
-    if (h->cs) cudaStreamDestroy(h->cs);
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
-    if (h->ev_out) cudaEventDestroy(h->ev_out);
     delete h;
     return VF_OK;
 }
@@ -325,13 +289,9 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
     // it near 2.5 GB.
     if (max_frames <= 0) max_frames = npx == 224 ? 352 : 160;
     if (max_frames > 4096) return fail(VF_ERR_INVALID, "clip_vitl_create: max_frames %d too large", max_frames);
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_clip_vitl* h = new vf_clip_vitl();
+    h->who = "clip_vitl_create";
     h->device = device; h->max_frames = max_frames; h->npx = npx;
     h->patches_per_frame = grid * grid; h->tokens = grid * grid + 1;
     auto body = [&]() -> int {
@@ -371,21 +331,16 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
             }
         }
         const size_t F = size_t(max_frames);
-        VF_TRY(vl_alloc(h, &h->patches, F * P * VITL_PK));
-        VF_TRY(vl_alloc(h, &h->emb, F * P * W));
-        VF_TRY(vl_alloc(h, &h->x, F * Tk * W));
-        VF_TRY(vl_alloc(h, &h->h, F * Tk * W));
-        VF_TRY(vl_alloc(h, &h->qkv, F * Tk * 3 * W));
-        VF_TRY(vl_alloc(h, &h->att, F * Tk * W));
-        VF_TRY(vl_alloc(h, &h->mlp, F * Tk * VL_MLP));
-        VF_TRY(vl_alloc(h, &h->cls, F * W));
-        VF_TRY(vl_alloc(h, &h->feat, F * VL_EMBED));
-        VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-        const char* e = getenv("VF_NO_GRAPH");
-        h->use_graph = !(e && e[0] == '1');
-        return VF_OK;
+        VF_TRY(ralloc(h, &h->patches, F * P * VITL_PK));
+        VF_TRY(ralloc(h, &h->emb, F * P * W));
+        VF_TRY(ralloc(h, &h->x, F * Tk * W));
+        VF_TRY(ralloc(h, &h->h, F * Tk * W));
+        VF_TRY(ralloc(h, &h->qkv, F * Tk * 3 * W));
+        VF_TRY(ralloc(h, &h->att, F * Tk * W));
+        VF_TRY(ralloc(h, &h->mlp, F * Tk * VL_MLP));
+        VF_TRY(ralloc(h, &h->cls, F * W));
+        VF_TRY(ralloc(h, &h->feat, F * VL_EMBED));
+        return open_stream(h);
     };
     const int st = body();
     if (st != VF_OK) { vf_clip_vitl_destroy(h); return st; }

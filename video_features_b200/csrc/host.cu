@@ -1,7 +1,8 @@
 // Host-side pieces of libvfeat.so that are not kernels: error text, the frame sampler and shard arithmetic,
-// Pillow coefficient tables, resize / transform entry points.
+// Pillow coefficient tables, resize / transform entry points, and the handle core every engine driver embeds.
 #include <math.h>
 #include <stdarg.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include <map>
@@ -148,6 +149,98 @@ int center_crop_offset(int dim, int crop) {
     if ((e & 1) == 0) return -(e / 2);
     const int q = e / 2;
     return -((q & 1) ? q + 1 : q);
+}
+
+// ---- engine handles
+int check_device(int device) {
+    VF_CUDA(cudaSetDevice(device));
+    int major = 0, minor = 0;
+    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
+    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+    if (major != 9 || minor != 0)
+        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    return VF_OK;
+}
+
+bool graphs_enabled() {
+    const char* e = getenv("VF_NO_GRAPH");
+    return !(e && e[0] == '1');
+}
+
+int engine_alloc(EngineCore* h, void** p, size_t bytes) {
+    void* q = nullptr;
+    bytes += 65536;
+    cudaError_t e = cudaMalloc(&q, bytes);
+    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "%s: cudaMalloc(%zu bytes): %s", h->who, bytes, cudaGetErrorString(e));
+    h->allocs.push_back(q);
+    VF_CUDA(cudaMemset(q, 0, bytes));
+    *p = q;
+    return VF_OK;
+}
+
+int open_stream(EngineCore* h) {
+    VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
+    VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
+    VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
+    return VF_OK;
+}
+
+int enter(EngineCore* h, cudaStream_t user) {
+    VF_CUDA(cudaSetDevice(h->device));
+    VF_CUDA(cudaEventRecord(h->ev_in, user));
+    VF_CUDA(cudaStreamWaitEvent(h->cs, h->ev_in, 0));
+    return VF_OK;
+}
+
+int leave(EngineCore* h, cudaStream_t user) {
+    VF_CUDA(cudaEventRecord(h->ev_out, h->cs));
+    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
+    return VF_OK;
+}
+
+void release(EngineCore* h) {
+    cudaSetDevice(h->device);
+    cudaDeviceSynchronize();
+    for (void* p : h->allocs) cudaFree(p);
+    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second.exec);
+    if (h->cs) cudaStreamDestroy(h->cs);
+    if (h->ev_in) cudaEventDestroy(h->ev_in);
+    if (h->ev_out) cudaEventDestroy(h->ev_out);
+}
+
+int capture_graph(EngineCore* h, cudaStream_t s, const std::function<int()>& run, CachedGraph* g) {
+    const int64_t before = h->launches;
+    cudaGraph_t graph = nullptr;
+    VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
+    const int st = run();
+    const cudaError_t ce = cudaStreamEndCapture(s, &graph);
+    g->launches = h->launches - before;
+    h->launches = before;
+    if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
+    if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
+    const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
+    return VF_OK;
+}
+
+int run_graphed(EngineCore* h, const GraphKey& key, const std::function<int()>& run) {
+    if (!h->use_graph || gemm_profile_on()) return run();
+    auto it = h->graphs.find(key);
+    if (it == h->graphs.end()) {
+        CachedGraph g;
+        VF_TRY(capture_graph(h, h->cs, run, &g));
+        // bounded cache: ragged last chunks of many videos, or videos of many resolutions, must not pile up executable
+        // graphs; an evicted graph that is still running is freed by the runtime when it completes
+        if (h->graphs.size() >= 16) {
+            cudaGraphExecDestroy(h->graphs.begin()->second.exec);
+            h->graphs.erase(h->graphs.begin());
+        }
+        it = h->graphs.emplace(key, g).first;
+    }
+    VF_CUDA(cudaGraphLaunch(it->second.exec, h->cs));
+    h->launches += it->second.launches;
+    return VF_OK;
 }
 
 }  // namespace vf

@@ -24,8 +24,6 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <map>
-#include <utility>
 #include <vector>
 
 #include "internal.h"
@@ -84,39 +82,20 @@ static const int kMixed[9][7] = {
     {512, 160, 112, 224, 24, 64, 64}, {512, 128, 128, 256, 24, 64, 64},  {512, 112, 144, 288, 32, 64, 64},
     {528, 256, 160, 320, 32, 128, 128}, {832, 256, 160, 320, 32, 128, 128}, {832, 384, 192, 384, 48, 128, 128}};
 
-struct vf_i3d {
-    int device = 0, cin = 3, max_stacks = 0, max_T = 0;
+struct vf_i3d : vf::EngineCore {
+    int cin = 3, max_stacks = 0, max_T = 0;
     int nsplit = 2;
-    std::vector<void*> allocs;
     ConvUnit units[VF_I3D_UNITS];
     // activation buffers (sized for max_stacks x max_T at create)
     __half *s0 = nullptr, *a1 = nullptr, *p1 = nullptr, *c2b = nullptr, *c2c = nullptr;
     __half *bufA = nullptr, *bufB = nullptr, *t1 = nullptr, *t2 = nullptr, *tp = nullptr;
     size_t cap_s0 = 0, cap_a1 = 0, cap_s1 = 0, cap_rows2 = 0;
-    int64_t launches = 0;
-    // engine-owned stream + per-(clips, T) CUDA graph of the trunk (same scheme as the CLIP tower)
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    bool use_graph = true;
-    std::map<std::pair<int, int>, cudaGraphExec_t> graphs;
     float* feat = nullptr;            // [max_stacks, 1024] trunk output
     // last forward's stage views, for vf_i3d_read_stage
     struct StageRef { const __half* p; Vol v; int C; } stages[5];
 };
 
 namespace vf {
-
-template <typename Tp>
-static int i3d_alloc(vf_i3d* h, Tp** p, size_t count) {
-    // + 64 KB: the overlapping-row TMA view of a conv input (row p = k_per_tap elements from element p*C) extends
-    // (kw-1)*C elements past the last row; those reads meet zero weights but must stay inside the allocation
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(Tp) + 65536);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "cudaMalloc(%zu bytes): %s", count * sizeof(Tp), cudaGetErrorString(e));
-    h->allocs.push_back(q);
-    *p = static_cast<Tp*>(q);
-    return VF_OK;
-}
 
 // fold BN, re-lay the filter for the shifted-row GEMM, split into hi/lo fp16, upload
 static int prepare_unit(vf_i3d* h, ConvUnit& u, const vf_conv_unit& src, int idx) {
@@ -198,9 +177,9 @@ static int prepare_unit(vf_i3d* h, ConvUnit& u, const vf_conv_unit& src, int idx
         sc[o] = s;
         bi[o] = src.bn_b[o] - src.bn_mean[o] * s;
     }
-    VF_TRY(i3d_alloc(h, &u.w, wh.size()));
-    VF_TRY(i3d_alloc(h, &u.scale, size_t(co)));
-    VF_TRY(i3d_alloc(h, &u.bias, size_t(co)));
+    VF_TRY(ralloc(h, &u.w, wh.size()));
+    VF_TRY(ralloc(h, &u.scale, size_t(co)));
+    VF_TRY(ralloc(h, &u.bias, size_t(co)));
     VF_CUDA(cudaMemcpy(u.w, wh.data(), wh.size() * sizeof(__half), cudaMemcpyHostToDevice));
     VF_CUDA(cudaMemcpy(u.scale, sc.data(), co * sizeof(float), cudaMemcpyHostToDevice));
     VF_CUDA(cudaMemcpy(u.bias, bi.data(), co * sizeof(float), cudaMemcpyHostToDevice));
@@ -269,13 +248,9 @@ int vf_i3d_create(vf_i3d_t** out, const vf_i3d_weights* w, int in_channels, int 
     if (in_channels != 3 && in_channels != 2) return fail(VF_ERR_INVALID, "i3d_create: in_channels must be 3 (rgb) or 2 (flow)");
     if (max_stacks <= 0) max_stacks = 4;
     if (max_T <= 0) max_T = 64;
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_i3d* h = new vf_i3d();
+    h->who = "i3d_create";
     h->device = device; h->cin = in_channels; h->max_stacks = max_stacks; h->max_T = max_T;
     {
         const char* e = getenv("VF_I3D_FAST");
@@ -287,28 +262,21 @@ int vf_i3d_create(vf_i3d_t** out, const vf_i3d_weights* w, int in_channels, int 
         const size_t n = size_t(max_stacks);
         const int T1 = max_T / 2, Tq = T1 + 3;       // stem: floor((T + 5 - 7) / 2) + 1 = T / 2
         const size_t rows0 = n * Tq * 115 * 115;
-        VF_TRY(i3d_alloc(h, &h->s0, rows0 * 32 * in_channels + 4096));
-        VF_TRY(i3d_alloc(h, &h->a1, rows0 * 128));          // pair tensors: 2 x channels
+        VF_TRY(ralloc(h, &h->s0, rows0 * 32 * in_channels + 4096));
+        VF_TRY(ralloc(h, &h->a1, rows0 * 128));          // pair tensors: 2 x channels
         const size_t rows1 = n * (T1 + 2) * 58 * 58;
-        VF_TRY(i3d_alloc(h, &h->p1, rows1 * 128));
-        VF_TRY(i3d_alloc(h, &h->c2b, rows1 * 64));
-        VF_TRY(i3d_alloc(h, &h->c2c, rows1 * 384));
+        VF_TRY(ralloc(h, &h->p1, rows1 * 128));
+        VF_TRY(ralloc(h, &h->c2b, rows1 * 64));
+        VF_TRY(ralloc(h, &h->c2c, rows1 * 384));
         const size_t rows2 = n * (T1 + 2) * 30 * 30;    // largest Mixed stage
-        VF_TRY(i3d_alloc(h, &h->bufA, rows2 * 2048));
-        VF_TRY(i3d_alloc(h, &h->bufB, rows2 * 2048));
-        VF_TRY(i3d_alloc(h, &h->t1, rows2 * 192));
-        VF_TRY(i3d_alloc(h, &h->t2, rows2 * 64));
-        VF_TRY(i3d_alloc(h, &h->tp, rows2 * 1664));
+        VF_TRY(ralloc(h, &h->bufA, rows2 * 2048));
+        VF_TRY(ralloc(h, &h->bufB, rows2 * 2048));
+        VF_TRY(ralloc(h, &h->t1, rows2 * 192));
+        VF_TRY(ralloc(h, &h->t2, rows2 * 64));
+        VF_TRY(ralloc(h, &h->tp, rows2 * 1664));
         h->cap_rows2 = rows2;
-        VF_TRY(i3d_alloc(h, &h->feat, n * 1024));
-        VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-        {
-            const char* e = getenv("VF_NO_GRAPH");
-            h->use_graph = !(e && e[0] == '1');
-        }
-        return VF_OK;
+        VF_TRY(ralloc(h, &h->feat, n * 1024));
+        return open_stream(h);
     };
     const int st = body();
     if (st != VF_OK) { vf_i3d_destroy(h); return st; }
@@ -318,13 +286,7 @@ int vf_i3d_create(vf_i3d_t** out, const vf_i3d_weights* w, int in_channels, int 
 
 int vf_i3d_destroy(vf_i3d_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
-    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
-    if (h->cs) cudaStreamDestroy(h->cs);
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
-    if (h->ev_out) cudaEventDestroy(h->ev_out);
+    release(h);
     delete h;
     return VF_OK;
 }
@@ -389,49 +351,19 @@ static int i3d_trunk(vf_i3d* h, int nb, int T, float* out, cudaStream_t s) {
     // ---- AvgPool3d((2,7,7),1) + mean over time
     VF_TRY(launch_i3d_head(h->bufB, v4, 1024, out, s));
     h->launches += 5;
-    set_stages(h, nb, T);
     return VF_OK;
 }
 
-// trunk through a CUDA graph (captured once per (clips, T)); the features land in h->feat and are copied out
+// the trunk, eagerly into out or through the graph of (clips, T), whose features land in h->feat and are copied out
 static int i3d_trunk_graphed(vf_i3d* h, int nb, int T, float* out, cudaStream_t s) {
-    if (!h->use_graph || gemm_profile_on()) return i3d_trunk(h, nb, T, out, s);
-    auto key = std::make_pair(nb, T);
-    auto it = h->graphs.find(key);
-    if (it == h->graphs.end()) {
-        const int64_t before = h->launches;
-        cudaGraph_t graph = nullptr;
-        VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-        const int st = i3d_trunk(h, nb, T, h->feat, s);
-        const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-        if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-        if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-        cudaGraphExec_t exec = nullptr;
-        const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-        if (h->graphs.size() >= 16) {          // bounded cache (an evicted graph still running is freed on completion)
-            cudaGraphExecDestroy(h->graphs.begin()->second);
-            h->graphs.erase(h->graphs.begin());
-        }
-        it = h->graphs.emplace(key, exec).first;
-        h->launches = before;
+    if (!h->use_graph || gemm_profile_on()) {
+        VF_TRY(i3d_trunk(h, nb, T, out, s));
+    } else {
+        VF_TRY(run_graphed(h, {nb, T, 0, 0}, [&] { return i3d_trunk(h, nb, T, h->feat, s); }));
+        VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(nb) * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        h->launches += 1;
     }
-    VF_CUDA(cudaGraphLaunch(it->second, s));
     set_stages(h, nb, T);
-    VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(nb) * 1024 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    h->launches += 72;
-    return VF_OK;
-}
-static int i3d_enter(vf_i3d* h, cudaStream_t user) {
-    VF_CUDA(cudaSetDevice(h->device));
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(h->cs, h->ev_in, 0));
-    return VF_OK;
-}
-static int i3d_leave(vf_i3d* h, cudaStream_t user) {
-    VF_CUDA(cudaEventRecord(h->ev_out, h->cs));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
     return VF_OK;
 }
 
@@ -448,14 +380,14 @@ int vf_i3d_forward_f32(vf_i3d_t* h, const float* clips, int n, int T, float* out
     VF_TRY(i3d_check(h, clips, n, T, out, 0));
     if (n <= 0) return VF_OK;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_TRY(i3d_enter(h, user));
+    VF_TRY(enter(h, user));
     for (int b0 = 0; b0 < n; b0 += h->max_stacks) {
         const int nb = (n - b0 < h->max_stacks) ? (n - b0) : h->max_stacks;
         VF_TRY(launch_i3d_phase_pack_f32(clips + size_t(b0) * h->cin * T * 224 * 224, nb, h->cin, T, h->s0, T / 2 + 3, s));
         h->launches += 1;
         VF_TRY(i3d_trunk_graphed(h, nb, T, out + size_t(b0) * 1024, s));
     }
-    return i3d_leave(h, user);
+    return leave(h, user);
 }
 
 int vf_i3d_forward_u8(vf_i3d_t* h, const uint8_t* frames, int n, int T, int Hr, int Wr, float* out, void* stream) {
@@ -469,7 +401,7 @@ int vf_i3d_forward_u8_strided(vf_i3d_t* h, const uint8_t* frames, int n, int T, 
     if (Hr < 224 || Wr < 224) return fail(VF_ERR_INVALID, "i3d_forward_u8: %dx%d frames are smaller than the 224 crop", Hr, Wr);
     if (n <= 0) return VF_OK;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_TRY(i3d_enter(h, user));
+    VF_TRY(enter(h, user));
     const int cy = (Hr - 224) / 2, cx = (Wr - 224) / 2;     // TensorCenterCrop: floor offsets (transforms.py:14-15)
     for (int b0 = 0; b0 < n; b0 += h->max_stacks) {
         const int nb = (n - b0 < h->max_stacks) ? (n - b0) : h->max_stacks;
@@ -478,7 +410,7 @@ int vf_i3d_forward_u8_strided(vf_i3d_t* h, const uint8_t* frames, int n, int T, 
         h->launches += 1;
         VF_TRY(i3d_trunk_graphed(h, nb, T, out + size_t(b0) * 1024, s));
     }
-    return i3d_leave(h, user);
+    return leave(h, user);
 }
 
 int vf_i3d_forward_flow(vf_i3d_t* h, const float* flow, int n, int T, int H, int W, float* out, void* stream) {
@@ -486,7 +418,7 @@ int vf_i3d_forward_flow(vf_i3d_t* h, const float* flow, int n, int T, int H, int
     if (H < 224 || W < 224) return fail(VF_ERR_INVALID, "i3d_forward_flow: %dx%d flow is smaller than the 224 crop", H, W);
     if (n <= 0) return VF_OK;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_TRY(i3d_enter(h, user));
+    VF_TRY(enter(h, user));
     const int cy = (H - 224) / 2, cx = (W - 224) / 2;
     for (int b0 = 0; b0 < n; b0 += h->max_stacks) {
         const int nb = (n - b0 < h->max_stacks) ? (n - b0) : h->max_stacks;
@@ -494,7 +426,7 @@ int vf_i3d_forward_flow(vf_i3d_t* h, const float* flow, int n, int T, int H, int
         h->launches += 1;
         VF_TRY(i3d_trunk_graphed(h, nb, T, out + size_t(b0) * 1024, s));
     }
-    return i3d_leave(h, user);
+    return leave(h, user);
 }
 
 int vf_i3d_read_stage(vf_i3d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream) {
@@ -506,9 +438,9 @@ int vf_i3d_read_stage(vf_i3d_t* h, int stage, float* out, int64_t capacity, int*
     if (!out) return VF_OK;
     if (capacity < need) return fail(VF_ERR_INVALID, "i3d_read_stage: capacity %lld < %lld", (long long)capacity, (long long)need);
     cudaStream_t user = static_cast<cudaStream_t>(stream);
-    VF_TRY(i3d_enter(h, user));
+    VF_TRY(enter(h, user));
     VF_TRY(launch_unpack_ndhwc(r.p, r.v, r.C, 0, r.C, 2 * r.C, r.C, out, h->cs));      // retained stages are pair tensors
-    return i3d_leave(h, user);
+    return leave(h, user);
 }
 
 int vf_i3d_debug_mixed(vf_i3d_t* h, int block, const void* x_pairs, int n, int T, void* out_pairs, void* stream) {
@@ -524,11 +456,11 @@ int vf_i3d_debug_mixed(vf_i3d_t* h, int block, const void* x_pairs, int n, int T
     const int cin = c[0], ctot = c[1] + c[3] + c[5] + c[6];
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
     for (vf_i3d::StageRef& r : h->stages) r.p = nullptr;      // bufA / bufB no longer hold the last forward's stages
-    VF_TRY(i3d_enter(h, user));
+    VF_TRY(enter(h, user));
     VF_CUDA(cudaMemcpyAsync(h->bufA, x_pairs, size_t(v.rows()) * 2 * cin * sizeof(__half), cudaMemcpyDeviceToDevice, s));
     VF_TRY(mixed_block(h, block, h->bufA, v, h->bufB, s));
     VF_CUDA(cudaMemcpyAsync(out_pairs, h->bufB, size_t(v.rows()) * 2 * ctot * sizeof(__half), cudaMemcpyDeviceToDevice, s));
-    return i3d_leave(h, user);
+    return leave(h, user);
 }
 
 int64_t vf_i3d_launch_count(const vf_i3d_t* h) { return h ? h->launches : 0; }

@@ -5,7 +5,12 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include <array>
+#include <functional>
+#include <map>
 #include <string>
+#include <vector>
 
 #include "../../include/vfeat.h"
 
@@ -27,6 +32,52 @@ int fail(int code, const char* fmt, ...);
         int _s = (expr);              \
         if (_s != VF_OK) return _s;   \
     } while (0)
+
+// ---- the host side every engine handle shares: device check, allocations, engine stream, graph cache, destroy.
+// cudaSetDevice(device), then VF_ERR_UNSUPPORTED unless the device is sm_90 (the library is built for sm_90a only)
+int check_device(int device);
+bool graphs_enabled();   // false under VF_NO_GRAPH=1: every call runs eagerly
+
+// graph-cache key: (frames), (clips, T), (F, Hp, Wp) or (F, H, W, iters), unused slots zero
+using GraphKey = std::array<int, 4>;
+struct CachedGraph {
+    cudaGraphExec_t exec = nullptr;
+    int64_t launches = 0;     // kernel launches recorded during capture: what one replay adds to the count
+};
+
+struct EngineCore {
+    const char* who = "";                          // prefixes error messages ("resnet_create", ...)
+    int device = 0;
+    std::vector<void*> allocs;                     // freed by release()
+    int64_t launches = 0;                          // every kernel launch, eager or inside a replayed graph
+    cudaStream_t cs = nullptr;                     // engine stream (open_stream), ordered against the caller's
+    cudaEvent_t ev_in = nullptr, ev_out = nullptr; // stream by enter() / leave()
+    bool use_graph = graphs_enabled();
+    std::map<GraphKey, CachedGraph> graphs;        // run_graphed's cache
+};
+
+// cudaMalloc'd, zero-filled, + 64 KB: the overlapping-row TMA view of a conv input extends up to (k_per_tap - C)
+// elements past its last row; zero-filled so that those elements are finite (they only feed masked border rows)
+int engine_alloc(EngineCore* h, void** p, size_t bytes);
+template <typename Tp>
+int ralloc(EngineCore* h, Tp** p, size_t count) {
+    void* q = nullptr;
+    VF_TRY(engine_alloc(h, &q, count * sizeof(Tp)));
+    *p = static_cast<Tp*>(q);
+    return VF_OK;
+}
+int open_stream(EngineCore* h);                    // the engine stream and its ev_in / ev_out pair
+int enter(EngineCore* h, cudaStream_t user);       // the engine stream waits for the work queued on `user`
+int leave(EngineCore* h, cudaStream_t user);       // `user` waits for the work queued on the engine stream
+// waits for the device, frees every allocation and graph, destroys the stream and events (the handle is not deleted)
+void release(EngineCore* h);
+// captures run() on stream s into an instantiated graph; h->launches is left as it was, g->launches gets what run()
+// counted
+int capture_graph(EngineCore* h, cudaStream_t s, const std::function<int()>& run, CachedGraph* g);
+// run() on the engine stream through the graph cache: eager under VF_NO_GRAPH=1 or GEMM profiling (event-bracketed
+// launches cannot be captured); otherwise the key's graph is captured on first use and replayed.  At most 16 graphs
+// are kept, the smallest key is evicted first.
+int run_graphed(EngineCore* h, const GraphKey& key, const std::function<int()>& run);
 
 // ---- tensor maps (driver entry point fetched at run time; the library does not link libcuda).
 // 2-D row-major tensor of 2- or 4-byte elements, 128-byte-swizzled boxes of box_rows x (128 / elem_bytes) columns.

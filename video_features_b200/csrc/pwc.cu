@@ -23,9 +23,7 @@
 
 #include <algorithm>
 #include <functional>
-#include <map>
 #include <string>
-#include <tuple>
 #include <vector>
 
 #include "internal.h"
@@ -122,9 +120,8 @@ Vol2 cat_vol(int l, int n, int Hp, int Wp) {
 
 using namespace vf;
 
-struct vf_pwc {
-    int device = 0, max_frames = 0, max_hp = 0, max_wp = 0;
-    std::vector<void*> allocs;
+struct vf_pwc : vf::EngineCore {
+    int max_frames = 0, max_hp = 0, max_wp = 0;
     PConv ext[7][3];                  // extractor level 1..6, convs .0 .2 .4
     PConv upflow[7], upfeat[7];       // decoder levels 2..5
     PConv dec[7][6];                  // decoder levels 2..6, moduleOne .. moduleSix
@@ -132,27 +129,12 @@ struct vf_pwc {
     __half *in0 = nullptr, *ph = nullptr, *tA = nullptr, *tB = nullptr, *rA = nullptr, *rB = nullptr;
     __half *feat[7] = {}, *cat[7] = {}, *flow[7] = {};
     float *upA = nullptr, *upB = nullptr, *f2w = nullptr, *refine = nullptr, *mask[7] = {};
-    int64_t launches = 0;
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    bool use_graph = true;
-    std::map<std::tuple<int, int, int>, std::pair<cudaGraphExec_t, int64_t>> graphs;
     int last_F = 0, last_hp = 0, last_wp = 0;     // geometry of the last call (debug reads)
 };
 
 namespace vf {
 
 namespace {
-
-template <typename Tp>
-int palloc(vf_pwc* h, Tp** p, size_t count) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(Tp) + 65536);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "cudaMalloc(%zu bytes): %s", count * sizeof(Tp), cudaGetErrorString(e));
-    h->allocs.push_back(q);
-    *p = static_cast<Tp*>(q);
-    return VF_OK;
-}
 
 struct TensorTable {
     const vf_named_tensor* t; int n;
@@ -202,9 +184,9 @@ int upload(vf_pwc* h, PConv& cw, const HostConv& hc) {
                     if (hc.hi[size_t(t) * hc.kpt + j]) m &= ~(1ull << kk);
         cw.lo_mask = blocks == 64 ? m : (m & ((1ull << blocks) - 1));
     }
-    VF_TRY(palloc(h, &cw.w, B.size()));
-    VF_TRY(palloc(h, &cw.scale, size_t(hc.n_out)));
-    VF_TRY(palloc(h, &cw.bias, size_t(hc.n_out)));
+    VF_TRY(ralloc(h, &cw.w, B.size()));
+    VF_TRY(ralloc(h, &cw.scale, size_t(hc.n_out)));
+    VF_TRY(ralloc(h, &cw.bias, size_t(hc.n_out)));
     VF_CUDA(cudaMemcpy(cw.w, B.data(), B.size() * sizeof(__half), cudaMemcpyHostToDevice));
     VF_CUDA(cudaMemcpy(cw.scale, sc.data(), sc.size() * sizeof(float), cudaMemcpyHostToDevice));
     VF_CUDA(cudaMemcpy(cw.bias, bi.data(), bi.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -435,13 +417,9 @@ int vf_pwc_create(vf_pwc_t** out, const vf_named_tensor* tensors, int n_tensors,
     *out = nullptr;
     if (max_frames < 2) max_frames = 2;
     if (max_h <= 0 || max_w <= 0) return fail(VF_ERR_INVALID, "pwc_create: max frame size required");
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_pwc* h = new vf_pwc();
+    h->who = "pwc_create";
     h->device = device; h->max_frames = max_frames;
     h->max_hp = (max_h + 63) / 64 * 64; h->max_wp = (max_w + 63) / 64 * 64;
     const TensorTable T{tensors, n_tensors};
@@ -449,37 +427,31 @@ int vf_pwc_create(vf_pwc_t** out, const vf_named_tensor* tensors, int n_tensors,
         VF_TRY(prep_all(h, T));
         const size_t F = size_t(max_frames), NP = F - 1;
         const int Hp = h->max_hp, Wp = h->max_wp;
-        VF_TRY(palloc(h, &h->in0, F * (Hp + 2) * (Wp + 2) * 16));
+        VF_TRY(ralloc(h, &h->in0, F * (Hp + 2) * (Wp + 2) * 16));
         size_t ph = 0, tmp = 0, up = 0, f2w = 0;
         for (int l = 1; l <= 6; ++l) {
             const size_t rows = size_t(feat_vol(l, int(F), Hp, Wp).rows());
             const int c8 = r8(kFeatC[l]), p8 = l == 1 ? 8 : r8(kFeatC[l - 1]);
             ph = std::max(ph, rows * 8 * p8);
             tmp = std::max(tmp, rows * 2 * c8);
-            VF_TRY(palloc(h, &h->feat[l], rows * 2 * c8));
+            VF_TRY(ralloc(h, &h->feat[l], rows * 2 * c8));
             if (l >= 2) {
                 const size_t crows = size_t(cat_vol(l, int(NP), Hp, Wp).rows());
-                VF_TRY(palloc(h, &h->cat[l], crows * layout(l).total));
-                VF_TRY(palloc(h, &h->flow[l], crows * 16));
-                VF_CUDA(cudaMemset(h->flow[l], 0, crows * 16 * sizeof(__half)));
+                VF_TRY(ralloc(h, &h->cat[l], crows * layout(l).total));
+                VF_TRY(ralloc(h, &h->flow[l], crows * 16));
                 if (l >= 3) up = std::max(up, crows * 8);
-                if (l < 6) VF_TRY(palloc(h, &h->mask[l], NP * size_t(Hp >> l) * (Wp >> l)));
+                if (l < 6) VF_TRY(ralloc(h, &h->mask[l], NP * size_t(Hp >> l) * (Wp >> l)));
                 f2w = std::max(f2w, NP * size_t((Hp >> l) + 8) * ((Wp >> l) + 8) * kFeatC[l]);
             }
         }
-        VF_TRY(palloc(h, &h->ph, ph));
-        VF_TRY(palloc(h, &h->tA, tmp)); VF_TRY(palloc(h, &h->tB, tmp));
-        VF_TRY(palloc(h, &h->upA, up)); VF_TRY(palloc(h, &h->upB, up));
-        VF_TRY(palloc(h, &h->f2w, f2w));
+        VF_TRY(ralloc(h, &h->ph, ph));
+        VF_TRY(ralloc(h, &h->tA, tmp)); VF_TRY(ralloc(h, &h->tB, tmp));
+        VF_TRY(ralloc(h, &h->upA, up)); VF_TRY(ralloc(h, &h->upB, up));
+        VF_TRY(ralloc(h, &h->f2w, f2w));
         const size_t rows2 = size_t(cat_vol(2, int(NP), Hp, Wp).rows());
-        VF_TRY(palloc(h, &h->rA, rows2 * 256)); VF_TRY(palloc(h, &h->rB, rows2 * 256));
-        VF_TRY(palloc(h, &h->refine, rows2 * 8));
-        VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-        const char* e = getenv("VF_NO_GRAPH");
-        h->use_graph = !(e && e[0] == '1');
-        return VF_OK;
+        VF_TRY(ralloc(h, &h->rA, rows2 * 256)); VF_TRY(ralloc(h, &h->rB, rows2 * 256));
+        VF_TRY(ralloc(h, &h->refine, rows2 * 8));
+        return open_stream(h);
     };
     const int st = body();
     if (st != VF_OK) { vf_pwc_destroy(h); return st; }
@@ -489,13 +461,7 @@ int vf_pwc_create(vf_pwc_t** out, const vf_named_tensor* tensors, int n_tensors,
 
 int vf_pwc_destroy(vf_pwc_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
-    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second.first);
-    if (h->cs) cudaStreamDestroy(h->cs);
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
-    if (h->ev_out) cudaEventDestroy(h->ev_out);
+    release(h);
     delete h;
     return VF_OK;
 }
@@ -511,46 +477,14 @@ int vf_pwc_flow(vf_pwc_t* h, const void* frames, int is_u8, int chw_layout, int 
         return fail(VF_ERR_INVALID, "pwc_flow: frame %dx%d outside the workspace (%dx%d)", Hs, Ws, h->max_hp, h->max_wp);
     const int F = n_frames, NP = F - 1;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_CUDA(cudaSetDevice(h->device));
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     VF_TRY(pwc_input_pack(frames, is_u8, chw_layout, F, Hs, Ws, h->in0, Vol2{F, Hp + 2, Wp + 2, 1, 1 + Hp, 1, 1 + Wp}, s));
     h->launches += 1;
-    if (!h->use_graph || gemm_profile_on()) {
-        VF_TRY(pwc_core(h, F, Hp, Wp, s));
-    } else {
-        auto key = std::make_tuple(F, Hp, Wp);
-        auto it = h->graphs.find(key);
-        if (it == h->graphs.end()) {
-            const int64_t before = h->launches;
-            cudaGraph_t graph = nullptr;
-            VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-            const int st = pwc_core(h, F, Hp, Wp, s);
-            const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-            const int64_t n_launch = h->launches - before;
-            h->launches = before;
-            if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-            if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-            cudaGraphExec_t exec = nullptr;
-            const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-            cudaGraphDestroy(graph);
-            if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-            // bounded cache, as RAFT's: an evicted graph that is still running is freed by the runtime when it completes
-            if (h->graphs.size() >= 16) {
-                cudaGraphExecDestroy(h->graphs.begin()->second.first);
-                h->graphs.erase(h->graphs.begin());
-            }
-            it = h->graphs.emplace(key, std::make_pair(exec, n_launch)).first;
-        }
-        VF_CUDA(cudaGraphLaunch(it->second.first, s));
-        h->launches += it->second.second;
-    }
+    VF_TRY(run_graphed(h, {F, Hp, Wp, 0}, [&] { return pwc_core(h, F, Hp, Wp, s); }));
     h->last_F = F; h->last_hp = Hp; h->last_wp = Wp;
     VF_TRY(pwc_output(h->flow[2], h->refine, cat_vol(2, NP, Hp, Wp), NP, Hs, Ws, Hp, Wp, out, s));
     h->launches += 1;
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
-    return VF_OK;
+    return leave(h, user);
 }
 
 int vf_pwc_debug_read(vf_pwc_t* h, int what, int level, float* out, int64_t capacity, int* dims4, void* stream) {

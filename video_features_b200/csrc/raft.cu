@@ -22,9 +22,7 @@
 #include <string.h>
 
 #include <functional>
-#include <map>
 #include <string>
-#include <tuple>
 #include <vector>
 
 #include "internal.h"
@@ -49,11 +47,10 @@ static const int CF = RAFT_CF;    // correlation-feature rows: raft_kernels.h
 
 using namespace vf;
 
-struct vf_raft {
-    int device = 0, max_frames = 0, max_h = 0, max_w = 0;
+struct vf_raft : vf::EngineCore {
+    int max_frames = 0, max_h = 0, max_w = 0;
     int lead_alloc = 0;         // guard rows in front of every update-block buffer (pointers below are past them)
     int wsplit = 2;             // weights as hi+lo fp16 pairs (VF_RAFT_FAST=1: single fp16 weights, outside the parity bar)
-    std::vector<void*> allocs;
     // encoders: [0] = fnet (instance norm), [1] = cnet (batch norm folded)
     struct Enc {
         ConvW conv1, l1[4], l2c1, l2down, l2[3], l3c1, l3down, l3[3], conv2;
@@ -70,30 +67,12 @@ struct vf_raft {
     float *h32 = nullptr, *zr = nullptr, *qb = nullptr;   // fp32 GRU state and gates
     __half *corrfeat = nullptr, *c1 = nullptr, *c2f = nullptr, *f1 = nullptr, *flow8 = nullptr, *hx = nullptr, *qx = nullptr,
            *fh = nullptr, *mk = nullptr;
-    int64_t launches = 0;
-    // engine-owned stream; everything between the input pack and the convex upsample is replayed as one CUDA graph per
-    // (frames, H, W, iterations): ~600-1000 launches and ~1000 tensor-map encodes per window otherwise
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    bool use_graph = true;
-    std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, int64_t>> graphs;
     // geometry of the last call (for debug reads)
     int last_n = 0, last_H8 = 0, last_W8 = 0, corr_ld = 0, P8 = 0;
     Vol2 g8e{}, g8u{};
 };
 
 namespace vf {
-
-template <typename Tp>
-static int ralloc(vf_raft* h, Tp** p, size_t count) {
-    // + 64 KB: the overlapping-row TMA view of a conv input extends (kw-1)*pitch elements past its last row
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(Tp) + 65536);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "cudaMalloc(%zu bytes): %s", count * sizeof(Tp), cudaGetErrorString(e));
-    h->allocs.push_back(q);
-    *p = static_cast<Tp*>(q);
-    return VF_OK;
-}
 
 struct TensorTable {
     const vf_named_tensor* t; int n;
@@ -398,13 +377,9 @@ int vf_raft_create(vf_raft_t** out, const vf_named_tensor* tensors, int n_tensor
     *out = nullptr;
     if (max_frames < 2) max_frames = 2;
     if (max_h <= 0 || max_w <= 0) return fail(VF_ERR_INVALID, "raft_create: max frame size required");
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_raft* h = new vf_raft();
+    h->who = "raft_create";
     h->device = device; h->max_frames = max_frames;
     h->max_h = (max_h + 7) / 8 * 8; h->max_w = (max_w + 7) / 8 * 8;
     const TensorTable T{tensors, n_tensors};
@@ -482,10 +457,7 @@ int vf_raft_create(vf_raft_t** out, const vf_named_tensor* tensors, int n_tensor
         VF_TRY(ralloc(h, &h->cnet32, rows8e * 256));
         const size_t P = size_t(H / 8) * (W / 8), P8 = (P + 7) / 8 * 8;
         VF_TRY(ralloc(h, &h->corrA, F * P8 * 768));
-        VF_TRY(ralloc(h, &h->corrB, F * P8 * 768));
-        // rows P .. P8-1 of a frame are never written: they must hold finite values (they only feed unread corr columns)
-        VF_CUDA(cudaMemset(h->corrA, 0, F * P8 * 768 * sizeof(__half)));
-        VF_CUDA(cudaMemset(h->corrB, 0, F * P8 * 768 * sizeof(__half)));
+        VF_TRY(ralloc(h, &h->corrB, F * P8 * 768));      // rows P .. P8-1 of a frame stay zero: finite, unread columns
         VF_TRY(ralloc(h, &h->st_a, F * 128 * 2)); VF_TRY(ralloc(h, &h->st_b, F * 128 * 2));
         const size_t ld = (P8 + P / 4 + P / 16 + P / 64 + 64 + 3) / 4 * 4;
         VF_TRY(ralloc(h, &h->corr, NP * P * ld));
@@ -493,9 +465,7 @@ int vf_raft_create(vf_raft_t** out, const vf_named_tensor* tensors, int n_tensor
         // update-block volumes: `lead` zeroed guard rows in front of the first sample (run_conv's row0), see raft_core
         h->lead_alloc = 3 * (W / 8 + 3) + 3;
         auto ualloc = [&](auto** p, size_t ld) -> int {
-            const size_t count = (size_t(h->lead_alloc) + rows8u + 8) * ld;
-            VF_TRY(ralloc(h, p, count));
-            VF_CUDA(cudaMemset(*p, 0, count * sizeof(**p)));
+            VF_TRY(ralloc(h, p, (size_t(h->lead_alloc) + rows8u + 8) * ld));
             *p += size_t(h->lead_alloc) * ld;
             return VF_OK;
         };
@@ -507,14 +477,7 @@ int vf_raft_create(vf_raft_t** out, const vf_named_tensor* tensors, int n_tensor
         VF_TRY(ualloc(&h->h32, 128));
         VF_TRY(ualloc(&h->mk, 256));
         VF_TRY(ualloc(&h->delta, 8));     VF_TRY(ualloc(&h->mask, 576));
-        VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-        {
-            const char* e = getenv("VF_NO_GRAPH");
-            h->use_graph = !(e && e[0] == '1');
-        }
-        return VF_OK;
+        return open_stream(h);
     };
     const int st = body();
     if (st != VF_OK) { vf_raft_destroy(h); return st; }
@@ -524,13 +487,7 @@ int vf_raft_create(vf_raft_t** out, const vf_named_tensor* tensors, int n_tensor
 
 int vf_raft_destroy(vf_raft_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
-    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second.first);
-    if (h->cs) cudaStreamDestroy(h->cs);
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
-    if (h->ev_out) cudaEventDestroy(h->ev_out);
+    release(h);
     delete h;
     return VF_OK;
 }
@@ -541,6 +498,17 @@ namespace vf {
 
 // geometry of the update-block volumes (see raft_core)
 static Vol2 update_vol(int NP, int H8, int W8) { return Vol2{NP, H8 + 3, W8 + 3, 0, H8, 0, W8}; }
+
+// the geometry of a call of F frames of H x W that the upsampling and the debug reads use
+static void set_geometry(vf_raft* h, int F, int H, int W) {
+    const int NP = F - 1, H8 = H / 8, W8 = W / 8, P = H8 * W8;
+    h->last_n = NP; h->last_H8 = H8; h->last_W8 = W8; h->P8 = (P + 7) / 8 * 8;
+    int ldc = h->P8, lh = H8, lw = W8;
+    for (int l = 1; l < 4; ++l) { lh /= 2; lw /= 2; ldc += lh * lw; }
+    h->corr_ld = (ldc + 3) / 4 * 4;
+    h->g8e = Vol2{NP, H8 + 2, W8 + 2, 1, 1 + H8, 1, 1 + W8};
+    h->g8u = update_vol(NP, H8, W8);
+}
 
 // encoders -> correlation pyramid -> `iters` refinement steps -> mask head; the stem phase volume is already in h->s0
 static int raft_core(vf_raft* h, int F, int H, int W, int iters, cudaStream_t s) {
@@ -608,7 +576,6 @@ static int raft_core(vf_raft* h, int F, int H, int W, int iters, cudaStream_t s)
     // ---- mask head (once, after the last iteration)
     VF_TRY(run_conv(h, h->mk0, h->hx, HX, g8u, h->mk, 256, 0, VF_ACT_RELU, s, 0, lead));
     VF_TRY(run_conv(h, h->mk2, h->mk, 256, g8u, h->mask, 576, 1, VF_ACT_NONE, s, 0, lead));
-    h->last_n = NP; h->last_H8 = H8; h->last_W8 = W8; h->corr_ld = ldc; h->P8 = P8; h->g8e = g8e; h->g8u = g8u;
     return VF_OK;
 }
 
@@ -631,59 +598,20 @@ int vf_raft_flow(vf_raft_t* h, const void* frames, int is_u8, int chw_layout, in
     // avg_pool2d raises there); from 64 to 127 px that level is 1 pixel wide, which the lookup samples correctly
     if (H < 64 || W < 64)
         return fail(VF_ERR_INVALID, "raft_flow: padded frame %dx%d is under 64 px: the 4th correlation level would be empty", H, W);
-    const int F = n_frames, NP = F - 1, H8 = H / 8, W8 = W / 8, P = H8 * W8;
+    const int F = n_frames, NP = F - 1, H8 = H / 8, W8 = W / 8;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_CUDA(cudaSetDevice(h->device));
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     VF_TRY(raft_input_pack(frames, is_u8, chw_layout, F, Hs, Ws, pt, pl, H, W, h->s0, H / 2 + 3, W / 2 + 3, s));
     h->launches += 1;
-    if (!h->use_graph || gemm_profile_on()) {
-        VF_TRY(raft_core(h, F, H, W, iters, s));
-    } else {
-        auto key = std::make_tuple(F, H, W, iters);
-        auto it = h->graphs.find(key);
-        if (it == h->graphs.end()) {
-            const int64_t before = h->launches;
-            cudaGraph_t graph = nullptr;
-            VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-            const int st = raft_core(h, F, H, W, iters, s);
-            const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-            const int64_t n_launch = h->launches - before;
-            h->launches = before;
-            if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-            if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-            cudaGraphExec_t exec = nullptr;
-            const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-            cudaGraphDestroy(graph);
-            if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-            // bounded cache: a list of videos of many resolutions (or ragged last calls) must not pile up executable
-            // graphs; an evicted graph that is still running is freed by the runtime when it completes
-            if (h->graphs.size() >= 16) {
-                cudaGraphExecDestroy(h->graphs.begin()->second.first);
-                h->graphs.erase(h->graphs.begin());
-            }
-            it = h->graphs.emplace(key, std::make_pair(exec, n_launch)).first;
-        }
-        VF_CUDA(cudaGraphLaunch(it->second.first, s));
-        h->launches += it->second.second;
-        // geometry bookkeeping normally done inside raft_core
-        h->last_n = NP; h->last_H8 = H8; h->last_W8 = W8;
-        {
-            int ldc = (P + 7) / 8 * 8, lh = H8, lw = W8;
-            for (int l = 1; l < 4; ++l) { lh /= 2; lw /= 2; ldc += lh * lw; }
-            h->corr_ld = (ldc + 3) / 4 * 4;
-        }
-        h->g8e = Vol2{NP, H8 + 2, W8 + 2, 1, 1 + H8, 1, 1 + W8};
-        h->g8u = update_vol(NP, H8, W8);
-    }
+    // everything between the input pack and the convex upsample is replayed as one CUDA graph per (frames, H, W,
+    // iterations): ~600-1000 launches and ~1000 tensor-map encodes per window otherwise
+    VF_TRY(run_graphed(h, {F, H, W, iters}, [&] { return raft_core(h, F, H, W, iters, s); }));
+    set_geometry(h, F, H, W);
     // ---- convex upsampling, once
     if (unpad) VF_TRY(raft_upsample_flow(h->coords1, h->mask, h->g8u, NP, H8, W8, pt, pl, Hs, Ws, out, s));
     else       VF_TRY(raft_upsample_flow(h->coords1, h->mask, h->g8u, NP, H8, W8, 0, 0, H, W, out, s));
     h->launches += 1;
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
-    return VF_OK;
+    return leave(h, user);
 }
 
 int vf_raft_padded_size(int Hs, int Ws, int* H, int* W) {

@@ -22,7 +22,6 @@
 
 #include <algorithm>
 #include <functional>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -42,8 +41,8 @@ struct ResBlock {
 
 using namespace vf;
 
-struct vf_resnet : vf::ConvHost {
-    int device = 0, depth = 0, max_frames = 0, out_dim = 0;
+struct vf_resnet : vf::EngineCore {
+    int depth = 0, max_frames = 0, out_dim = 0;
     bool bottleneck = false;
     int nblocks[4] = {0, 0, 0, 0}, cout[4] = {0, 0, 0, 0};
     ResConv stem;
@@ -51,10 +50,6 @@ struct vf_resnet : vf::ConvHost {
     // workspace: s0 = stem phase volume; stage outputs are kept for vf_resnet_read_stage
     __half *s0 = nullptr, *stem_out = nullptr, *pool_out = nullptr, *stage_out[4] = {nullptr, nullptr, nullptr, nullptr};
     __half *bufA = nullptr, *bufB = nullptr, *t1 = nullptr, *t2 = nullptr, *ds = nullptr, *ph1 = nullptr, *ph2 = nullptr;
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    bool use_graph = true;
-    std::map<int, std::pair<cudaGraphExec_t, int64_t>> graphs;     // frames -> (trunk graph, launches in it)
     int last_n = 0;
 };
 
@@ -66,16 +61,7 @@ static const int kSide[4] = {56, 28, 14, 7};
 static Vol2 stem_vol(int n) { return Vol2{n, kStemQ, kStemQ, 2, 114, 2, 114}; }
 static Vol2 stage_vol(int n, int L) { return Vol2{n, kSide[L] + 2, kSide[L] + 2, 1, kSide[L] + 1, 1, kSide[L] + 1}; }
 
-// stem 7x7/2 pad 3 on the phase volume of the transform (rows [16 hi | 16 lo], 4 channels per phase, 3 used):
-// phase row q holds x[2(q-2)+p]; 4 taps (kernel row pairs), each a run of 4 phase positions x 32 elements.
-static int prep_stem(vf_resnet* h, ResConv& cw, const ResTensors& T) {
-    cw.ntaps = 4; cw.k_per_tap = 128;
-    for (int a = 0; a < 4; ++a) { cw.dh[a] = a - 2; cw.dw[a] = -2; }
-    return upload_conv(h, cw, T, "conv1", "bn1", 64, 3, 7, 16, [](int kh, int kw, int c) {
-        const int a = (kh + 1) / 2, ph = (kh + 1) % 2, b = (kw + 1) / 2, pw = (kw + 1) % 2;
-        return a * 128 + b * 32 + (ph * 2 + pw) * 4 + c;
-    });
-}
+static const double kEps = 1e-5;                                // torchvision BatchNorm2d
 
 // torchvision BasicBlock / Bottleneck (v1.5: the stride sits on the 3x3): x (valid region vi, cin channels) ->
 // dst (vo, cout channels)
@@ -159,18 +145,13 @@ int vf_resnet_create(vf_resnet_t** out, const vf_named_tensor* tensors, int n_te
         default: return fail(VF_ERR_INVALID, "resnet_create: depth %d is not one of 18, 34, 50, 101, 152", depth);
     }
     if (max_frames <= 0) max_frames = 64;
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_resnet* h = new vf_resnet();
     h->who = "resnet_create";
     h->device = device; h->depth = depth; h->max_frames = max_frames; h->bottleneck = bottleneck;
     const ResTensors T{tensors, n_tensors, "resnet_create"};
     auto body = [&]() -> int {
-        VF_TRY(prep_stem(h, h->stem, T));
+        VF_TRY(prep_stem(h, h->stem, T, "conv1", "bn1", kEps, 64));
         // per-frame element counts of the working buffers, found while walking the blocks
         size_t e_act = 0, e_ph = 0;
         auto rows = [](const Vol2& v) { return size_t(v.rows()); };
@@ -187,18 +168,18 @@ int vf_resnet_create(vf_resnet_t** out, const vf_named_tensor* tensors, int n_te
                 const Vol2 vi = B.stride == 2 ? stage_vol(1, L - 1) : vo;
                 const std::string p = "layer" + std::to_string(L + 1) + "." + std::to_string(b);
                 if (!bottleneck) {
-                    if (B.stride == 2) VF_TRY(prep_stride2(h, B.c1, T, p + ".conv1", p + ".bn1", width, B.cin));
-                    else               VF_TRY(prep_same(h, B.c1, T, p + ".conv1", p + ".bn1", width, B.cin, 3));
-                    VF_TRY(prep_same(h, B.c2, T, p + ".conv2", p + ".bn2", width, width, 3));
+                    if (B.stride == 2) VF_TRY(prep_stride2(h, B.c1, T, p + ".conv1", p + ".bn1", kEps, width, B.cin));
+                    else               VF_TRY(prep_same(h, B.c1, T, p + ".conv1", p + ".bn1", kEps, width, B.cin, 3));
+                    VF_TRY(prep_same(h, B.c2, T, p + ".conv2", p + ".bn2", kEps, width, width, 3));
                 } else {
-                    VF_TRY(prep_same(h, B.c1, T, p + ".conv1", p + ".bn1", width, B.cin, 1));
-                    if (B.stride == 2) VF_TRY(prep_stride2(h, B.c2, T, p + ".conv2", p + ".bn2", width, width));
-                    else               VF_TRY(prep_same(h, B.c2, T, p + ".conv2", p + ".bn2", width, width, 3));
-                    VF_TRY(prep_same(h, B.c3, T, p + ".conv3", p + ".bn3", cout, width, 1));
+                    VF_TRY(prep_same(h, B.c1, T, p + ".conv1", p + ".bn1", kEps, width, B.cin, 1));
+                    if (B.stride == 2) VF_TRY(prep_stride2(h, B.c2, T, p + ".conv2", p + ".bn2", kEps, width, width));
+                    else               VF_TRY(prep_same(h, B.c2, T, p + ".conv2", p + ".bn2", kEps, width, width, 3));
+                    VF_TRY(prep_same(h, B.c3, T, p + ".conv3", p + ".bn3", kEps, cout, width, 1));
                     e_act = std::max(e_act, rows(vi) * 2 * width);                  // c1 output at the input geometry
                     if (B.stride == 2) e_ph = std::max(e_ph, rows(vo) * 8 * width);
                 }
-                if (B.down) VF_TRY(prep_same(h, B.dn, T, p + ".downsample.0", p + ".downsample.1", cout, B.cin, 1));
+                if (B.down) VF_TRY(prep_same(h, B.dn, T, p + ".downsample.0", p + ".downsample.1", kEps, cout, B.cin, 1));
                 if (B.stride == 2) e_ph = std::max(e_ph, rows(vo) * 8 * B.cin);
                 e_act = std::max(e_act, rows(vo) * 2 * std::max(width, cout));
                 h->blocks.push_back(B);
@@ -214,12 +195,7 @@ int vf_resnet_create(vf_resnet_t** out, const vf_named_tensor* tensors, int n_te
         for (__half** b : {&h->bufA, &h->bufB, &h->t1, &h->t2, &h->ds}) VF_TRY(ralloc(h, b, F * e_act));
         VF_TRY(ralloc(h, &h->ph1, F * std::max<size_t>(e_ph, 8)));
         VF_TRY(ralloc(h, &h->ph2, F * std::max<size_t>(e_ph, 8)));
-        VF_CUDA(cudaStreamCreateWithFlags(&h->cs, cudaStreamNonBlocking));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-        const char* e = getenv("VF_NO_GRAPH");
-        h->use_graph = !(e && e[0] == '1');
-        return VF_OK;
+        return open_stream(h);
     };
     const int st = body();
     if (st != VF_OK) { vf_resnet_destroy(h); return st; }
@@ -229,13 +205,7 @@ int vf_resnet_create(vf_resnet_t** out, const vf_named_tensor* tensors, int n_te
 
 int vf_resnet_destroy(vf_resnet_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
-    for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second.first);
-    if (h->cs) cudaStreamDestroy(h->cs);
-    if (h->ev_in) cudaEventDestroy(h->ev_in);
-    if (h->ev_out) cudaEventDestroy(h->ev_out);
+    release(h);
     delete h;
     return VF_OK;
 }
@@ -243,35 +213,6 @@ int vf_resnet_destroy(vf_resnet_t* h) {
 }  // extern "C"
 
 namespace vf {
-
-static int trunk_graph(vf_resnet* h, int m, cudaStream_t s) {
-    if (!h->use_graph || gemm_profile_on()) return run_trunk(h, m, s);
-    auto it = h->graphs.find(m);
-    if (it == h->graphs.end()) {
-        const int64_t before = h->launches;
-        cudaGraph_t graph = nullptr;
-        VF_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed));
-        const int st = run_trunk(h, m, s);
-        const cudaError_t ce = cudaStreamEndCapture(s, &graph);
-        const int64_t n_launch = h->launches - before;
-        h->launches = before;
-        if (st != VF_OK) { if (graph) cudaGraphDestroy(graph); return st; }
-        if (ce != cudaSuccess) return fail(VF_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(ce));
-        cudaGraphExec_t exec = nullptr;
-        const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) return fail(VF_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie));
-        // bounded cache: ragged last chunks of many videos must not pile up executable graphs
-        if (h->graphs.size() >= 16) {
-            cudaGraphExecDestroy(h->graphs.begin()->second.first);
-            h->graphs.erase(h->graphs.begin());
-        }
-        it = h->graphs.emplace(m, std::make_pair(exec, n_launch)).first;
-    }
-    VF_CUDA(cudaGraphLaunch(it->second.first, s));
-    h->launches += it->second.second;
-    return VF_OK;
-}
 
 static int resnet_forward(vf_resnet* h, const void* frames, int is_u8, int n, int Hr, int Wr, float* out, void* stream) {
     if (!h || !frames || !out) return fail(VF_ERR_INVALID, "resnet_forward: null argument");
@@ -282,22 +223,18 @@ static int resnet_forward(vf_resnet* h, const void* frames, int is_u8, int n, in
     const int cy = is_u8 ? center_crop_offset(Hr, 224) : 0, cx = is_u8 ? center_crop_offset(Wr, 224) : 0;
     const size_t frame_elems = is_u8 ? size_t(Hr) * Wr * 3 : size_t(3) * 224 * 224;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_CUDA(cudaSetDevice(h->device));
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    VF_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+    VF_TRY(enter(h, user));
     for (int off = 0; off < n; off += h->max_frames) {      // calls beyond the workspace run in chunks
         const int m = std::min(h->max_frames, n - off);
         const void* src = is_u8 ? static_cast<const void*>(static_cast<const uint8_t*>(frames) + off * frame_elems)
                                 : static_cast<const void*>(static_cast<const float*>(frames) + off * frame_elems);
         VF_TRY(resnet_input_pack(src, is_u8, m, Hr, Wr, cy, cx, h->s0, s));
-        VF_TRY(trunk_graph(h, m, s));
+        VF_TRY(run_graphed(h, {m, 0, 0, 0}, [&] { return run_trunk(h, m, s); }));
         VF_TRY(resnet_avgpool(h->stage_out[3], stage_vol(m, 3), h->out_dim, out + size_t(off) * h->out_dim, s));
         h->launches += 2;
         h->last_n = m;
     }
-    VF_CUDA(cudaEventRecord(h->ev_out, s));
-    VF_CUDA(cudaStreamWaitEvent(user, h->ev_out, 0));
-    return VF_OK;
+    return leave(h, user);
 }
 
 }  // namespace vf

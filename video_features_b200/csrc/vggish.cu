@@ -34,8 +34,8 @@ static const int kConvOut[6] = {64, 128, 256, 256, 512, 512};
 
 using namespace vf;
 
-struct vf_vggish : vf::ConvHost {
-    int device = 0, max_examples = 0, num_table = 0, nwin = 0, rate = 0;
+struct vf_vggish : vf::EngineCore {
+    int max_examples = 0, num_table = 0, nwin = 0, rate = 0;
     std::vector<double> base_win;                  // the unscaled filter table
     ResConv conv[6], fc[3];
     double *win = nullptr, *delta = nullptr, *hann = nullptr, *twiddle = nullptr, *mel = nullptr, *wave = nullptr;
@@ -59,7 +59,8 @@ static int prep_conv3(vf_vggish* h, ResConv& cw, const float* w, const float* bi
     for (int a = 0; a < 3; ++a) { cw.dh[a] = a - 1; cw.dw[a] = -1; }
     const int kpt = cw.k_per_tap;
     const std::vector<float> sc(size_t(co), 1.f), sh(bias, bias + co);
-    return upload_weights(h, cw, w, co, ci, 3, ci, [=](int a, int d, int c) { return a * kpt + d * 2 * ci + c; }, sc, sh);
+    return upload_weights(h, cw, w, {co, ci, 1, 3, 3}, ci, [=](int, int a, int d, int c) { return a * kpt + d * 2 * ci + c; },
+                          sc, sh);
 }
 
 // one-tap GEMM over M rows of X (pitch elements) + bias + ReLU -> split rows of 2*n_out, or fp32 rows of n_out
@@ -119,9 +120,7 @@ extern "C" {
 
 int vf_vggish_destroy(vf_vggish_t* h) {
     if (!h) return VF_OK;
-    cudaSetDevice(h->device);
-    cudaDeviceSynchronize();
-    for (void* p : h->allocs) cudaFree(p);
+    release(h);
     delete h;
     return VF_OK;
 }
@@ -134,12 +133,7 @@ int vf_vggish_create(vf_vggish_t** out, const vf_named_tensor* tensors, int n_te
     if (n_win < 2 || num_table <= 0) return fail(VF_ERR_INVALID, "vggish_create: bad filter table (%d entries)", n_win);
     *out = nullptr;
     if (max_examples <= 0) max_examples = 64;
-    VF_CUDA(cudaSetDevice(device));
-    int major = 0, minor = 0;
-    VF_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    VF_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 9 || minor != 0)
-        return fail(VF_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only", device, major, minor);
+    VF_TRY(check_device(device));
     vf_vggish* h = new vf_vggish();
     h->who = "vggish_create";
     h->device = device; h->max_examples = max_examples; h->num_table = num_table; h->nwin = n_win;
@@ -156,7 +150,7 @@ int vf_vggish_create(vf_vggish_t** out, const vf_named_tensor* tensors, int n_te
                 ResConv& c = h->conv[0];
                 c.ntaps = 1; c.k_per_tap = 32;
                 const std::vector<float> sc(size_t(co), 1.f), sh(b, b + co);
-                VF_TRY(upload_weights(h, c, w, co, 1, 3, 16, [](int a, int d, int) { return a * 3 + d; }, sc, sh));
+                VF_TRY(upload_weights(h, c, w, {co, 1, 1, 3, 3}, 16, [](int, int a, int d, int) { return a * 3 + d; }, sc, sh));
             } else {
                 VF_TRY(prep_conv3(h, h->conv[i], w, b, co, ci));
             }
@@ -171,10 +165,11 @@ int vf_vggish_create(vf_vggish_t** out, const vf_named_tensor* tensors, int n_te
             c.ntaps = 1; c.k_per_tap = 2 * fin[i];
             const std::vector<float> sc(size_t(fout[i]), 1.f), sh(b, b + fout[i]);
             if (i == 0)               // input feature (h * 4 + w) * 512 + c sits in position block h * 4 + w of 1024
-                VF_TRY(upload_weights(h, c, w, fout[i], fin[i], 1, 512,
-                                      [](int, int, int c) { return (c / 512) * 1024 + c % 512; }, sc, sh));
+                VF_TRY(upload_weights(h, c, w, {fout[i], fin[i], 1, 1, 1}, 512,
+                                      [](int, int, int, int c) { return (c / 512) * 1024 + c % 512; }, sc, sh));
             else
-                VF_TRY(upload_weights(h, c, w, fout[i], fin[i], 1, fin[i], [](int, int, int c) { return c; }, sc, sh));
+                VF_TRY(upload_weights(h, c, w, {fout[i], fin[i], 1, 1, 1}, fin[i], [](int, int, int, int c) { return c; }, sc,
+                                      sh));
         }
         const size_t E = size_t(max_examples);
         VF_TRY(ralloc(h, &h->win, size_t(n_win)));

@@ -6,10 +6,9 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, Sequence
 
-import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib, read_conv
+from ._lib import check, lib, named_tensors, read_conv
 
 OUT_DIM = 512
 
@@ -27,18 +26,9 @@ class R21DEngine:
             raise RuntimeError("R21DEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         self.out_dim = OUT_DIM
-        keep = []
-        items = [(k, v) for k, v in state_dict.items() if torch.is_tensor(v) and v.dtype.is_floating_point]
-        arr = (NamedTensor * max(len(items), 1))()
-        for i, (k, v) in enumerate(items):
-            a = np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
-            nm = k.encode()
-            keep.append((a, nm))
-            arr[i].name = nm
-            arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
-            arr[i].numel = a.size
+        arr, n, keep = named_tensors(state_dict)
         h = C.c_void_p()
-        check(lib().vf_r21d_create2(C.byref(h), arr, len(items), device, max_clips, max_T, float(bn_eps)))
+        check(lib().vf_r21d_create2(C.byref(h), arr, n, device, max_clips, max_T, float(bn_eps)))
         self._h = h
         del keep
 

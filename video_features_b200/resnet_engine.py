@@ -5,10 +5,9 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict
 
-import numpy as np
 import torch
 
-from ._lib import NamedTensor, check, lib, read_conv
+from ._lib import check, lib, named_tensors, read_conv
 
 DEPTHS = (18, 34, 50, 101, 152)
 
@@ -23,18 +22,9 @@ class ResNetEngine:
         self.device = torch.device("cuda", device)
         self.depth = depth
         self.out_dim = 512 if depth in (18, 34) else 2048
-        keep = []
-        items = [(k, v) for k, v in state_dict.items() if torch.is_tensor(v) and v.dtype.is_floating_point]
-        arr = (NamedTensor * max(len(items), 1))()
-        for i, (k, v) in enumerate(items):
-            a = np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
-            nm = k.encode()
-            keep.append((a, nm))
-            arr[i].name = nm
-            arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
-            arr[i].numel = a.size
+        arr, n, keep = named_tensors(state_dict)
         h = C.c_void_p()
-        check(lib().vf_resnet_create(C.byref(h), arr, len(items), depth, device, max_frames))
+        check(lib().vf_resnet_create(C.byref(h), arr, n, depth, device, max_frames))
         self._h = h
         del keep
 

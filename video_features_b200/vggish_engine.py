@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import audio
-from ._lib import NamedTensor, check, lib, read_conv
+from ._lib import check, lib, named_tensors, read_conv
 
 KEYS = tuple(f"features.{i}.{p}" for i in (0, 3, 6, 8, 11, 13) for p in ("weight", "bias")) + \
     tuple(f"embeddings.{i}.{p}" for i in (0, 2, 4) for p in ("weight", "bias"))
@@ -27,22 +27,14 @@ class VGGishEngine:
             raise RuntimeError("VGGishEngine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         items = [(k[7:] if k.startswith("module.") else k, v) for k, v in state_dict.items()]
-        items = [(k, v) for k, v in items if k in KEYS and torch.is_tensor(v) and v.dtype.is_floating_point]
-        keep = []
-        arr = (NamedTensor * max(len(items), 1))()
-        for i, (k, v) in enumerate(items):
-            a = np.ascontiguousarray(v.detach().to("cpu", torch.float32).numpy())
-            nm = k.encode()
-            keep.append((a, nm))
-            arr[i].name = nm
-            arr[i].data = a.ctypes.data_as(C.POINTER(C.c_float))
-            arr[i].numel = a.size
+        items = [(k, v) for k, v in items if k in KEYS]
+        arr, n, keep = named_tensors(items)
         hann = np.ascontiguousarray(audio.periodic_hann())
         mel = np.ascontiguousarray(audio.mel_matrix())
         win, num_table = audio.kaiser_best()
         win = np.ascontiguousarray(win)
         h = C.c_void_p()
-        check(lib().vf_vggish_create(C.byref(h), arr, max(len(items), 1), hann.ctypes.data, mel.ctypes.data,
+        check(lib().vf_vggish_create(C.byref(h), arr, max(n, 1), hann.ctypes.data, mel.ctypes.data,
                                      win.ctypes.data, win.shape[0], num_table, device, max_examples))
         self._h = h
         del keep
