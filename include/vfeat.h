@@ -29,6 +29,8 @@ extern "C" {
 #define VF_ACT_SIGMOID 3
 #define VF_ACT_TANH 4
 #define VF_ACT_LEAKY 5     /* LeakyReLU(0.1): built for the conv mode with split weights (nsplit = 2) only */
+#define VF_ACT_GELU 6      /* exact GELU, 0.5 x (1 + erf(x / sqrt 2)): built for the plain GEMM (vf_gemm_f16) and the
+                              conv mode with split weights (nsplit = 2), without split output, only */
 
 #define VF_FILTER_BILINEAR 2 /* PIL.Image.BILINEAR */
 #define VF_FILTER_BICUBIC 3  /* PIL.Image.BICUBIC  */
@@ -515,6 +517,41 @@ int vf_debug_maxpool3d(const void* in, const int* vol_in, void* out, const int* 
                        const int* s, const int* p, int* path, void* stream);
 /* AvgPool3d((2,7,7), 1) of a T3 (>= 2) x 7 x 7 valid region, then the mean over time: out n x C fp32. */
 int vf_debug_i3d_head(const void* in, const int* vol, int C, float* out, void* stream);
+
+/* ---- Swin3D clip features: torchvision `swin3d_t` / `swin3d_s` / `swin3d_b` in eval mode, the feature
+ * `flatten(avgpool(norm(features(patch_embed(x)))))` (768-d for t / s, 1024-d for b), and the
+ * Swin3D_*_Weights.KINETICS400_V1 clip transform.  Weights: the torchvision state_dict by key (optionally with the
+ * "module." prefix), HOST fp32; head.* and relative_position_index are ignored (the index is computed).  The shape is
+ * inferred from the weights: embed dim from patch_embed.proj, depths from the features.{0,2,4,6}.* block keys, heads =
+ * dim / 32; patch (2,4,4) and window (8,7,7) are checked against the conv weight and the bias-table size.  Exactly the
+ * t / s / b shapes are accepted (VF_ERR_UNSUPPORTED naming the key otherwise). */
+typedef struct vf_swin3d vf_swin3d_t;
+
+/* Workspace holds max_clips clips of max_T frames (0 = 4 and 32); a call runs in chunks of as many clips of its T as the
+ * workspace holds (at most 256). */
+int vf_swin3d_create(vf_swin3d_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips,
+                     int max_T);
+int vf_swin3d_destroy(vf_swin3d_t* h);
+/* info receives 8 ints: out_dim, embed dim, the 4 depths, max_clips, max_T. */
+int vf_swin3d_info(const vf_swin3d_t* h, int* info);
+/* clips: n x 3 x T x 224 x 224 fp32 on the device, already transformed; T >= 1 (an odd T gets PatchEmbed3d's zero
+ * frame) -> out: n x out_dim fp32. */
+int vf_swin3d_forward_f32(vf_swin3d_t* h, const float* clips, int n, int T, float* out, void* stream);
+/* transform fused: frames n_frames x H x W x 3 uint8 BGR on the device, any size; clip i is frames starts[i] ..
+ * starts[i] + T - 1 (starts on the HOST) -> BGR->RGB, Resize([256]) bilinear without antialias on uint8, CenterCrop(224),
+ * /255, Normalize -> network.  Bit-identical to vf_swin3d_forward_f32 on the same transformed clips. */
+int vf_swin3d_forward_u8(vf_swin3d_t* h, const uint8_t* frames, int n_frames, int H, int W, const int* starts, int n,
+                         int T, float* out, void* stream);
+/* Diagnostics, the last chunk of the last forward, fp32 channels-last: stage 0 patch_embed (conv + norm), 1..4 the output
+ * of features.0 / 2 / 4 / 6, 5 the final norm.  dims5 receives (n, T', H', W', C); out == NULL only queries the shape. */
+int vf_swin3d_read_stage(vf_swin3d_t* h, int stage, float* out, int64_t capacity, int* dims5, void* stream);
+/* The window attention alone on caller rows: qkv n x Tq x H x W x 3C fp16 (q | k | v after the bias, heads of 32),
+ * bias_qkv the 3C fp32 qkv bias and table the (2535, C / 32) fp32 relative_position_bias_table, both on the device ->
+ * out n x Tq x H x W x C fp16.  Window (8,7,7), shift (4,3,3) if `shifted`, both clamped as torchvision's
+ * _get_window_and_shift_size does. */
+int vf_swin3d_attention(const void* qkv, const float* bias_qkv, const float* table, int n, int Tq, int H, int W, int C,
+                        int shifted, void* out, void* stream);
+int64_t vf_swin3d_launch_count(const vf_swin3d_t* h);
 
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),

@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("VF_LIBVFEAT") or os.path.join(_HERE, "libvfeat.so")
 
 VF_OK = 0
 VF_ACT_NONE, VF_ACT_QUICKGELU, VF_ACT_RELU, VF_ACT_SIGMOID, VF_ACT_TANH, VF_ACT_LEAKY = 0, 1, 2, 3, 4, 5
+VF_ACT_GELU = 6
 VF_FILTER_BILINEAR, VF_FILTER_BICUBIC = 2, 3
 VF_POOL_GENERAL, VF_POOL_FAST, VF_POOL_SAME3 = 0, 1, 2
 
@@ -193,6 +194,16 @@ SIGNATURES = {
     "vf_clip_rn_debug_attnpool_read": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
     "vf_debug_clip_rn_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                              C.c_void_p]),
+    "vf_swin3d_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int, C.c_int]),
+    "vf_swin3d_destroy": (C.c_int, [C.c_void_p]),
+    "vf_swin3d_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "vf_swin3d_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_swin3d_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int,
+                                       C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_swin3d_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_swin3d_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_swin3d_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_clip_vitl_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
     "vf_clip_vitl_destroy": (C.c_int, [C.c_void_p]),
     "vf_clip_vitl_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),

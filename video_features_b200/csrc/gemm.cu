@@ -121,7 +121,7 @@ static int run_gemm(const CUtensorMap& tmA, bool pp, const __half* B, int ldb, i
     if (reinterpret_cast<uintptr_t>(ep.out) & 15) return fail(VF_ERR_INVALID, "gemm: output must be 16-byte aligned");
     if (ep.accumulate && !ep.out_f32) return fail(VF_ERR_INVALID, "gemm: accumulate needs fp32 output");
     if (N % 8) return fail(VF_ERR_INVALID, "gemm: N=%d must be a multiple of 8", N);
-    if (ep.act < VF_ACT_NONE || ep.act > VF_ACT_LEAKY) return fail(VF_ERR_INVALID, "gemm: unknown activation %d", ep.act);
+    if (ep.act < VF_ACT_NONE || ep.act > VF_ACT_GELU) return fail(VF_ERR_INVALID, "gemm: unknown activation %d", ep.act);
     if (ep.out_f32 ? (ep.ldo % 4) : (ep.ldo % 8)) return fail(VF_ERR_INVALID, "gemm: ldo breaks 16-byte rows");
     if (ep.split_off && (ep.out_f32 || ep.split_off < N || ep.split_off % 8))
         return fail(VF_ERR_INVALID, "gemm: split output needs fp16 out and split_off >= N, multiple of 8");

@@ -69,6 +69,8 @@ __device__ __forceinline__ float apply_act(float v) {
         return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * v));   // saturates cleanly to +-1
     } else if (ACT == VF_ACT_LEAKY) {
         return v > 0.0f ? v : __fmul_rn(v, 0.1f);            // torch's leaky_relu: x * negative_slope below 0
+    } else if (ACT == VF_ACT_GELU) {
+        return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));   // torch's nn.GELU(): x * Phi(x), erf form
     }
     return v;
 }
@@ -379,6 +381,13 @@ int launch_act(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap
                 return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_LEAKY>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
             else
                 return fail(VF_ERR_INVALID, "gemm: LeakyReLU is built for split-weight convolutions (nsplit = 2) only");
+        case VF_ACT_GELU:
+            // Swin3D's MLP: only the plain ping-pong GEMM and the split-weight conv mode (Swin3D's 1-tap linears),
+            // without split output, carry the kernels
+            if constexpr (!SPLIT && ((NSPLIT == 1 && PP) || (NSPLIT == 2 && !PP)))
+                return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_GELU>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
+            else
+                return fail(VF_ERR_INVALID, "gemm: GELU is built for gemm_f16 and split-weight convolutions, without split output, only");
         default:
             return launch_gemm<BN, NSPLIT, SPLIT, PP, VF_ACT_NONE>(tmA, tmB, tmD, tmD2, ep, M, N, cg, stream);
     }
