@@ -553,6 +553,47 @@ int vf_swin3d_attention(const void* qkv, const float* bias_qkv, const float* tab
                         int shifted, void* out, void* stream);
 int64_t vf_swin3d_launch_count(const vf_swin3d_t* h);
 
+/* ---- MViT clip features: torchvision `mvit_v1_b` / `mvit_v2_s` in eval mode, the feature `norm(x)[:, 0]` (the class
+ * token after the final norm, 768-d), and the MViT_*_Weights.KINETICS400_V1 clip transform (16 frames, Resize([256]),
+ * CenterCrop(224), Normalize(0.45, 0.225)).  Weights: the torchvision state_dict by key (optionally with the "module."
+ * prefix), HOST fp32; head.* is ignored.  v2 is inferred from blocks.0.attn.rel_pos_h, v1 from
+ * pos_encoding.spatial_pos; every other key must have the size torchvision gives it (VF_ERR_INVALID /
+ * VF_ERR_UNSUPPORTED naming the key otherwise). */
+typedef struct vf_mvit vf_mvit_t;
+
+/* Workspace holds max_clips clips (0 = 4), about 190 MB each; a call runs in chunks of as many clips (at most 256). */
+int vf_mvit_create(vf_mvit_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_clips);
+int vf_mvit_destroy(vf_mvit_t* h);
+/* info receives 4 ints: out_dim (768), version (1 or 2), T (16), max_clips. */
+int vf_mvit_info(const vf_mvit_t* h, int* info);
+/* clips: n x 3 x 16 x 224 x 224 fp32 on the device, already transformed; T must be 16 -> out: n x 768 fp32. */
+int vf_mvit_forward_f32(vf_mvit_t* h, const float* clips, int n, int T, float* out, void* stream);
+/* transform fused: frames n_frames x H x W x 3 uint8 BGR on the device, any size; clip i is frames starts[i] ..
+ * starts[i] + 15 (starts on the HOST) -> BGR->RGB, Resize([256]) bilinear without antialias on uint8, CenterCrop(224),
+ * /255, Normalize -> network.  Bit-identical to vf_mvit_forward_f32 on the same transformed clips. */
+int vf_mvit_forward_u8(vf_mvit_t* h, const uint8_t* frames, int n_frames, int H, int W, const int* starts, int n, int T,
+                       float* out, void* stream);
+/* Diagnostics, the last chunk of the last forward, fp32 token rows [class | T' x H' x W' tokens]: stage 0 the patch
+ * embedding with class token and positions, 1..4 the output of blocks 0 / 2 / 13 / 15 (the blocks before each q stride
+ * and the last), 5 the final norm on every row.  dims3 receives (n, tokens, C); out == NULL only queries the shape. */
+int vf_mvit_read_stage(vf_mvit_t* h, int stage, float* out, int64_t capacity, int* dims3, void* stream);
+/* The pooling attention alone: q n x (1 + prod(q_thw)) rows of pitch ldq, k / v n x (1 + prod(k_thw)) x heads*96 fp16
+ * (heads of 96 channels) -> out n x (1 + prod(q_thw)) x heads*96 fp16.  rel: the decomposed rel-pos bias from rel_h /
+ * rel_w (2 max(q_h, k_h) - 1 rows of 96) and rel_t (2 max(q_t, k_t) - 1 rows), fp32 on the device; resid: + q on the
+ * token rows.  k_thw[0] + k_thw[1] + k_thw[2] <= 48. */
+int vf_mvit_attention(const void* q, int ldq, const void* k, const void* v, const float* rel_h, const float* rel_w,
+                      const float* rel_t, int n, int heads, const int* q_thw, const int* k_thw, int rel, int resid,
+                      void* out, void* stream);
+/* The head pooling alone: src n x (1 + T H W) rows of pitch ld_src fp16 -> depthwise 3x3x3 conv, stride
+ * (1, stride, stride), pad 1 (weight 96 x 27 fp32) per head of 96 on the tokens, class row passed through, then
+ * LayerNorm(96, eps 1e-6) (gamma, beta) on every row -> dst n x (1 + T Ho Wo) x heads*96 fp16. */
+int vf_mvit_head_pool(const void* src, int ld_src, int n, int heads, int T, int H, int W, int stride,
+                      const float* weight, const float* gamma, const float* beta, void* dst, void* stream);
+/* The skip max-pool alone: MaxPool3d((1,3,3), (1,2,2), (0,1,1)) of x n x (1 + T H W) x C fp32 tokens, class row
+ * copied -> y n x (1 + T Ho Wo) x C. */
+int vf_mvit_skip_pool(const float* x, int n, int C, int T, int H, int W, float* y, void* stream);
+int64_t vf_mvit_launch_count(const vf_mvit_t* h);
+
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),
  * and the softmax + sort of utils/utils.py:19-47.  weight: n_classes x n_features, bias: n_classes, HOST fp32. */

@@ -6,7 +6,7 @@ feature type (torchvision's S3D, the Kinetics-400 clip feature upstream video_fe
 outside the reference's list, and the ``CLIP-ViT-L/14`` / ``CLIP-ViT-L/14@336px`` feature types (openai's largest
 released ViT, 768-d features), which the reference does not offer either; ``--model_name`` selects upstream's IG65M
 R(2+1)D-34 models for ``r21d_rgb``; ``swin3d_t`` / ``swin3d_s`` / ``swin3d_b`` are torchvision's Swin3D video
-transformers (Kinetics-400 clip features).
+transformers and ``mvit_v1_b`` / ``mvit_v2_s`` its Multiscale Vision Transformers (Kinetics-400 clip features).
 """
 import argparse
 import functools
@@ -18,7 +18,7 @@ from video_features_b200.utils import form_list_from_user_input, sanity_check
 
 SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
              'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch', 's3d', 'CLIP-ViT-L/14', 'CLIP-ViT-L/14@336px',
-             'swin3d_t', 'swin3d_s', 'swin3d_b']
+             'swin3d_t', 'swin3d_s', 'swin3d_b', 'mvit_v1_b', 'mvit_v2_s']
 
 
 def build_extractor(args):
@@ -47,6 +47,9 @@ def build_extractor(args):
     if args.feature_type in ['swin3d_t', 'swin3d_s', 'swin3d_b']:
         from video_features_b200.extract.extract_swin3d import ExtractSwin3D
         return ExtractSwin3D(args)
+    if args.feature_type in ['mvit_v1_b', 'mvit_v2_s']:
+        from video_features_b200.extract.extract_mvit import ExtractMViT
+        return ExtractMViT(args)
     if args.feature_type == 'vggish_torch':
         from video_features_b200.extract.extract_vggish import ExtractVGGish
         return ExtractVGGish(args)
@@ -86,7 +89,7 @@ def parallel_feature_extraction(args):
 
 
 _FEATURE_TYPES = ('i3d vggish r21d_rgb resnet18 resnet34 resnet50 resnet101 resnet152 raft pwc CLIP-ViT-B/32 CLIP-ViT-B/16 '
-                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d CLIP-ViT-L/14 CLIP-ViT-L/14@336px swin3d_t swin3d_s swin3d_b').split()
+                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d CLIP-ViT-L/14 CLIP-ViT-L/14@336px swin3d_t swin3d_s swin3d_b mvit_v1_b mvit_v2_s').split()
 
 # (flag, argparse keywords): names, types, defaults, choices and dests are the reference's (main.py:93-149)
 _FLAGS = [
@@ -111,8 +114,8 @@ _FLAGS = [
                                    'r2plus1d_34_8_ig65m_ft_kinetics'], default=None,
                           help='r21d_rgb network (default r2plus1d_18_16_kinetics; the R(2+1)D-34 IG65M models default '
                                'to 32 / 32 and 8 / 8 frame stacks)')),
-    ('--stack_size', dict(type=int, help='frames per I3D / R(2+1)D / S3D / Swin3D stack')),
-    ('--step_size', dict(type=int, help='frames between I3D / R(2+1)D / S3D / Swin3D stacks')),
+    ('--stack_size', dict(type=int, help='frames per I3D / R(2+1)D / S3D / Swin3D stack (MViT: 16 only)')),
+    ('--step_size', dict(type=int, help='frames between I3D / R(2+1)D / S3D / Swin3D / MViT stacks')),
     ('--streams', dict(nargs='+', choices=['flow', 'rgb'], help='I3D streams (default: both)')),
     ('--flow_type', dict(choices=['raft', 'pwc', 'flow'], default='pwc', help='optical flow feeding the I3D flow stream')),
     ('--batch_size', dict(type=int, default=1, help='frame pairs per RAFT call')),
@@ -120,7 +123,7 @@ _FLAGS = [
                                     help='--side_size applies to the larger edge instead of the smaller one')),
     ('--side_size', dict(type=int, help='RAFT: resize frames to this edge length first')),
     ('--show_pred', dict(dest='show_pred', action='store_true', default=False,
-                         help='print the top-5 classes of every feature (I3D, R(2+1)D, S3D, Swin3D: Kinetics-400; ResNet: ImageNet)')),
+                         help='print the top-5 classes of every feature (I3D, R(2+1)D, S3D, Swin3D, MViT: Kinetics-400; ResNet: ImageNet)')),
     # not in the reference: after extraction, ONE all-gather (NCCL over NVLink) returns every rank's feature blocks and
     # rank 0 writes them, list order, to this .npz
     ('--gather_features', dict(type=str, default=None, help='also all-gather the features of all GPUs into this .npz')),

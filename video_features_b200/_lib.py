@@ -204,6 +204,20 @@ SIGNATURES = {
     "vf_swin3d_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_int, C.c_void_p, C.c_void_p]),
     "vf_swin3d_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_mvit_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
+    "vf_mvit_destroy": (C.c_int, [C.c_void_p]),
+    "vf_mvit_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "vf_mvit_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_mvit_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int,
+                                     C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_mvit_read_stage": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int), C.c_void_p]),
+    "vf_mvit_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int,
+                                    C.c_void_p, C.c_void_p]),
+    "vf_mvit_head_pool": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vf_mvit_skip_pool": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_mvit_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_clip_vitl_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
     "vf_clip_vitl_destroy": (C.c_int, [C.c_void_p]),
     "vf_clip_vitl_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),

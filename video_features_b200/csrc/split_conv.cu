@@ -197,4 +197,43 @@ int clip_window(const char* who, const int* starts, int n, int T, int per_chunk,
     return VF_OK;
 }
 
+int upload_vec(EngineCore* h, const ResTensors& T, const std::string& name, int64_t n, float** dst) {
+    const float* a;
+    VF_TRY(T.get(name, n, &a));
+    VF_TRY(ralloc(h, dst, size_t(n)));
+    VF_CUDA(cudaMemcpy(*dst, a, size_t(n) * sizeof(float), cudaMemcpyHostToDevice));
+    return VF_OK;
+}
+
+int upload_split_mat(EngineCore* h, const ResTensors& T, const std::string& name, int64_t rows, int64_t cols,
+                     __half** dst, int64_t cols_pad) {
+    const float* a;
+    VF_TRY(T.get(name, rows * cols, &a));
+    const int64_t kp = cols_pad > 0 ? cols_pad : cols;
+    std::vector<__half> tmp(size_t(rows * kp * 2), __float2half_rn(0.f));
+    for (int64_t r = 0; r < rows; ++r)
+        for (int64_t c = 0; c < cols; ++c) {
+            const __half hi = __float2half_rn(a[r * cols + c]);
+            tmp[size_t(r * 2 * kp + c)] = hi;
+            tmp[size_t(r * 2 * kp + kp + c)] = __float2half_rn(a[r * cols + c] - __half2float(hi));
+        }
+    VF_TRY(ralloc(h, dst, tmp.size()));
+    VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    return VF_OK;
+}
+
+GemmEpi linear_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate) {
+    GemmEpi e;
+    memset(&e, 0, sizeof(e));
+    e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.bias = bias; e.act = act; e.accumulate = accumulate;
+    return e;
+}
+
+int split_linear(const __half* A, int M, int N, int K, const __half* W2, const GemmEpi& ep, cudaStream_t s) {
+    ConvGeom g;
+    memset(&g, 0, sizeof(g));
+    g.ntaps = 1; g.k_per_tap = K; g.nsplit = 2; g.lo_mask = 0; g.mask = 0;
+    return conv_gemm_f16(A, K, M, W2, N, g, ep, s);
+}
+
 }  // namespace vf

@@ -76,6 +76,18 @@ int run_conv(EngineCore* h, const ResConv& cw, const __half* X, int pitch, const
 int run_conv(EngineCore* h, const ResConv& cw, const __half* X, int pitch, const Vol2& v, __half* out, bool relu,
              cudaStream_t s);
 
+// ---- split-fp16 linears of the video transformers (swin3d.cu, mvit.cu)
+// fp32 vector `name` of n elements -> device copy
+int upload_vec(EngineCore* h, const ResTensors& T, const std::string& name, int64_t n, float** dst);
+// weight [rows][cols] -> split-fp16 pair rows [hi kp | lo kp] (kp = cols_pad, 0: cols; columns from cols on zero),
+// lo = fp16(w - hi), round-to-nearest-even
+int upload_split_mat(EngineCore* h, const ResTensors& T, const std::string& name, int64_t rows, int64_t cols,
+                     __half** dst, int64_t cols_pad = 0);
+GemmEpi linear_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate = 0);
+// out = A[M, K] . (W_hi + W_lo)^T with the epilogue `ep`: a 1-tap split-weight linear on the conv-mode GEMM (A rows of
+// pitch K, no row mask), as clip_resnet.cu's linears
+int split_linear(const __half* A, int M, int N, int K, const __half* W2, const GemmEpi& ep, cudaStream_t s);
+
 // vf_*_conv read-back: geometry, lo_mask and (when the pointers are set) the uploaded weights / scale / bias
 int read_back_conv(int device, const ResConv& c, int* geom, uint64_t* lo_mask, void* w, float* scale, float* bias);
 

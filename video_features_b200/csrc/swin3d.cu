@@ -56,60 +56,18 @@ struct vf_swin3d : vf::EngineCore {
 
 namespace vf {
 
-static int sw_upload_f32(vf_swin3d* h, float** dst, const float* src, size_t count) {
-    VF_TRY(ralloc(h, dst, count));
-    VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-static int sw_vec(vf_swin3d* h, const ResTensors& T, const std::string& name, int64_t n, float** dst) {
-    const float* a;
-    VF_TRY(T.get(name, n, &a));
-    return sw_upload_f32(h, dst, a, size_t(n));
-}
-// weight [rows][cols] -> split-fp16 pair rows [hi cols | lo cols], lo = fp16(w - hi), round-to-nearest-even
-static int sw_mat(vf_swin3d* h, const ResTensors& T, const std::string& name, int64_t rows, int64_t cols, __half** dst) {
-    const float* a;
-    VF_TRY(T.get(name, rows * cols, &a));
-    std::vector<__half> tmp(size_t(rows * cols * 2));
-    for (int64_t r = 0; r < rows; ++r)
-        for (int64_t c = 0; c < cols; ++c) {
-            const __half hi = __float2half_rn(a[r * cols + c]);
-            tmp[size_t(r * 2 * cols + c)] = hi;
-            tmp[size_t(r * 2 * cols + cols + c)] = __float2half_rn(a[r * cols + c] - __half2float(hi));
-        }
-    VF_TRY(ralloc(h, dst, tmp.size()));
-    VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-
-static GemmEpi sw_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate = 0) {
-    GemmEpi e;
-    memset(&e, 0, sizeof(e));
-    e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.bias = bias; e.act = act; e.accumulate = accumulate;
-    return e;
-}
-
-// out = A[M, K] . (W_hi + W_lo)^T with the epilogue `ep`: a 1-tap split-weight linear on the conv-mode GEMM (A rows of
-// pitch K, no row mask), as clip_resnet.cu's linears
-static int sw_linear(const __half* A, int M, int N, int K, const __half* W2, const GemmEpi& ep, cudaStream_t s) {
-    ConvGeom g;
-    memset(&g, 0, sizeof(g));
-    g.ntaps = 1; g.k_per_tap = K; g.nsplit = 2; g.lo_mask = 0; g.mask = 0;
-    return conv_gemm_f16(A, K, M, W2, N, g, ep, s);
-}
-
 static int tq_of(int T) { return (T + 1) / 2; }
 
 // one SwinTransformerBlock on the stage's residual stream x (rows R of C), in place
 static int run_block(vf_swin3d* h, const SwBlock& w, float* x, int m, int Tq, int S, int C, bool shifted, cudaStream_t s) {
     const int R = m * Tq * S * S;
     VF_TRY(swin3d_layernorm(x, C, w.n1w, w.n1b, h->hbuf, 0, R, s));
-    VF_TRY(sw_linear(h->hbuf, R, 3 * C, C, w.wqkv, sw_epi(h->qkv, 3 * C, 0, w.bqkv, VF_ACT_NONE), s));
+    VF_TRY(split_linear(h->hbuf, R, 3 * C, C, w.wqkv, linear_epi(h->qkv, 3 * C, 0, w.bqkv, VF_ACT_NONE), s));
     VF_TRY(swin3d_attention(h->qkv, w.bqkv, w.table, h->att, swin3d_attn_geom(m, Tq, S, S, C, shifted), s));
-    VF_TRY(sw_linear(h->att, R, C, C, w.wproj, sw_epi(x, C, 1, w.bproj, VF_ACT_NONE, 1), s));
+    VF_TRY(split_linear(h->att, R, C, C, w.wproj, linear_epi(x, C, 1, w.bproj, VF_ACT_NONE, 1), s));
     VF_TRY(swin3d_layernorm(x, C, w.n2w, w.n2b, h->hbuf, 0, R, s));
-    VF_TRY(sw_linear(h->hbuf, R, 4 * C, C, w.wfc1, sw_epi(h->mlp, 4 * C, 0, w.bfc1, VF_ACT_GELU), s));
-    VF_TRY(sw_linear(h->mlp, R, C, 4 * C, w.wfc2, sw_epi(x, C, 1, w.bfc2, VF_ACT_NONE, 1), s));
+    VF_TRY(split_linear(h->hbuf, R, 4 * C, C, w.wfc1, linear_epi(h->mlp, 4 * C, 0, w.bfc1, VF_ACT_GELU), s));
+    VF_TRY(split_linear(h->mlp, R, C, 4 * C, w.wfc2, linear_epi(x, C, 1, w.bfc2, VF_ACT_NONE, 1), s));
     h->launches += 7;
     return VF_OK;
 }
@@ -118,7 +76,7 @@ static int run_block(vf_swin3d* h, const SwBlock& w, float* x, int m, int Tq, in
 static int run_net(vf_swin3d* h, int m, int T, cudaStream_t s) {
     const int Tq = tq_of(T), C = h->dim;
     const int R = m * Tq * 3136;
-    VF_TRY(sw_linear(h->patches, R, C, SW_PK, h->w_patch, sw_epi(h->emb, C, 1, h->b_patch, VF_ACT_NONE), s));
+    VF_TRY(split_linear(h->patches, R, C, SW_PK, h->w_patch, linear_epi(h->emb, C, 1, h->b_patch, VF_ACT_NONE), s));
     VF_TRY(swin3d_layernorm(h->emb, C, h->pe_w, h->pe_b, h->x[0], 1, R, s, h->x[1]));
     h->launches += 2;
     for (int st = 0; st < 4; ++st) {
@@ -128,8 +86,8 @@ static int run_net(vf_swin3d* h, int m, int T, cudaStream_t s) {
         if (st < 3) {
             const int Rn = m * Tq * (S / 2) * (S / 2);
             VF_TRY(swin3d_merge_layernorm(h->x[st + 1], m, Tq, S, S, Cs, h->merge[st].nw, h->merge[st].nb, h->hbuf, s));
-            VF_TRY(sw_linear(h->hbuf, Rn, 2 * Cs, 4 * Cs, h->merge[st].wred,
-                             sw_epi(h->x[st + 2], 2 * Cs, 1, nullptr, VF_ACT_NONE), s));
+            VF_TRY(split_linear(h->hbuf, Rn, 2 * Cs, 4 * Cs, h->merge[st].wred,
+                                linear_epi(h->x[st + 2], 2 * Cs, 1, nullptr, VF_ACT_NONE), s));
             h->launches += 2;
         }
     }
@@ -205,37 +163,37 @@ int vf_swin3d_create(vf_swin3d_t** out, const vf_named_tensor* tensors, int n_te
     h->cap_rows = int64_t(max_clips) * tq_of(max_T) * 3136;
     auto body = [&]() -> int {
         const int C = dim;
-        VF_TRY(sw_mat(h, Tn, "patch_embed.proj.weight", C, SW_PK, &h->w_patch));   // [C][c kt kh kw] pairs
-        VF_TRY(sw_vec(h, Tn, "patch_embed.proj.bias", C, &h->b_patch));
-        VF_TRY(sw_vec(h, Tn, "patch_embed.norm.weight", C, &h->pe_w));
-        VF_TRY(sw_vec(h, Tn, "patch_embed.norm.bias", C, &h->pe_b));
-        VF_TRY(sw_vec(h, Tn, "norm.weight", 8 * C, &h->norm_w));
-        VF_TRY(sw_vec(h, Tn, "norm.bias", 8 * C, &h->norm_b));
+        VF_TRY(upload_split_mat(h, Tn, "patch_embed.proj.weight", C, SW_PK, &h->w_patch));   // [C][c kt kh kw] pairs
+        VF_TRY(upload_vec(h, Tn, "patch_embed.proj.bias", C, &h->b_patch));
+        VF_TRY(upload_vec(h, Tn, "patch_embed.norm.weight", C, &h->pe_w));
+        VF_TRY(upload_vec(h, Tn, "patch_embed.norm.bias", C, &h->pe_b));
+        VF_TRY(upload_vec(h, Tn, "norm.weight", 8 * C, &h->norm_w));
+        VF_TRY(upload_vec(h, Tn, "norm.bias", 8 * C, &h->norm_b));
         for (int st = 0; st < 4; ++st) {
             const int64_t Cs = C << st, heads = Cs / SW_HEAD_DIM;
             for (int d = 0; d < depths[st]; ++d) {
                 const std::string p = "features." + std::to_string(2 * st) + "." + std::to_string(d) + ".";
                 SwBlock w;
-                VF_TRY(sw_vec(h, Tn, p + "norm1.weight", Cs, &w.n1w));
-                VF_TRY(sw_vec(h, Tn, p + "norm1.bias", Cs, &w.n1b));
-                VF_TRY(sw_vec(h, Tn, p + "norm2.weight", Cs, &w.n2w));
-                VF_TRY(sw_vec(h, Tn, p + "norm2.bias", Cs, &w.n2b));
-                VF_TRY(sw_vec(h, Tn, p + "attn.qkv.bias", 3 * Cs, &w.bqkv));
-                VF_TRY(sw_vec(h, Tn, p + "attn.proj.bias", Cs, &w.bproj));
-                VF_TRY(sw_vec(h, Tn, p + "mlp.0.bias", 4 * Cs, &w.bfc1));
-                VF_TRY(sw_vec(h, Tn, p + "mlp.3.bias", Cs, &w.bfc2));
-                VF_TRY(sw_vec(h, Tn, p + "attn.relative_position_bias_table", SW_TABLE * heads, &w.table));
-                VF_TRY(sw_mat(h, Tn, p + "attn.qkv.weight", 3 * Cs, Cs, &w.wqkv));
-                VF_TRY(sw_mat(h, Tn, p + "attn.proj.weight", Cs, Cs, &w.wproj));
-                VF_TRY(sw_mat(h, Tn, p + "mlp.0.weight", 4 * Cs, Cs, &w.wfc1));
-                VF_TRY(sw_mat(h, Tn, p + "mlp.3.weight", Cs, 4 * Cs, &w.wfc2));
+                VF_TRY(upload_vec(h, Tn, p + "norm1.weight", Cs, &w.n1w));
+                VF_TRY(upload_vec(h, Tn, p + "norm1.bias", Cs, &w.n1b));
+                VF_TRY(upload_vec(h, Tn, p + "norm2.weight", Cs, &w.n2w));
+                VF_TRY(upload_vec(h, Tn, p + "norm2.bias", Cs, &w.n2b));
+                VF_TRY(upload_vec(h, Tn, p + "attn.qkv.bias", 3 * Cs, &w.bqkv));
+                VF_TRY(upload_vec(h, Tn, p + "attn.proj.bias", Cs, &w.bproj));
+                VF_TRY(upload_vec(h, Tn, p + "mlp.0.bias", 4 * Cs, &w.bfc1));
+                VF_TRY(upload_vec(h, Tn, p + "mlp.3.bias", Cs, &w.bfc2));
+                VF_TRY(upload_vec(h, Tn, p + "attn.relative_position_bias_table", SW_TABLE * heads, &w.table));
+                VF_TRY(upload_split_mat(h, Tn, p + "attn.qkv.weight", 3 * Cs, Cs, &w.wqkv));
+                VF_TRY(upload_split_mat(h, Tn, p + "attn.proj.weight", Cs, Cs, &w.wproj));
+                VF_TRY(upload_split_mat(h, Tn, p + "mlp.0.weight", 4 * Cs, Cs, &w.wfc1));
+                VF_TRY(upload_split_mat(h, Tn, p + "mlp.3.weight", Cs, 4 * Cs, &w.wfc2));
                 h->blocks[st].push_back(w);
             }
             if (st < 3) {
                 const std::string p = "features." + std::to_string(2 * st + 1) + ".";
-                VF_TRY(sw_vec(h, Tn, p + "norm.weight", 4 * Cs, &h->merge[st].nw));
-                VF_TRY(sw_vec(h, Tn, p + "norm.bias", 4 * Cs, &h->merge[st].nb));
-                VF_TRY(sw_mat(h, Tn, p + "reduction.weight", 2 * Cs, 4 * Cs, &h->merge[st].wred));
+                VF_TRY(upload_vec(h, Tn, p + "norm.weight", 4 * Cs, &h->merge[st].nw));
+                VF_TRY(upload_vec(h, Tn, p + "norm.bias", 4 * Cs, &h->merge[st].nb));
+                VF_TRY(upload_split_mat(h, Tn, p + "reduction.weight", 2 * Cs, 4 * Cs, &h->merge[st].wred));
             }
         }
         // workspace for cap_rows stage-1 rows R: stage s has R / 4^s rows of C << s, so every per-row buffer is largest

@@ -4,6 +4,8 @@
 #include <atomic>
 
 #include "common.cuh"
+#include "mma_sync.cuh"
+#include "resize_u8.cuh"
 #include "swin3d_kernels.h"
 
 namespace vf {
@@ -15,17 +17,6 @@ __constant__ float kSwMean[3] = {0.485f, 0.456f, 0.406f};
 __constant__ float kSwStd[3] = {0.229f, 0.224f, 0.225f};
 
 inline unsigned nb(int64_t total, int threads) { return unsigned((total + threads - 1) / threads); }
-
-// torch's CPU upsample_bilinear2d (align_corners=False, no scale factor) source index and weights for output index d,
-// as r21d_kernels.cu computes them, with the output size a run-time value
-__device__ __forceinline__ void bilinear_tap(int d, int in, int out, int& i0, int& i1, float& l0, float& l1) {
-    const float scale = __fdiv_rn(float(in), float(out));
-    const float src = fmaxf(__fmaf_rn(scale, __fadd_rn(float(d), 0.5f), -0.5f), 0.f);
-    i0 = min(int(floorf(src)), in - 1);
-    l1 = fminf(fmaxf(__fsub_rn(src, float(i0)), 0.f), 1.f);
-    i1 = i0 + (i0 < in - 1 ? 1 : 0);
-    l0 = __fsub_rn(1.f, l1);
-}
 
 // One thread per (patch row, channel c, temporal tap kt): the 16 columns c * 32 + kt * 16 + kh * 4 + kw.
 // U8: F.resize of the uint8 frame (float interpolation of the bytes, torch.round half to even, uint8), /255, Normalize,
@@ -57,10 +48,7 @@ __global__ void patch_kernel(const void* __restrict__ src, R21DStarts st, int m,
                     int w0, w1;
                     float b0, b1;
                     bilinear_tap(wq * 4 + kw + cx, W, rw, w0, w1, b0, b1);
-                    auto px = [&](int hh, int ww) { return float(__ldg(fr + (int64_t(hh) * W + ww) * 3 + sc)); };
-                    const float t0 = __fmaf_rn(b0, px(h0, w0), __fmul_rn(b1, px(h0, w1)));
-                    const float t1 = __fmaf_rn(b0, px(h1, w0), __fmul_rn(b1, px(h1, w1)));
-                    const float r = __fdiv_rn(rintf(__fmaf_rn(a0, t0, __fmul_rn(a1, t1))), 255.f);
+                    const float r = resized_unit(fr, W, sc, h0, h1, a0, a1, w0, w1, b0, b1);
                     v[kh * 4 + kw] = __float2half_rn(__fdiv_rn(__fsub_rn(r, kSwMean[c]), kSwStd[c]));
                 }
             }
@@ -79,7 +67,8 @@ __global__ void patch_kernel(const void* __restrict__ src, R21DStarts st, int m,
 }
 
 // LayerNorm statistics of one row of C fp32 (one warp; lane-strided partial sums, then the butterfly): two passes
-__device__ __forceinline__ void ln_stats(const float* __restrict__ xr, int C, int lane, float& mean, float& rstd) {
+__device__ __forceinline__ void ln_stats(const float* __restrict__ xr, int C, int lane, float& mean, float& rstd,
+                                         float eps = 1e-5f) {
     float s = 0.f;
     for (int c = lane; c < C; c += 32) s += xr[c];
     mean = warp_sum(s) / float(C);
@@ -88,18 +77,19 @@ __device__ __forceinline__ void ln_stats(const float* __restrict__ xr, int C, in
         const float d = xr[c] - mean;
         q += d * d;
     }
-    rstd = rsqrtf(warp_sum(q) / float(C) + 1e-5f);
+    rstd = rsqrtf(warp_sum(q) / float(C) + eps);
 }
 
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, int C, const float* __restrict__ gamma,
                                                         const float* __restrict__ beta, void* __restrict__ out,
-                                                        int out_f32, float* __restrict__ out2, int64_t rows) {
+                                                        int out_f32, float* __restrict__ out2, int64_t rows,
+                                                        float eps) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t row = int64_t(blockIdx.x) * 8 + warp;
     if (row >= rows) return;
     const float* xr = x + row * C;
     float mean, rstd;
-    ln_stats(xr, C, lane, mean, rstd);
+    ln_stats(xr, C, lane, mean, rstd, eps);
     for (int c = lane; c < C; c += 32) {
         const float y = (xr[c] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
         if (out_f32) {
@@ -201,24 +191,6 @@ __global__ void __launch_bounds__(256) norm_mean_kernel(const float* __restrict_
 // score -inf; padded queries are computed and not stored.
 constexpr int WA_LD = 40, WA_KB = 64, WA_MAXN = 448;
 constexpr int WA_SMEM = 2 * WA_MAXN * WA_LD * 2 + SW_TABLE * 4 + 3 * WA_MAXN * 4;
-
-__device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t* r, const void* p) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ void ldsm_x4_trans(uint32_t* r, const void* p) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
-}
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
-}
 
 __global__ void __launch_bounds__(256, 2) window_attention_kernel(const __half* __restrict__ qkv,
                                                                   const float* __restrict__ bias_qkv,
@@ -405,9 +377,9 @@ int swin3d_patch_f32(const float* clips, int m, int T, __half* out, cudaStream_t
 }
 
 int swin3d_layernorm(const float* x, int C, const float* gamma, const float* beta, void* out, int out_f32, int64_t rows,
-                     cudaStream_t s, float* out2) {
+                     cudaStream_t s, float* out2, float eps) {
     if (out2 && !out_f32) return fail(VF_ERR_INVALID, "swin3d_layernorm: a second copy needs fp32 output");
-    layernorm_kernel<<<nb(rows, 8), 256, 0, s>>>(x, C, gamma, beta, out, out_f32, out2, rows);
+    layernorm_kernel<<<nb(rows, 8), 256, 0, s>>>(x, C, gamma, beta, out, out_f32, out2, rows, eps);
     LAUNCH_CHECK();
 }
 

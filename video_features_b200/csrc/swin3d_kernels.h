@@ -18,10 +18,10 @@ int swin3d_patch_u8(const uint8_t* frames, const R21DStarts& st, int m, int T, i
                     int cx, __half* out, cudaStream_t s);
 // f32: m x 3 x T x 224 x 224 clips, already transformed
 int swin3d_patch_f32(const float* clips, int m, int T, __half* out, cudaStream_t s);
-// LayerNorm (eps 1e-5, two-pass fp32 statistics) of rows of C fp32 -> fp16 or fp32 rows (pitch C); out_f32 only: a
-// non-null out2 receives a second copy
+// LayerNorm (two-pass fp32 statistics, eps 1e-5 unless given: MViT's are 1e-6) of rows of C fp32 -> fp16 or fp32 rows
+// (pitch C); out_f32 only: a non-null out2 receives a second copy
 int swin3d_layernorm(const float* x, int C, const float* gamma, const float* beta, void* out, int out_f32, int64_t rows,
-                     cudaStream_t s, float* out2 = nullptr);
+                     cudaStream_t s, float* out2 = nullptr, float eps = 1e-5f);
 // PatchMerging: x [n][T'][H][W][C] fp32 (H, W even) -> LayerNorm of the rows [x0 | x1 | x2 | x3] (4C) -> fp16
 // [n][T'][H/2][W/2][4C]
 int swin3d_merge_layernorm(const float* x, int n, int Tq, int H, int W, int C, const float* gamma, const float* beta,

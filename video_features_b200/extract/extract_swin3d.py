@@ -59,20 +59,25 @@ def load_swin3d_weights(feature_type: str) -> Dict[str, torch.Tensor]:
 
 
 class ExtractSwin3D(torch.nn.Module):
+    # what a subclass for another torchvision video model replaces (extract_mvit.py)
+    patterns = PATTERNS
+    head_keys = SWIN3D_KEYS
+    default_stack = DEFAULT_SWIN3D_STACK_SIZE
+    default_step = DEFAULT_SWIN3D_STEP_SIZE
 
     def __init__(self, args):
         super(ExtractSwin3D, self).__init__()
         self.feature_type = args.feature_type
-        if self.feature_type not in PATTERNS:
+        if self.feature_type not in self.patterns:
             raise NotImplementedError(self.feature_type)
         self.path_list = form_list_from_user_input(args)
         self.extraction_fps = args.extraction_fps
         self.step_size = args.step_size
         self.stack_size = args.stack_size
         if self.step_size is None:
-            self.step_size = DEFAULT_SWIN3D_STEP_SIZE
+            self.step_size = self.default_step
         if self.stack_size is None:
-            self.stack_size = DEFAULT_SWIN3D_STACK_SIZE
+            self.stack_size = self.default_stack
         if self.extraction_fps is not None:
             raise NotImplementedError("extraction_fps re-encodes with ffmpeg (outside the rebuilt path, SURVEY.md §2)")
         if self.stack_size < 1 or self.step_size < 1:
@@ -86,7 +91,7 @@ class ExtractSwin3D(torch.nn.Module):
         self.output_path = os.path.join(args.output_path, self.feature_type)
         self.progress = tqdm(total=len(self.path_list))
         self.keep_features = False
-        self._engines: Dict[int, Swin3DEngine] = {}
+        self._engines: Dict[int, object] = {}
         self._heads: Dict[int, ClassHead] = {}
         self._pinned: Dict[tuple, List[torch.Tensor]] = {}
 
@@ -122,19 +127,24 @@ class ExtractSwin3D(torch.nn.Module):
                 sink.close()
         return feats_list
 
-    def _engine(self, device: torch.device) -> Swin3DEngine:
+    def load_weights(self) -> Dict[str, torch.Tensor]:
+        return load_swin3d_weights(self.feature_type)
+
+    def new_engine(self, idx: int):
+        # a workspace of about CLIPS_PER_CALL 32-frame stacks whatever the stack size; the engine chunks larger calls
+        T = self.stack_size
+        return Swin3DEngine(self.load_weights(), idx, max_clips=max(1, CLIPS_PER_CALL * 16 // ((T + 1) // 2)), max_T=T)
+
+    def _engine(self, device: torch.device):
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if idx not in self._engines:
-            # a workspace of about CLIPS_PER_CALL 32-frame stacks whatever the stack size; the engine chunks larger calls
-            T = self.stack_size
-            self._engines[idx] = Swin3DEngine(load_swin3d_weights(self.feature_type), idx,
-                                              max_clips=max(1, CLIPS_PER_CALL * 16 // ((T + 1) // 2)), max_T=T)
+            self._engines[idx] = self.new_engine(idx)
         return self._engines[idx]
 
     def _head(self, device: torch.device) -> ClassHead:
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if idx not in self._heads:
-            self._heads[idx] = ClassHead.from_state_dict(load_swin3d_weights(self.feature_type), SWIN3D_KEYS, idx,
+            self._heads[idx] = ClassHead.from_state_dict(self.load_weights(), self.head_keys, idx,
                                                          f"{self.feature_type} checkpoint")
         return self._heads[idx]
 
