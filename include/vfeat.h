@@ -594,6 +594,31 @@ int vf_mvit_head_pool(const void* src, int ld_src, int n, int heads, int T, int 
 int vf_mvit_skip_pool(const float* x, int n, int C, int T, int H, int W, float* y, void* stream);
 int64_t vf_mvit_launch_count(const vf_mvit_t* h);
 
+/* ---- CLIP text tower (zero-shot --show_pred of the CLIP feature types): openai/CLIP's `CLIP.encode_text` followed by
+ * L2 normalisation.  Weights: the checkpoint's non-visual tensors by key (token_embedding.weight, positional_embedding,
+ * transformer.resblocks.*, ln_final.*, text_projection), HOST fp32.  The geometry is read from them as
+ * clip.build_model reads it; 12 blocks at width 512 (8 heads), 640 (10) or 768 (12) are built, anything else is
+ * refused (VF_ERR_UNSUPPORTED). */
+typedef struct vf_clip_text vf_clip_text_t;
+
+/* Workspace of max_rows token rows (0 = 8192); a call runs in chunks of max_rows / L prompts. */
+int vf_clip_text_create(vf_clip_text_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_rows);
+int vf_clip_text_destroy(vf_clip_text_t* h);
+/* info receives 7 ints: width, heads, layers, context, embed, vocabulary size, max_rows. */
+int vf_clip_text_info(const vf_clip_text_t* h, int* info);
+/* tokens: n x context int32 on the HOST (clip.tokenize rows) -> out: n x embed fp32 on the device, each row
+ * encode_text / ||encode_text||.  The EOT row of a prompt is its argmax id; the tower runs on L = 1 + the largest EOT
+ * position of the call rows per prompt.  An id outside the vocabulary is refused. */
+int vf_clip_text_encode(vf_clip_text_t* h, const int32_t* tokens, int n, float* out, void* stream);
+/* Diagnostics: blocks first .. first + count - 1 in place on the residual stream x, n x L x width fp32 on the device. */
+int vf_clip_text_blocks(vf_clip_text_t* h, float* x, int n, int L, int first, int count, void* stream);
+/* The causal attention alone: qkv n x L rows [q | k | v] of 3 x heads*64 fp16 -> out n x L x heads*64 fp16; L <= 77.
+ * Row i reads rows 0..i only, in an order fixed by i: its bits do not depend on L. */
+int vf_clip_text_attention(const void* qkv, int n, int L, int heads, void* out, void* stream);
+/* out[r] = x[r] / ||x[r]||_2, n rows of C fp32 on the device (out == x allowed). */
+int vf_l2_normalize_rows(const float* x, int n, int C, float* out, void* stream);
+int64_t vf_clip_text_launch_count(const vf_clip_text_t* h);
+
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),
  * and the softmax + sort of utils/utils.py:19-47.  weight: n_classes x n_features, bias: n_classes, HOST fp32. */

@@ -7,6 +7,8 @@ outside the reference's list, and the ``CLIP-ViT-L/14`` / ``CLIP-ViT-L/14@336px`
 released ViT, 768-d features), which the reference does not offer either; ``--model_name`` selects upstream's IG65M
 R(2+1)D-34 models for ``r21d_rgb``; ``swin3d_t`` / ``swin3d_s`` / ``swin3d_b`` are torchvision's Swin3D video
 transformers and ``mvit_v1_b`` / ``mvit_v2_s`` its Multiscale Vision Transformers (Kinetics-400 clip features).
+``--show_pred`` on the CLIP feature types is upstream video_features' zero-shot prediction: every frame's image feature
+against the text features of ``--pred_texts`` (default: "a photo of {name}" for the Kinetics-400 classes).
 """
 import argparse
 import functools
@@ -123,7 +125,12 @@ _FLAGS = [
                                     help='--side_size applies to the larger edge instead of the smaller one')),
     ('--side_size', dict(type=int, help='RAFT: resize frames to this edge length first')),
     ('--show_pred', dict(dest='show_pred', action='store_true', default=False,
-                         help='print the top-5 classes of every feature (I3D, R(2+1)D, S3D, Swin3D, MViT: Kinetics-400; ResNet: ImageNet)')),
+                         help='print the top-5 classes of every feature (I3D, R(2+1)D, S3D, Swin3D, MViT: Kinetics-400; ResNet: '
+                              'ImageNet; CLIP: zero-shot over --pred_texts)')),
+    ('--pred_texts', dict(nargs='+', default=None,
+                          help='CLIP --show_pred: the prompts each frame is compared with (default: "a photo of {name}" '
+                               'for the 400 Kinetics-400 classes; needs the BPE vocabulary bpe_simple_vocab_16e6.txt.gz '
+                               'in $VF_CLIP_BPE, extract/checkpoints/ or ~/.cache/clip/)')),
     # not in the reference: after extraction, ONE all-gather (NCCL over NVLink) returns every rank's feature blocks and
     # rank 0 writes them, list order, to this .npz
     ('--gather_features', dict(type=str, default=None, help='also all-gather the features of all GPUs into this .npz')),

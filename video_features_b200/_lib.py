@@ -241,6 +241,14 @@ SIGNATURES = {
     "vf_vggish_conv": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64), C.c_void_p,
                                  C.c_void_p, C.c_void_p]),
     "vf_vggish_time_register": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
+    "vf_clip_text_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
+    "vf_clip_text_destroy": (C.c_int, [C.c_void_p]),
+    "vf_clip_text_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "vf_clip_text_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_text_blocks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vf_clip_text_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_l2_normalize_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_clip_text_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_head_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "vf_head_destroy": (C.c_int, [C.c_void_p]),
     "vf_head_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -35,12 +35,13 @@ import numpy as np
 import torch
 from tqdm import tqdm
 
-from .. import synthetic_weights
+from .. import clip_tokenizer, synthetic_weights
 from ..clip_engine import ClipEngine
 from ..clip_resnet_engine import ClipResNetEngine
+from ..clip_text_engine import ZeroShotHead, check_vocabulary, text_state_dict
 from ..clip_vitl_engine import ClipViTLEngine
 from ..utils import (AsyncSink, FrameStream, action_on_extraction, already_extracted, extract_frames,
-                     form_list_from_user_input)
+                     form_list_from_user_input, print_top_predictions)
 
 # the ResNet towers' names are the basenames clip.load caches its downloads under
 _RN_CKPT_NAMES = {'CLIP-RN50': 'RN50.pt', 'CLIP-RN101': 'RN101.pt', 'CLIP-RN50x4': 'RN50x4.pt', 'CLIP-RN50x16': 'RN50x16.pt'}
@@ -48,6 +49,8 @@ _RN_CKPT_NAMES = {'CLIP-RN50': 'RN50.pt', 'CLIP-RN101': 'RN101.pt', 'CLIP-RN50x4
 _VITL_CKPT_NAMES = {'CLIP-ViT-L/14': 'ViT-L-14.pt', 'CLIP-ViT-L/14@336px': 'ViT-L-14-336px.pt'}
 _CKPT_NAMES = {'CLIP-ViT-B/32': 'ViT-B-32.pt', 'CLIP-ViT-B/16': 'ViT-B-16.pt', 'CLIP4CLIP-ViT-B-32': 'CLIP4CLIP-ViT-B-32.pth',
                **_RN_CKPT_NAMES, **_VITL_CKPT_NAMES}
+# the text towers of the synthetic ViT weights: (width, embed), as in openai's releases
+_SYNTHETIC_TEXT = {'CLIP-ViT-L/14': (768, 768), 'CLIP-ViT-L/14@336px': (768, 768)}
 
 
 def read_clip_checkpoint(path: str) -> Dict[str, torch.Tensor]:
@@ -64,16 +67,22 @@ def read_clip_checkpoint(path: str) -> Dict[str, torch.Tensor]:
     return dict(sd)
 
 
-def load_clip_state_dict(feature_type: str) -> Dict[str, torch.Tensor]:
+def load_clip_state_dict(feature_type: str, text_vocab: Optional[int] = None) -> Dict[str, torch.Tensor]:
     """``$VF_CLIP_CKPT``, then ``<this dir>/checkpoints/<name>`` (where the reference keeps CLIP4CLIP's file,
     extract_clip.py:56), then ``~/.cache/clip/<name>`` (where ``clip.load`` caches its download).
     ``VF_CLIP_SYNTHETIC=<seed>[:outliers]`` selects seeded synthetic ViT weights instead (benchmarks without the file);
-    it does not apply to the ResNet towers."""
+    it does not apply to the ResNet towers.  ``text_vocab``: the synthetic weights also carry a text tower whose token
+    embedding has this many rows (--show_pred)."""
     if os.environ.get("VF_CLIP_SYNTHETIC") is not None and feature_type not in _RN_CKPT_NAMES:
         seed, outliers = synthetic_weights.parse_env(os.environ["VF_CLIP_SYNTHETIC"])
         if feature_type in _VITL_CKPT_NAMES:
-            return synthetic_weights.clip_vit_l14_state_dict(seed, outliers, n_px=336 if feature_type.endswith('336px') else 224)
-        return synthetic_weights.clip_vit_b32_state_dict(seed, outliers, patch=16 if feature_type.endswith('/16') else 32)
+            sd = synthetic_weights.clip_vit_l14_state_dict(seed, outliers, n_px=336 if feature_type.endswith('336px') else 224)
+        else:
+            sd = synthetic_weights.clip_vit_b32_state_dict(seed, outliers, patch=16 if feature_type.endswith('/16') else 32)
+        if text_vocab is not None:
+            width, embed = _SYNTHETIC_TEXT.get(feature_type, (512, 512))
+            sd.update(synthetic_weights.clip_text_state_dict(seed, width, embed, text_vocab))
+        return sd
     name = _CKPT_NAMES[feature_type]
     cands = [os.environ.get("VF_CLIP_CKPT"), os.path.join(pathlib.Path(__file__).parent, 'checkpoints', name),
              os.path.expanduser(os.path.join("~/.cache/clip", name))]
@@ -134,6 +143,20 @@ class ExtractCLIP(torch.nn.Module):
             self.output_path = args.output_path if self.output_direct is True else os.path.join(args.output_path, self.feature_type)
         self.progress = tqdm(total=len(self.path_list))
         self._engines: Dict[int, object] = {}             # ClipEngine, ClipResNetEngine or ClipViTLEngine
+        # --show_pred: zero-shot top-5 of every frame over the prompts (default: "a photo of {name}" for the Kinetics-400
+        # classes).  Vocabulary, tokens and text weights are checked here, before any video is opened.
+        self.show_pred = getattr(args, 'show_pred', False)
+        self.pred_texts = None
+        self._zero_shot: Dict[int, ZeroShotHead] = {}
+        self._head_device = None
+        if self.show_pred:
+            if self.feature_type not in _CKPT_NAMES:
+                raise NotImplementedError(self.feature_type)
+            self.pred_texts = list(getattr(args, 'pred_texts', None) or clip_tokenizer.default_prompts())
+            tokenizer = clip_tokenizer.load()
+            self._pred_tokens = tokenizer.tokenize(self.pred_texts)
+            self._text_sd = text_state_dict(load_clip_state_dict(self.feature_type, tokenizer.vocab_size))
+            check_vocabulary(self._text_sd, tokenizer)
         # engine-side knobs (not in the reference): where frames come from, and how many go into one engine call
         self.frame_source = extract_frames                  # (path, method) -> (frames, fps, timestamps_ms)
         # two-step source used by the list path: stream = frame_stream(path, method) knows .count / .hw / .fps /
@@ -165,6 +188,9 @@ class ExtractCLIP(torch.nn.Module):
                 self._engines[idx] = ClipViTLEngine(sd, device=idx)
             else:
                 self._engines[idx] = ClipEngine(sd, device=idx)
+        if self.show_pred and idx not in self._zero_shot:
+            self._zero_shot[idx] = ZeroShotHead(self._text_sd, self._pred_tokens, idx)
+        self._head_device = torch.device('cuda', idx)
         return self._engines[idx]
 
     # ------------------------------------------------------------------ forward
@@ -210,7 +236,11 @@ class ExtractCLIP(torch.nn.Module):
         print(f'Extraction failed at: {video} with error (↑). Continuing extraction')
         traceback.print_exception(type(err), err, err.__traceback__)
 
-    def _deliver(self, feats: dict, pos: int, video, collected: dict, sink: Optional[AsyncSink]):
+    def _deliver(self, feats: dict, pos: int, video, collected: dict, sink: Optional[AsyncSink],
+                 dev: Optional[torch.Tensor] = None):
+        """``dev``: the same features still on the GPU, if the caller has them (--show_pred reads them)."""
+        if self.show_pred:
+            self._show(feats[self.feature_type], dev)
         if self.external_call or self.keep_features:
             collected[pos] = feats
         if self.external_call:
@@ -219,6 +249,13 @@ class ExtractCLIP(torch.nn.Module):
             sink.submit(feats, video, self.output_path, self.on_extraction, self.output_direct)
         else:
             action_on_extraction(feats, video, self.output_path, self.on_extraction, self.output_direct)
+
+    def _show(self, feats: np.ndarray, dev: Optional[torch.Tensor]):
+        """Print the zero-shot top-5 of every frame (``--show_pred``)."""
+        head = self._zero_shot[self._head_device.index]
+        rows = dev if dev is not None else torch.from_numpy(np.ascontiguousarray(feats)).to(self._head_device)
+        with torch.cuda.device(self._head_device):
+            print_top_predictions(*head.top_k_host(rows), 'kinetics', classes=self.pred_texts)
 
     def _decode(self, video):
         frames, fps, stamps = self.frame_source(str(video), self.extract_method)
@@ -267,11 +304,11 @@ class ExtractCLIP(torch.nn.Module):
         lock = threading.Lock()
         waits = self.stage_wait = dict.fromkeys(self.stage_wait, 0.0)
 
-        def deliver_one(pos, video, feats, fps, stamps):
+        def deliver_one(pos, video, feats, fps, stamps, dev=None):
             try:
                 with lock:
                     self._deliver({self.feature_type: feats, 'fps': np.array(fps), 'timestamps_ms': np.array(stamps)},
-                                  pos, video, collected, sink)
+                                  pos, video, collected, sink, dev)
                 ok = True
             except Exception as err:
                 self._report(err, video)
@@ -288,9 +325,10 @@ class ExtractCLIP(torch.nn.Module):
                 elif k <= 0:
                     self._report(RuntimeError(f"no frames decoded from {video}"), video)
                     self.progress.update()
-                elif deliver_one(pos, video, feats[row0:row0 + k].copy(), st.fps, st.timestamps_ms):
+                elif deliver_one(pos, video, feats[row0:row0 + k].copy(), st.fps, st.timestamps_ms,
+                                 None if dev is None else dev[row0:row0 + k]):
                     good.append((row0, k))
-            if dev is not None and good:
+            if self.keep_features and dev is not None and good:
                 # the same rows, still on the GPU, for a gather: the call's tensor as it is when every video made it
                 rows = dev[:batch.rows] if sum(k for _, k in good) == batch.rows else torch.cat([dev[a:a + k] for a, k in good])
                 with lock:
@@ -332,7 +370,7 @@ class ExtractCLIP(torch.nn.Module):
             view = pinned[batch.slot][:batch.rows * h * w * 3].view(batch.rows, h, w, 3)
             feats = feats_out[batch.slot][:batch.rows]
             try:
-                ticket, dev = model.encode_frames_u8_host_async(view, feats, out_dev=self.keep_features)
+                ticket, dev = model.encode_frames_u8_host_async(view, feats, out_dev=self.keep_features or self.show_pred)
             except Exception:
                 batch_failed(batch, counts, view)
                 return None

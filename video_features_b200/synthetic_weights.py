@@ -4,6 +4,7 @@ here).  ``VF_CLIP_SYNTHETIC=<seed>[:outliers]`` makes ``ExtractCLIP`` use them i
 """
 from __future__ import annotations
 
+import math
 from collections import OrderedDict
 
 import torch
@@ -90,6 +91,42 @@ def _vit_state_dict(seed, outliers, WIDTH, LAYERS, patch, n_px, EMBED) -> "Order
             sd[p + "attn.out_proj.weight"][loud] *= 6.0
             sd[p + "mlp.c_proj.weight"][loud] *= 6.0
         sd["visual.ln_post.weight"][dims] = 0.05
+    return sd
+
+
+def clip_text_state_dict(seed: int = 0, width: int = 512, embed: int = 512, vocab_size: int = 49408,
+                         layers: int = LAYERS, context: int = 77) -> "OrderedDict[str, torch.Tensor]":
+    """openai's text-tower keys (``token_embedding``, ``positional_embedding``, ``transformer.*``, ``ln_final``,
+    ``text_projection``, ``logit_scale`` = ln 100), fp32, for ``--show_pred`` without a checkpoint.  ``vocab_size``
+    must be the size of the BPE vocabulary the prompts are tokenized with.  Scales as openai's
+    ``initialize_parameters``, with perturbed LayerNorms as ``_vit_state_dict``."""
+    g = torch.Generator().manual_seed(seed + 1000)
+
+    def rn(*shape, std=1.0):
+        return torch.randn(*shape, generator=g, dtype=torch.float32) * std
+
+    proj_std = (width ** -0.5) * ((2 * layers) ** -0.5)
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    sd["token_embedding.weight"] = rn(vocab_size, width, std=0.02)
+    sd["positional_embedding"] = rn(context, width, std=0.01)
+    for i in range(layers):
+        p = f"transformer.resblocks.{i}."
+        sd[p + "attn.in_proj_weight"] = rn(3 * width, width, std=width ** -0.5)
+        sd[p + "attn.in_proj_bias"] = rn(3 * width, std=0.02)
+        sd[p + "attn.out_proj.weight"] = rn(width, width, std=proj_std)
+        sd[p + "attn.out_proj.bias"] = rn(width, std=0.02)
+        sd[p + "ln_1.weight"] = 1.0 + rn(width, std=0.1)
+        sd[p + "ln_1.bias"] = rn(width, std=0.05)
+        sd[p + "mlp.c_fc.weight"] = rn(4 * width, width, std=(2 * width) ** -0.5)
+        sd[p + "mlp.c_fc.bias"] = rn(4 * width, std=0.02)
+        sd[p + "mlp.c_proj.weight"] = rn(width, 4 * width, std=proj_std)
+        sd[p + "mlp.c_proj.bias"] = rn(width, std=0.02)
+        sd[p + "ln_2.weight"] = 1.0 + rn(width, std=0.1)
+        sd[p + "ln_2.bias"] = rn(width, std=0.05)
+    sd["ln_final.weight"] = 1.0 + rn(width, std=0.1)
+    sd["ln_final.bias"] = rn(width, std=0.05)
+    sd["text_projection"] = rn(width, embed, std=width ** -0.5)
+    sd["logit_scale"] = torch.tensor(math.log(100.0))
     return sd
 
 

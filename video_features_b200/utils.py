@@ -276,6 +276,12 @@ def sanity_check(args: argparse.Namespace):
         raise AssertionError(f'I3D model does not support inputs shorter than 10 timestamps. You have: {args.stack_size}')
     if getattr(args, 'model_name', None) is not None and args.feature_type != 'r21d_rgb':
         raise AssertionError(f'--model_name selects the r21d_rgb network; it does not apply to {args.feature_type}')
+    if getattr(args, 'pred_texts', None) is not None:
+        if not args.feature_type.startswith('CLIP'):
+            raise AssertionError(f'--pred_texts are zero-shot prompts of the CLIP feature types; they do not apply to '
+                                 f'{args.feature_type}')
+        if not args.show_pred:
+            raise AssertionError('--pred_texts only takes effect with --show_pred')
 
 
 def _paired(videos, flows):
