@@ -619,6 +619,41 @@ int vf_clip_text_attention(const void* qkv, int n, int L, int heads, void* out, 
 int vf_l2_normalize_rows(const float* x, int n, int C, float* out, void* stream);
 int64_t vf_clip_text_launch_count(const vf_clip_text_t* h);
 
+/* ---- DINOv2 frame features: `torch.hub.load('facebookresearch/dinov2', name)(x)` at 224 px, the class token after the
+ * final norm, for dinov2_vit{s,b,l,g}14 and their _reg variants.  Weights: the hub checkpoint's tensors by key, HOST
+ * fp32, plus "pos_embed_224", the (257, D) positional table the hub interpolates for a 224-px input
+ * (video_features_b200/dinov2_engine.py pos_table_224 computes it).  The shape is read from the weights: width from cls_token, depth from the blocks.{i} keys,
+ * heads = width / 64, SwiGLU when blocks.0.mlp.w12.weight is present, registers when register_tokens is.  Exactly
+ * (384, 12), (768, 12), (1024, 24) and (1536, 40, SwiGLU) are built; anything else is refused naming the key. */
+typedef struct vf_dinov2 vf_dinov2_t;
+
+/* Workspace of max_frames frames (0 = a default that keeps it near 2.5 GB); a call runs in chunks. */
+int vf_dinov2_create(vf_dinov2_t** out, const vf_named_tensor* tensors, int n_tensors, int device, int max_frames);
+int vf_dinov2_destroy(vf_dinov2_t* h);
+/* info receives 7 ints: width D, depth, heads, tokens (257 or 261), registers, FFN kind (0 GELU MLP, 1 SwiGLU),
+ * max_frames. */
+int vf_dinov2_info(const vf_dinov2_t* h, int* info);
+/* frames: n x 3 x 224 x 224 fp32 on the device, already transformed -> out: n x D fp32. */
+int vf_dinov2_encode_f32(vf_dinov2_t* h, const float* frames, int n, float* out, void* stream);
+/* transform fused: frames n x H x W x 3 uint8 BGR on the device, any size -> Resize(256, bicubic, Pillow-exact),
+ * CenterCrop(224), BGR->RGB, ToTensor, Normalize (ImageNet) -> network.  Bit-identical to vf_dinov2_encode_f32 on the
+ * same transformed frames. */
+int vf_dinov2_encode_u8(vf_dinov2_t* h, const uint8_t* frames, int n, int H, int W, float* out, void* stream);
+/* Diagnostics, eagerly on the caller's stream, n <= max_frames: the embedding (token assembly) -> x_out n x tokens x D
+ * fp32; blocks [layer_begin, layer_end) in place on x (the last block updates the class rows only); the final norm of
+ * the class rows of x -> out n x D. */
+int vf_dinov2_debug_embed_f32(vf_dinov2_t* h, const float* frames, int n, float* x_out, void* stream);
+int vf_dinov2_debug_embed_u8(vf_dinov2_t* h, const uint8_t* frames, int n, int H, int W, float* x_out, void* stream);
+int vf_dinov2_debug_blocks(vf_dinov2_t* h, float* x, int n, int layer_begin, int layer_end, void* stream);
+int vf_dinov2_debug_head(vf_dinov2_t* h, const float* x, int n, float* out, void* stream);
+/* The SwiGLU kernel alone: ab rows x 2 hidden fp32 ([a | b], the w12 output) -> out rows x hidden fp16,
+ * silu(a) * b in fp32 rounded once. */
+int vf_dinov2_swiglu(const float* ab, int rows, int hidden, void* out, void* stream);
+/* The attention the blocks use alone: qkv n x S rows [q | k | v] of 3 x heads*64 fp16 -> out n x S x heads*64 fp16,
+ * scale 1/8, no mask, S <= 577. */
+int vf_dinov2_attention(const void* qkv, int n, int S, int heads, void* out, void* stream);
+int64_t vf_dinov2_launch_count(const vf_dinov2_t* h);
+
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),
  * and the softmax + sort of utils/utils.py:19-47.  weight: n_classes x n_features, bias: n_classes, HOST fp32. */

@@ -6,7 +6,9 @@ feature type (torchvision's S3D, the Kinetics-400 clip feature upstream video_fe
 outside the reference's list, and the ``CLIP-ViT-L/14`` / ``CLIP-ViT-L/14@336px`` feature types (openai's largest
 released ViT, 768-d features), which the reference does not offer either; ``--model_name`` selects upstream's IG65M
 R(2+1)D-34 models for ``r21d_rgb``; ``swin3d_t`` / ``swin3d_s`` / ``swin3d_b`` are torchvision's Swin3D video
-transformers and ``mvit_v1_b`` / ``mvit_v2_s`` its Multiscale Vision Transformers (Kinetics-400 clip features).
+transformers and ``mvit_v1_b`` / ``mvit_v2_s`` its Multiscale Vision Transformers (Kinetics-400 clip features);
+``dinov2_vit{s,b,l,g}14`` and their ``_reg`` variants are DINOv2's self-supervised ViTs (per-frame features, the hub
+model's class token after its final norm).
 ``--show_pred`` on the CLIP feature types is upstream video_features' zero-shot prediction: every frame's image feature
 against the text features of ``--pred_texts`` (default: "a photo of {name}" for the Kinetics-400 classes).
 """
@@ -20,7 +22,9 @@ from video_features_b200.utils import form_list_from_user_input, sanity_check
 
 SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-ViT-B-32', 'resnet18', 'resnet34', 'resnet50',
              'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch', 's3d', 'CLIP-ViT-L/14', 'CLIP-ViT-L/14@336px',
-             'swin3d_t', 'swin3d_s', 'swin3d_b', 'mvit_v1_b', 'mvit_v2_s']
+             'swin3d_t', 'swin3d_s', 'swin3d_b', 'mvit_v1_b', 'mvit_v2_s', 'dinov2_vits14', 'dinov2_vitb14',
+             'dinov2_vitl14', 'dinov2_vitg14', 'dinov2_vits14_reg', 'dinov2_vitb14_reg', 'dinov2_vitl14_reg',
+             'dinov2_vitg14_reg']
 
 
 def build_extractor(args):
@@ -52,6 +56,9 @@ def build_extractor(args):
     if args.feature_type in ['mvit_v1_b', 'mvit_v2_s']:
         from video_features_b200.extract.extract_mvit import ExtractMViT
         return ExtractMViT(args)
+    if args.feature_type.startswith('dinov2_'):
+        from video_features_b200.extract.extract_dinov2 import ExtractDINOv2
+        return ExtractDINOv2(args)
     if args.feature_type == 'vggish_torch':
         from video_features_b200.extract.extract_vggish import ExtractVGGish
         return ExtractVGGish(args)
@@ -91,7 +98,9 @@ def parallel_feature_extraction(args):
 
 
 _FEATURE_TYPES = ('i3d vggish r21d_rgb resnet18 resnet34 resnet50 resnet101 resnet152 raft pwc CLIP-ViT-B/32 CLIP-ViT-B/16 '
-                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d CLIP-ViT-L/14 CLIP-ViT-L/14@336px swin3d_t swin3d_s swin3d_b mvit_v1_b mvit_v2_s').split()
+                  'CLIP4CLIP-ViT-B-32 vggish_torch s3d CLIP-ViT-L/14 CLIP-ViT-L/14@336px swin3d_t swin3d_s swin3d_b mvit_v1_b mvit_v2_s '
+                  'dinov2_vits14 dinov2_vitb14 dinov2_vitl14 dinov2_vitg14 dinov2_vits14_reg dinov2_vitb14_reg '
+                  'dinov2_vitl14_reg dinov2_vitg14_reg').split()
 
 # (flag, argparse keywords): names, types, defaults, choices and dests are the reference's (main.py:93-149)
 _FLAGS = [
@@ -126,7 +135,8 @@ _FLAGS = [
     ('--side_size', dict(type=int, help='RAFT: resize frames to this edge length first')),
     ('--show_pred', dict(dest='show_pred', action='store_true', default=False,
                          help='print the top-5 classes of every feature (I3D, R(2+1)D, S3D, Swin3D, MViT: Kinetics-400; ResNet: '
-                              'ImageNet; CLIP: zero-shot over --pred_texts)')),
+                              'ImageNet; CLIP: zero-shot over --pred_texts; not DINOv2, whose checkpoints have no '
+                              'classifier)')),
     ('--pred_texts', dict(nargs='+', default=None,
                           help='CLIP --show_pred: the prompts each frame is compared with (default: "a photo of {name}" '
                                'for the 400 Kinetics-400 classes; needs the BPE vocabulary bpe_simple_vocab_16e6.txt.gz '

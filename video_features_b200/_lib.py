@@ -249,6 +249,18 @@ SIGNATURES = {
     "vf_clip_text_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_l2_normalize_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_clip_text_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_dinov2_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.c_int, C.c_int]),
+    "vf_dinov2_destroy": (C.c_int, [C.c_void_p]),
+    "vf_dinov2_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "vf_dinov2_encode_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_encode_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_debug_embed_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_debug_embed_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_debug_blocks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vf_dinov2_debug_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_swiglu": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_dinov2_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_head_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "vf_head_destroy": (C.c_int, [C.c_void_p]),
     "vf_head_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -269,6 +269,11 @@ def sanity_check(args: argparse.Namespace):
     """utils/utils.py:129-150 (the checks that concern CLIP / I3D / RAFT)."""
     if os.path.relpath(args.output_path) == os.path.relpath(args.tmp_path):
         raise AssertionError('The same path for out & tmp')
+    if args.feature_type.startswith('dinov2_'):
+        if args.show_pred:
+            raise AssertionError(f'--show_pred: the {args.feature_type} checkpoint is a backbone without a classifier')
+        if args.stack_size is not None:
+            raise AssertionError(f'--stack_size: {args.feature_type} gives one feature per frame; stacks do not apply')
     if args.show_pred:
         print('--show_pred: only the first of the listed GPUs is used')
         args.device_ids = args.device_ids[:1]
