@@ -10,7 +10,6 @@
 #include <string.h>
 
 #include <atomic>
-#include <map>
 #include <vector>
 
 #include "internal.h"
@@ -42,9 +41,10 @@ struct vf_clip : vf::EngineCore {
     __half *patches = nullptr, *h = nullptr, *qkv = nullptr, *att = nullptr, *mlp = nullptr, *cls = nullptr;
     float *x = nullptr, *emb = nullptr;   // residual stream (fp32), patch embeddings (fp32)
     __half* y = nullptr;                  // residual-branch increment written by out-proj / fc2 (fp16)
-    // transform scratch (grown on demand)
-    uint8_t *stage_u8 = nullptr, *resized = nullptr, *resize_tmp = nullptr;
-    size_t stage_cap = 0, resized_cap = 0, tmp_cap = 0;
+    float* feat = nullptr;                // [chunk, 512] tower output
+    // host-buffer entries: two staging slots of frames (grown on demand)
+    uint8_t* stage_u8 = nullptr;
+    size_t stage_cap = 0;
     size_t stage_fbytes = 0;      // frame size the two staging slots were last laid out for
     float* out_dev = nullptr;
     size_t out_cap = 0;
@@ -55,28 +55,12 @@ struct vf_clip : vf::EngineCore {
     double prof_cat_ms[4] = {0, 0, 0, 0};
     size_t prof_used = 0;
     double prof_flops = 0.0;
-    // All work of a call runs on the engine's own compute stream `cs` (ordered against the caller's stream with a
-    // pair of events), so that the per-chunk tower can be captured once into a CUDA graph and replayed: ~90 kernel
-    // launches and ~150 tensor-map encodes per chunk collapse into one cudaGraphLaunch (the legacy NULL stream, which
-    // is what torch hands over by default, cannot be captured).
-    //
-    // Two LANES (stream + private workspace) take the chunks of a call alternately.  A GEMM owns every SM's shared
-    // memory, so GEMMs of the two lanes serialise, but the memory-bound kernels of one lane (LayerNorm, attention,
-    // transform: no shared memory to speak of) co-reside with the tensor-bound GEMM of the other and fill its tails.
-    struct Lane {
-        __half *patches = nullptr, *h = nullptr, *qkv = nullptr, *att = nullptr, *mlp = nullptr, *cls = nullptr, *y = nullptr;
-        float *x = nullptr, *emb = nullptr, *feat = nullptr;
-        uint8_t *resized = nullptr, *resize_tmp = nullptr;
-        size_t resized_cap = 0, tmp_cap = 0;
-        cudaStream_t cs = nullptr;
-        cudaEvent_t ev_out = nullptr;
-        std::map<int, vf::CachedGraph> graphs;   // frames in chunk -> instantiated tower graph (writes feat)
-        std::map<int, int> seen;                 // frames in chunk -> times this size has been run without a graph
-    } lanes[2];
-    int n_lanes = 2, cur = 0;                 // the lane streams stand in for EngineCore::cs, which stays null
+    // All work of a call runs on the engine stream `cs` (ordered against the caller's stream with a pair of events), so
+    // that the per-chunk tower can be captured once into a CUDA graph and replayed: ~90 kernel launches and ~150
+    // tensor-map encodes per chunk collapse into one cudaGraphLaunch (the legacy NULL stream, which is what torch hands
+    // over by default, cannot be captured).
     bool acc_o = true, acc_m = true;          // residual adds in the GEMM epilogue (fp32 reductions) instead of an fp16 y
     bool fused_attn = true;                   // QKV projection + attention in one kernel (VF_CLIP_ATTN=split: GEMM + kernel)
-    float* feat = nullptr;                    // [chunk, 512] tower output of the active lane
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_copy[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
     // asynchronous host calls (vf_clip_encode_u8_host_async): completion events of the last kTickets calls
@@ -86,45 +70,6 @@ struct vf_clip : vf::EngineCore {
 };
 
 namespace vf {
-
-static int upload_f32(vf_clip* h, float** dst, const float* src, size_t count) {
-    if (!src) return fail(VF_ERR_INVALID, "clip_create: missing weight tensor");
-    VF_TRY(ralloc(h, dst, count));
-    VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-// fp32 host [rows, cols] (optionally transposed on the way) -> fp16 device, round-to-nearest-even
-static int upload_f16(vf_clip* h, __half** dst, const float* src, size_t rows, size_t cols, bool transpose) {
-    if (!src) return fail(VF_ERR_INVALID, "clip_create: missing weight tensor");
-    std::vector<__half> tmp(rows * cols);
-    if (!transpose) {
-        for (size_t i = 0; i < rows * cols; ++i) tmp[i] = __float2half_rn(src[i]);
-    } else {   // src is [rows, cols]; produce [cols, rows]
-        for (size_t r = 0; r < rows; ++r)
-            for (size_t c = 0; c < cols; ++c) tmp[c * rows + r] = __float2half_rn(src[r * cols + c]);
-    }
-    VF_TRY(ralloc(h, dst, rows * cols));
-    VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-
-static int grow(uint8_t** p, size_t* cap, size_t need) {
-    if (need <= *cap) return VF_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), need);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "cudaMalloc(%zu bytes): %s", need, cudaGetErrorString(e));
-    *cap = need;
-    return VF_OK;
-}
-
-static GemmEpi epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate = 0) {
-    GemmEpi e;
-    memset(&e, 0, sizeof(e));
-    e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.bias = bias; e.act = act; e.accumulate = accumulate;
-    return e;
-}
 
 // event bracket around one launch when profiling is on (vf_clip_profile): category 0 gemm, 1 layernorm,
 // 2 attention, 3 transform
@@ -183,7 +128,7 @@ static int tower_attention(vf_clip* h, int c, cudaStream_t s) {
 static int tower_embed(vf_clip* h, int c, cudaStream_t s) {
     const int P = h->P, PK = h->PK;
     // patch embedding: [c*P, PK] x [768, PK]^T -> emb (fp32)
-    VF_TRY(tower_gemm(h, h->patches, PK, h->w_patch, PK, c * P, W, PK, epi(h->emb, W, 1, nullptr, VF_ACT_NONE), s));
+    VF_TRY(tower_gemm(h, h->patches, PK, h->w_patch, PK, c * P, W, PK, linear_epi(h->emb, W, 1, nullptr, VF_ACT_NONE), s));
     // token assembly (+ class / positional embedding) fused with ln_pre -> x
     VF_TRY(tower_embed_ln(h, c, s));
     h->launches += 2;
@@ -207,7 +152,7 @@ static int tower_blocks(vf_clip* h, int c, int l0, int l1, cudaStream_t s) {
         if (h->fused_attn) {
             VF_TRY(tower_qkv_attention(h, w, c, s));
         } else {
-            VF_TRY(tower_gemm(h, h->h, W, w.w_qkv, W, M, 3 * W, W, epi(h->qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
+            VF_TRY(tower_gemm(h, h->h, W, w.w_qkv, W, M, 3 * W, W, linear_epi(h->qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
             VF_TRY(tower_attention(h, c, s));
         }
         // Last block: only the CLS token reaches ln_post / proj (encode_image returns x[:, 0]), so after the attention
@@ -217,15 +162,15 @@ static int tower_blocks(vf_clip* h, int c, int l0, int l1, cudaStream_t s) {
         const int rows = last ? c : M;
         const int a_ld = last ? T * W : W;                    // row pitch of att / x when only the CLS rows are read
         if (acc_o) {
-            VF_TRY(tower_gemm(h, h->att, a_ld, w.w_o, W, rows, W, W, epi(h->x, a_ld, 1, w.b_o, VF_ACT_NONE, 1), s));
+            VF_TRY(tower_gemm(h, h->att, a_ld, w.w_o, W, rows, W, W, linear_epi(h->x, a_ld, 1, w.b_o, VF_ACT_NONE, 1), s));
             VF_TRY(tower_add_ln(h, h->x, a_ld, nullptr, W, 0, w.ln2_w, w.ln2_b, h->h, W, rows, s));
         } else {
-            VF_TRY(tower_gemm(h, h->att, a_ld, w.w_o, W, rows, W, W, epi(h->y, W, 0, w.b_o, VF_ACT_NONE), s));
+            VF_TRY(tower_gemm(h, h->att, a_ld, w.w_o, W, rows, W, W, linear_epi(h->y, W, 0, w.b_o, VF_ACT_NONE), s));
             VF_TRY(tower_add_ln(h, h->x, a_ld, h->y, W, 1, w.ln2_w, w.ln2_b, h->h, W, rows, s));
         }
-        VF_TRY(tower_gemm(h, h->h, W, w.w_fc, W, rows, MLPW, W, epi(h->mlp, MLPW, 0, w.b_fc, VF_ACT_QUICKGELU), s));
-        if (acc_m) VF_TRY(tower_gemm(h, h->mlp, MLPW, w.w_proj, MLPW, rows, W, MLPW, epi(h->x, a_ld, 1, w.b_proj, VF_ACT_NONE, 1), s));
-        else       VF_TRY(tower_gemm(h, h->mlp, MLPW, w.w_proj, MLPW, rows, W, MLPW, epi(h->y, W, 0, w.b_proj, VF_ACT_NONE), s));
+        VF_TRY(tower_gemm(h, h->h, W, w.w_fc, W, rows, MLPW, W, linear_epi(h->mlp, MLPW, 0, w.b_fc, VF_ACT_QUICKGELU), s));
+        if (acc_m) VF_TRY(tower_gemm(h, h->mlp, MLPW, w.w_proj, MLPW, rows, W, MLPW, linear_epi(h->x, a_ld, 1, w.b_proj, VF_ACT_NONE, 1), s));
+        else       VF_TRY(tower_gemm(h, h->mlp, MLPW, w.w_proj, MLPW, rows, W, MLPW, linear_epi(h->y, W, 0, w.b_proj, VF_ACT_NONE), s));
         h->launches += h->fused_attn ? 6 : 7;
     }
     return VF_OK;
@@ -235,7 +180,7 @@ static int tower_blocks(vf_clip* h, int c, int l0, int l1, cudaStream_t s) {
 // the 768 -> 512 projection -> out (c x 512 fp32)
 static int tower_head(vf_clip* h, int c, const __half* y, float* out, cudaStream_t s) {
     VF_TRY(tower_add_ln(h, h->x, int64_t(h->T) * W, y, W, 0, h->lnpost_w, h->lnpost_b, h->cls, W, c, s));
-    VF_TRY(tower_gemm(h, h->cls, W, h->w_proj, W, c, E, W, epi(out, E, 1, nullptr, VF_ACT_NONE), s));
+    VF_TRY(tower_gemm(h, h->cls, W, h->w_proj, W, c, E, W, linear_epi(out, E, 1, nullptr, VF_ACT_NONE), s));
     h->launches += 2;
     return VF_OK;
 }
@@ -247,99 +192,25 @@ static int clip_tower_eager(vf_clip* h, int c, float* out, cudaStream_t s) {
     return tower_head(h, c, h->acc_m ? nullptr : h->y, out, s);
 }
 
-constexpr size_t kMaxTowerGraphs = 32;    // per lane; further sizes run eagerly
-
-// Tower on one chunk: replay (capturing on first use) the CUDA graph for this chunk size, then copy the features out.
-static int clip_tower_chunk(vf_clip* h, int c, float* out, cudaStream_t s) {
-    if (!h->use_graph || h->prof) return clip_tower_eager(h, c, out, s);
-    auto& graphs = h->lanes[h->cur].graphs;
-    auto it = graphs.find(c);
-    if (it == graphs.end()) {
-        // A chunk size is captured the SECOND time it shows up: one-off sizes (the ragged tail of a list, batches of
-        // videos of unequal length) run eagerly instead of paying capture + instantiation for a graph that is never
-        // replayed, and the cache stays bounded.
-        auto& seen = h->lanes[h->cur].seen;
-        if (seen.size() > 4096) seen.clear();
-        if (++seen[c] < 2 || graphs.size() >= kMaxTowerGraphs) return clip_tower_eager(h, c, out, s);
-        CachedGraph g;
-        VF_TRY(capture_graph(h, s, [&] { return clip_tower_eager(h, c, h->feat, s); }, &g));
-        it = graphs.emplace(c, g).first;
-    }
-    VF_CUDA(cudaGraphLaunch(it->second.exec, s));
-    VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(c) * E * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    h->launches += it->second.launches;
-    return VF_OK;
-}
-
-// frames per chunk for a batch of n: as few chunks as the workspace allows, all (nearly) the same size, so no
-// ragged tail chunk runs the 12-layer launch sequence on a handful of rows
-static int balanced_chunk(const vf_clip* h, int n) {
-    const int nchunks = (n + h->chunk - 1) / h->chunk;
-    return nchunks > 0 ? (n + nchunks - 1) / nchunks : h->chunk;
-}
-
-// make lane `l` the active one: its workspace pointers and stream become the ones the launch helpers use
-static cudaStream_t activate(vf_clip* h, int l) {
-    vf_clip::Lane& L = h->lanes[l];
-    h->cur = l;
-    h->patches = L.patches; h->h = L.h; h->qkv = L.qkv; h->att = L.att; h->mlp = L.mlp; h->cls = L.cls; h->y = L.y;
-    h->x = L.x; h->emb = L.emb; h->feat = L.feat;
-    h->resized = L.resized; h->resize_tmp = L.resize_tmp; h->resized_cap = L.resized_cap; h->tmp_cap = L.tmp_cap;
-    return L.cs;
-}
-static void deactivate(vf_clip* h) {      // keep the (possibly grown) resize scratch with its lane
-    vf_clip::Lane& L = h->lanes[h->cur];
-    L.resized = h->resized; L.resize_tmp = h->resize_tmp; L.resized_cap = h->resized_cap; L.tmp_cap = h->tmp_cap;
-}
-// keeps a lane's (possibly re-allocated) resize scratch with the lane on EVERY exit path of a chunk, early error returns
-// included: a lane left holding pointers that grow() has already freed would be a use-after-free on the next call
-struct LaneScope {
-    vf_clip* h;
-    cudaStream_t s;
-    LaneScope(vf_clip* h_, int l) : h(h_), s(activate(h_, l)) {}
-    ~LaneScope() { deactivate(h); }
-};
-// order the lane streams after the caller's stream (enter) and the caller's stream after the lanes (leave)
-static int enter(vf_clip* h, cudaStream_t user) {
-    VF_CUDA(cudaSetDevice(h->device));
-    VF_CUDA(cudaEventRecord(h->ev_in, user));
-    for (int l = 0; l < h->n_lanes; ++l) VF_CUDA(cudaStreamWaitEvent(h->lanes[l].cs, h->ev_in, 0));
-    return VF_OK;
-}
-static int leave(vf_clip* h, cudaStream_t user) {
-    for (int l = 0; l < h->n_lanes; ++l) {
-        VF_CUDA(cudaEventRecord(h->lanes[l].ev_out, h->lanes[l].cs));
-        VF_CUDA(cudaStreamWaitEvent(user, h->lanes[l].ev_out, 0));
-    }
-    return VF_OK;
-}
-
-// transform geometry of the CLIP preprocess for a (src_h, src_w) frame
-struct ClipGeom { int rh, rw, cy, cx; bool resize; };
-static int clip_geometry(int src_h, int src_w, ClipGeom* g) {
-    if (src_h <= 0 || src_w <= 0) return fail(VF_ERR_INVALID, "clip: bad frame geometry %dx%d", src_h, src_w);
-    VF_TRY(vf_resize_geometry(src_h, src_w, 224, 1, &g->rh, &g->rw));
-    g->resize = (g->rh != src_h) || (g->rw != src_w);
-    g->cy = center_crop_offset(g->rh, 224);
-    g->cx = center_crop_offset(g->rw, 224);
-    return VF_OK;
-}
-
 // device uint8 frames (c of them, original geometry) -> h->patches
-static int clip_transform_chunk(vf_clip* h, const uint8_t* frames, int c, int src_h, int src_w, const ClipGeom& g,
+static int clip_transform_chunk(vf_clip* h, const uint8_t* frames, int c, int src_h, int src_w, const FrameGeom& g,
                                 cudaStream_t s) {
     ProfScope p(h, 3, s);
-    const uint8_t* cur = frames;
-    int ch = src_h, cw = src_w;
-    if (g.resize) {
-        VF_TRY(grow(&h->resized, &h->resized_cap, size_t(h->chunk) * g.rh * g.rw * 3));
-        VF_TRY(grow(&h->resize_tmp, &h->tmp_cap, size_t(h->chunk) * src_h * g.rw * 3));
-        VF_TRY(resize_u8(frames, c, src_h, src_w, h->resized, g.rh, g.rw, VF_FILTER_BICUBIC, h->resize_tmp, s));
-        h->launches += (g.rh != src_h) + (g.rw != src_w);
-        cur = h->resized; ch = g.rh; cw = g.rw;
-    }
-    VF_TRY(launch_clip_patchify(cur, c, ch, cw, g.cy, g.cx, h->patches, h->patch, s));
+    const uint8_t* src;
+    VF_TRY(resize_frames(h, frames, c, src_h, src_w, g, h->chunk, s, &src));
+    VF_TRY(launch_clip_patchify(src, c, g.rh, g.rw, g.cy, g.cx, h->patches, h->patch, s));
     h->launches += 1;
+    return VF_OK;
+}
+
+// The tower on one chunk whose patch matrix is in h->patches -> out (c x 512): through the graph cache (a chunk size is
+// captured the second time it shows up, so one-off sizes -- the ragged tail of a list, batches of videos of unequal
+// length -- run eagerly instead of paying capture + instantiation for a graph that is never replayed), eagerly while
+// profiling (vf_clip_profile brackets launches with events).
+static int clip_tower_run(vf_clip* h, int c, float* out) {
+    auto tower = [&] { return clip_tower_eager(h, c, h->feat, h->cs); };
+    VF_TRY(h->prof ? tower() : run_graphed(h, {c, 0, 0, 0}, tower));
+    VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(c) * E * sizeof(float), cudaMemcpyDeviceToDevice, h->cs));
     return VF_OK;
 }
 
@@ -369,6 +240,9 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
     h->who = "clip_create";
     h->device = device;
     h->chunk = chunk_frames;
+    h->capture_after = 2;            // one-off chunk sizes run eagerly
+    h->max_graphs = 32;
+    h->evict_when_full = false;
     h->patch = patch_size;
     h->P = (224 / patch_size) * (224 / patch_size);
     h->T = h->P + 1;
@@ -376,8 +250,8 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
     const int T = h->T, P = h->P, PK = h->PK;
     int st = VF_OK;
     auto body = [&]() -> int {
-        VF_TRY(upload_f16(h, &h->w_patch, w->conv1_w, W, PK, false));
-        VF_TRY(upload_f16(h, &h->w_proj, w->proj, W, E, true));
+        VF_TRY(upload_f16(h, &h->w_patch, w->conv1_w, W, PK));
+        VF_TRY(upload_f16(h, &h->w_proj, w->proj, E, W, W, true));
         VF_TRY(upload_f32(h, &h->pos, w->positional_embedding, size_t(T) * W));
         if (!w->class_embedding) return fail(VF_ERR_INVALID, "clip_create: missing class_embedding");
         {
@@ -400,7 +274,7 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
             VF_TRY(upload_f32(h, &d.b_o, s.out_proj_b, W));
             VF_TRY(upload_f32(h, &d.b_fc, s.c_fc_b, MLPW));
             VF_TRY(upload_f32(h, &d.b_proj, s.c_proj_b, W));
-            VF_TRY(upload_f16(h, &d.w_qkv, s.in_proj_w, 3 * W, W, false));
+            VF_TRY(upload_f16(h, &d.w_qkv, s.in_proj_w, 3 * W, W));
             {
                 if (!s.in_proj_w || !s.in_proj_b) return fail(VF_ERR_INVALID, "clip_create: missing weight tensor");
                 std::vector<float> wp(size_t(3) * W * W), bp(3 * W);
@@ -411,36 +285,25 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
                             memcpy(&wp[dst * W], &s.in_proj_w[src * W], W * sizeof(float));
                             bp[dst] = s.in_proj_b[src];
                         }
-                VF_TRY(upload_f16(h, &d.w_qkv_heads, wp.data(), 3 * W, W, false));
+                VF_TRY(upload_f16(h, &d.w_qkv_heads, wp.data(), 3 * W, W));
                 VF_TRY(upload_f32(h, &d.b_qkv_heads, bp.data(), 3 * W));
             }
-            VF_TRY(upload_f16(h, &d.w_o, s.out_proj_w, W, W, false));
-            VF_TRY(upload_f16(h, &d.w_fc, s.c_fc_w, MLPW, W, false));
-            VF_TRY(upload_f16(h, &d.w_proj, s.c_proj_w, W, MLPW, false));
+            VF_TRY(upload_f16(h, &d.w_o, s.out_proj_w, W, W));
+            VF_TRY(upload_f16(h, &d.w_fc, s.c_fc_w, MLPW, W));
+            VF_TRY(upload_f16(h, &d.w_proj, s.c_proj_w, W, MLPW));
         }
         const size_t C = size_t(chunk_frames);
-        {
-            // the persistent GEMM leaves no room for co-resident blocks, so one lane is the default and the second is
-            // opt-in for experiments
-            const char* e = getenv("VF_CLIP_LANES");
-            h->n_lanes = (e && e[0] == '2') ? 2 : 1;
-        }
-        for (int l = 0; l < h->n_lanes; ++l) {
-            vf_clip::Lane& L = h->lanes[l];
-            VF_TRY(ralloc(h, &L.patches, C * P * PK));
-            VF_TRY(ralloc(h, &L.x, C * T * W));
-            VF_TRY(ralloc(h, &L.y, C * T * W));
-            VF_TRY(ralloc(h, &L.emb, C * P * W));
-            VF_TRY(ralloc(h, &L.h, C * T * W));
-            VF_TRY(ralloc(h, &L.qkv, C * T * 3 * W));
-            VF_TRY(ralloc(h, &L.att, C * T * W));
-            VF_TRY(ralloc(h, &L.mlp, C * T * MLPW));
-            VF_TRY(ralloc(h, &L.cls, C * W));
-            VF_TRY(ralloc(h, &L.feat, C * E));
-            VF_CUDA(cudaStreamCreateWithFlags(&L.cs, cudaStreamNonBlocking));
-            VF_CUDA(cudaEventCreateWithFlags(&L.ev_out, cudaEventDisableTiming));
-        }
-        VF_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
+        VF_TRY(ralloc(h, &h->patches, C * P * PK));
+        VF_TRY(ralloc(h, &h->x, C * T * W));
+        VF_TRY(ralloc(h, &h->y, C * T * W));
+        VF_TRY(ralloc(h, &h->emb, C * P * W));
+        VF_TRY(ralloc(h, &h->h, C * T * W));
+        VF_TRY(ralloc(h, &h->qkv, C * T * 3 * W));
+        VF_TRY(ralloc(h, &h->att, C * T * W));
+        VF_TRY(ralloc(h, &h->mlp, C * T * MLPW));
+        VF_TRY(ralloc(h, &h->cls, C * W));
+        VF_TRY(ralloc(h, &h->feat, C * E));
+        VF_TRY(open_stream(h));
         {
             const char* r = getenv("VF_CLIP_RESID");     // acc (default) | y | mix (reduction for the MLP only)
             h->acc_o = !(r && (r[0] == 'y' || r[0] == 'm'));
@@ -448,7 +311,6 @@ int vf_clip_create_vit(vf_clip_t** out, const vf_clip_weights* w, int device, in
             const char* a = getenv("VF_CLIP_ATTN");
             h->fused_attn = !(a && a[0] == 's') && T == 50;     // the fused kernel is built for 50-token frames
         }
-        activate(h, 0);
         VF_CUDA(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
             VF_CUDA(cudaEventCreateWithFlags(&h->ev_copy[i], cudaEventDisableTiming));
@@ -470,16 +332,6 @@ int vf_clip_destroy(vf_clip_t* h) {
     if (h->stage_u8) cudaFree(h->stage_u8);
     if (h->out_dev) cudaFree(h->out_dev);
     for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
-    deactivate(h);
-    for (int l = 0; l < 2; ++l) {
-        vf_clip::Lane& L = h->lanes[l];
-        for (auto& kv : L.graphs) cudaGraphExecDestroy(kv.second.exec);
-        if (L.cs) cudaStreamDestroy(L.cs);
-        if (L.ev_out) cudaEventDestroy(L.ev_out);
-        if (L.resized) cudaFree(L.resized);
-        if (L.resize_tmp) cudaFree(L.resize_tmp);
-    }
-    h->resized = nullptr; h->resize_tmp = nullptr;
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
     for (int i = 0; i < 2; ++i) {
         if (h->ev_copy[i]) cudaEventDestroy(h->ev_copy[i]);
@@ -496,14 +348,12 @@ int vf_clip_encode_f32(vf_clip_t* h, const float* frames, int n, float* out, voi
     if (n <= 0) return VF_OK;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
     VF_TRY(enter(h, user));
-    const int step = balanced_chunk(h, n);
-    for (int b0 = 0, i = 0; b0 < n; b0 += step, ++i) {
+    const int step = balanced_step(n, h->chunk);
+    for (int b0 = 0; b0 < n; b0 += step) {
         const int c = (n - b0 < step) ? (n - b0) : step;
-        LaneScope lane(h, i % h->n_lanes);
-        cudaStream_t s = lane.s;
-        VF_TRY(launch_clip_patchify_f32(frames + size_t(b0) * 3 * 224 * 224, c, h->patches, h->patch, s));
+        VF_TRY(launch_clip_patchify_f32(frames + size_t(b0) * 3 * 224 * 224, c, h->patches, h->patch, h->cs));
         h->launches += 1;
-        VF_TRY(clip_tower_chunk(h, c, out + size_t(b0) * E, s));
+        VF_TRY(clip_tower_run(h, c, out + size_t(b0) * E));
     }
     return leave(h, user);
 }
@@ -512,17 +362,15 @@ int vf_clip_encode_u8(vf_clip_t* h, const uint8_t* frames, int n, int src_h, int
     if (!h || (n > 0 && (!frames || !out))) return fail(VF_ERR_INVALID, "clip_encode_u8: null argument");
     if (n <= 0) return VF_OK;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
-    ClipGeom g;
-    VF_TRY(clip_geometry(src_h, src_w, &g));
+    FrameGeom g;
+    VF_TRY(frame_geometry("clip", src_h, src_w, 224, 224, &g));
     VF_TRY(enter(h, user));
     const size_t fbytes = size_t(src_h) * src_w * 3;
-    const int step = balanced_chunk(h, n);
-    for (int b0 = 0, i = 0; b0 < n; b0 += step, ++i) {
+    const int step = balanced_step(n, h->chunk);
+    for (int b0 = 0; b0 < n; b0 += step) {
         const int c = (n - b0 < step) ? (n - b0) : step;
-        LaneScope lane(h, i % h->n_lanes);
-        cudaStream_t s = lane.s;
-        VF_TRY(clip_transform_chunk(h, frames + size_t(b0) * fbytes, c, src_h, src_w, g, s));
-        VF_TRY(clip_tower_chunk(h, c, out + size_t(b0) * E, s));
+        VF_TRY(clip_transform_chunk(h, frames + size_t(b0) * fbytes, c, src_h, src_w, g, h->cs));
+        VF_TRY(clip_tower_run(h, c, out + size_t(b0) * E));
     }
     return leave(h, user);
 }
@@ -540,13 +388,13 @@ static int clip_encode_u8_host(vf_clip_t* h, const uint8_t* frames_host, int n, 
         return VF_OK;
     }
     cudaStream_t user = static_cast<cudaStream_t>(stream);
-    ClipGeom g;
-    VF_TRY(clip_geometry(src_h, src_w, &g));
+    FrameGeom g;
+    VF_TRY(frame_geometry("clip", src_h, src_w, 224, 224, &g));
     VF_TRY(enter(h, user));
     const size_t fbytes = size_t(src_h) * src_w * 3;
-    // two staging slots: the H2D copy of chunk i+1 (copy stream) overlaps the tower on chunk i (compute stream).
+    // two staging slots: the H2D copy of chunk i+1 (copy stream) overlaps the tower on chunk i (engine stream).
     // (a re-allocation frees the old buffer with cudaFree, which waits for the calls in flight)
-    VF_TRY(grow(&h->stage_u8, &h->stage_cap, 2 * size_t(h->chunk) * fbytes));
+    VF_TRY(grow(h, &h->stage_u8, &h->stage_cap, 2 * size_t(h->chunk) * fbytes));
     float* feats = out_dev;                 // the caller's device buffer, else the handle's own
     if (!feats) {
         if (h->out_cap < size_t(n) * E * sizeof(float)) {
@@ -557,7 +405,7 @@ static int clip_encode_u8_host(vf_clip_t* h, const uint8_t* frames_host, int n, 
         }
         feats = h->out_dev;
     }
-    const int step = balanced_chunk(h, n);
+    const int step = balanced_step(n, h->chunk);
     const int nchunks = (n + step - 1) / step;
     // the staging copies read HOST memory that is ready now: they are not ordered behind the caller's stream (which, after
     // an asynchronous call, waits for that call's tower) -- only behind the staging slot's previous user
@@ -572,8 +420,6 @@ static int clip_encode_u8_host(vf_clip_t* h, const uint8_t* frames_host, int n, 
         const int b0 = i * step;
         const int c = (n - b0 < step) ? (n - b0) : step;
         const int slot = i & 1;
-        LaneScope lane(h, i % h->n_lanes);
-        cudaStream_t s = lane.s;
         uint8_t* dst = h->stage_u8 + size_t(slot) * h->chunk * fbytes;
         // slot free again: its previous user (an earlier chunk of this call, or of a call still in flight) has been
         // transformed.  Waiting on a never-recorded event is a no-op.
@@ -581,33 +427,27 @@ static int clip_encode_u8_host(vf_clip_t* h, const uint8_t* frames_host, int n, 
         VF_CUDA(cudaMemcpyAsync(dst, frames_host + size_t(b0) * fbytes, size_t(c) * fbytes, cudaMemcpyHostToDevice,
                                 h->copy_stream));
         VF_CUDA(cudaEventRecord(h->ev_copy[slot], h->copy_stream));
-        VF_CUDA(cudaStreamWaitEvent(s, h->ev_copy[slot], 0));
-        VF_TRY(clip_transform_chunk(h, dst, c, src_h, src_w, g, s));
-        VF_CUDA(cudaEventRecord(h->ev_done[slot], s));   // staging slot consumed
-        VF_TRY(clip_tower_chunk(h, c, feats + size_t(b0) * E, s));
-    }
-    // gather point: lane 0 waits for lane 1, then one D2H of all features
-    cudaStream_t s0 = h->lanes[0].cs;
-    if (h->n_lanes > 1) {
-        VF_CUDA(cudaEventRecord(h->lanes[1].ev_out, h->lanes[1].cs));
-        VF_CUDA(cudaStreamWaitEvent(s0, h->lanes[1].ev_out, 0));
+        VF_CUDA(cudaStreamWaitEvent(h->cs, h->ev_copy[slot], 0));
+        VF_TRY(clip_transform_chunk(h, dst, c, src_h, src_w, g, h->cs));
+        VF_CUDA(cudaEventRecord(h->ev_done[slot], h->cs));   // staging slot consumed
+        VF_TRY(clip_tower_run(h, c, feats + size_t(b0) * E));
     }
     if (out_host)
-        VF_CUDA(cudaMemcpyAsync(out_host, feats, size_t(n) * E * sizeof(float), cudaMemcpyDeviceToHost, s0));
+        VF_CUDA(cudaMemcpyAsync(out_host, feats, size_t(n) * E * sizeof(float), cudaMemcpyDeviceToHost, h->cs));
     if (ticket) {
-        // everything this call reads from / writes to the host is complete once s0 reaches this point (the tower
+        // everything this call reads from / writes to the host is complete once the engine stream reaches this point (the tower
         // depends on every staging copy)
         const int64_t t = h->seq.load();
         cudaEvent_t ev = h->ev_ticket[t % vf_clip::kTickets];
         if (t >= vf_clip::kTickets) VF_CUDA(cudaEventSynchronize(ev));          // at most kTickets calls in flight
-        VF_CUDA(cudaEventRecord(ev, s0));
+        VF_CUDA(cudaEventRecord(ev, h->cs));
         *ticket = t;
         h->seq.store(t + 1);
         return leave(h, user);
     }
     VF_TRY(leave(h, user));
     // the host frames may be reused (and out_host read) as soon as this returns
-    VF_CUDA(cudaStreamSynchronize(out_host ? s0 : h->copy_stream));
+    VF_CUDA(cudaStreamSynchronize(out_host ? h->cs : h->copy_stream));
     return VF_OK;
 }
 
@@ -651,23 +491,14 @@ int vf_clip_block_attention(vf_clip_t* h, int layer, const void* x, int n_frames
     const __half* xin = static_cast<const __half*>(x);
     __half* o = static_cast<__half*>(out);
     if (fused) return qkv_attention(xin, W, w.w_qkv_heads, w.b_qkv_heads, o, n_frames, H, s);
-    __half* qkv = h->lanes[0].qkv;
-    VF_TRY(gemm_f16(xin, W, w.w_qkv, W, n_frames * T, 3 * W, W, epi(qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
-    return launch_attention(qkv, o, n_frames, T, H, s);
+    VF_TRY(gemm_f16(xin, W, w.w_qkv, W, n_frames * T, 3 * W, W, linear_epi(h->qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
+    return launch_attention(h->qkv, o, n_frames, T, H, s);
 }
 
-// The three pieces of the tower one at a time, eagerly, on lane 0's workspace and the caller's stream.
-static int debug_args(vf_clip_t* h, const void* a, const void* b, int n, const char* what) {
-    if (!h || !a || !b) return fail(VF_ERR_INVALID, "%s: null argument", what);
-    if (n <= 0 || n > h->chunk) return fail(VF_ERR_INVALID, "%s: %d frames (1 .. %d, the handle's chunk)", what, n, h->chunk);
-    VF_CUDA(cudaSetDevice(h->device));
-    return VF_OK;
-}
-
+// The three pieces of the tower one at a time, eagerly, on the handle's workspace and the caller's stream.
 int vf_clip_debug_embed_f32(vf_clip_t* h, const float* frames, int n, float* x_out, void* stream) {
-    VF_TRY(debug_args(h, frames, x_out, n, "clip_debug_embed_f32"));
+    VF_TRY(debug_frames(h, frames, x_out, n, h ? h->chunk : 0, "chunk", "clip_debug_embed_f32"));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    LaneScope lane(h, 0);
     VF_TRY(launch_clip_patchify_f32(frames, n, h->patches, h->patch, s));
     h->launches += 1;
     VF_TRY(tower_embed(h, n, s));
@@ -676,11 +507,10 @@ int vf_clip_debug_embed_f32(vf_clip_t* h, const float* frames, int n, float* x_o
 }
 
 int vf_clip_debug_embed_u8(vf_clip_t* h, const uint8_t* frames, int n, int src_h, int src_w, float* x_out, void* stream) {
-    VF_TRY(debug_args(h, frames, x_out, n, "clip_debug_embed_u8"));
-    ClipGeom g;
-    VF_TRY(clip_geometry(src_h, src_w, &g));
+    VF_TRY(debug_frames(h, frames, x_out, n, h ? h->chunk : 0, "chunk", "clip_debug_embed_u8"));
+    FrameGeom g;
+    VF_TRY(frame_geometry("clip", src_h, src_w, 224, 224, &g));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    LaneScope lane(h, 0);
     VF_TRY(clip_transform_chunk(h, frames, n, src_h, src_w, g, s));
     VF_TRY(tower_embed(h, n, s));
     VF_CUDA(cudaMemcpyAsync(x_out, h->x, size_t(n) * h->T * W * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -688,11 +518,10 @@ int vf_clip_debug_embed_u8(vf_clip_t* h, const uint8_t* frames, int n, int src_h
 }
 
 int vf_clip_debug_blocks(vf_clip_t* h, float* x, int n_frames, int layer_begin, int layer_end, void* stream) {
-    VF_TRY(debug_args(h, x, x, n_frames, "clip_debug_blocks"));
+    VF_TRY(debug_frames(h, x, x, n_frames, h ? h->chunk : 0, "chunk", "clip_debug_blocks"));
     if (layer_begin < 0 || layer_begin >= layer_end || layer_end > L)
         return fail(VF_ERR_INVALID, "clip_debug_blocks: layers [%d, %d) are not a range within [0, %d)", layer_begin, layer_end, L);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    LaneScope lane(h, 0);
     const int T = h->T;
     const size_t bytes = size_t(n_frames) * T * W * sizeof(float);
     VF_CUDA(cudaMemcpyAsync(h->x, x, bytes, cudaMemcpyDeviceToDevice, s));
@@ -711,9 +540,8 @@ int vf_clip_debug_blocks(vf_clip_t* h, float* x, int n_frames, int layer_begin, 
 }
 
 int vf_clip_debug_head(vf_clip_t* h, const float* x, int n_frames, float* out, void* stream) {
-    VF_TRY(debug_args(h, x, out, n_frames, "clip_debug_head"));
+    VF_TRY(debug_frames(h, x, out, n_frames, h ? h->chunk : 0, "chunk", "clip_debug_head"));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    LaneScope lane(h, 0);
     VF_CUDA(cudaMemcpyAsync(h->x, x, size_t(n_frames) * h->T * W * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return tower_head(h, n_frames, nullptr, out, s);
 }

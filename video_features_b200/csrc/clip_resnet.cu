@@ -57,8 +57,6 @@ struct vf_clip_rn : vf::EngineCore {
     __half *bufA = nullptr, *bufB = nullptr, *t1 = nullptr, *t2 = nullptr, *ds = nullptr, *ph1 = nullptr, *ph2 = nullptr;
     __half *tok = nullptr, *att = nullptr;
     float *kvo = nullptr, *qo = nullptr;
-    uint8_t *resized = nullptr, *resize_tmp = nullptr;        // grown on demand for the u8 entry's resize
-    size_t resized_cap = 0, tmp_cap = 0;
     int last_n = 0;
     int attn_n = 0;           // frames of the last vf_clip_rn_debug_attnpool (its intermediates stay readable)
 };
@@ -74,12 +72,6 @@ static Vol2 stem_vol(const vf_clip_rn* h, int n) {
 static Vol2 stage_vol(const vf_clip_rn* h, int n, int L) {
     const int S = h->npx / (4 << L);
     return Vol2{n, S + 2, S + 2, 1, S + 1, 1, S + 1};
-}
-
-static int64_t numel_of(const ResTensors& T, const std::string& name) {
-    for (int i = 0; i < T.n; ++i)
-        if (T.t[i].name && name == T.t[i].name) return T.t[i].numel;
-    return -1;
 }
 
 // stem conv1 3x3/2 pad 1 on the transform's phase volume: phase row q holds x[2(q-1)+p]; tap a (kernel rows 2a-1,
@@ -194,51 +186,24 @@ static int run_trunk(vf_clip_rn* h, int m, cudaStream_t s) {
     return run_attention(h, h->stage_out[3], m, s);
 }
 
-// a resize buffer of at least `need` bytes; the engine stream is drained before an old one is freed
-static int grow(vf_clip_rn* h, uint8_t** p, size_t* cap, size_t need) {
-    if (need <= *cap) return VF_OK;
-    if (*p) {
-        VF_CUDA(cudaStreamSynchronize(h->cs));
-        VF_CUDA(cudaFree(*p));
-        *p = nullptr; *cap = 0;
-    }
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, need);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "clip_rn_encode: cudaMalloc(%zu bytes): %s", need, cudaGetErrorString(e));
-    *p = static_cast<uint8_t*>(q);
-    *cap = need;
-    return VF_OK;
-}
-
 static int clip_rn_encode(vf_clip_rn* h, const void* frames, int is_u8, int n, int H, int W, float* out, void* stream) {
     if (!h || !frames || !out) return fail(VF_ERR_INVALID, "clip_rn_encode: null argument");
     if (n < 0) return fail(VF_ERR_INVALID, "clip_rn_encode: %d frames", n);
-    if (is_u8 && (H <= 0 || W <= 0)) return fail(VF_ERR_INVALID, "clip_rn_encode: bad frame geometry %dx%d", H, W);
-    if (n == 0) return VF_OK;
     const int npx = h->npx;
-    int rh = npx, rw = npx;
-    if (is_u8) VF_TRY(vf_resize_geometry(H, W, npx, 1, &rh, &rw));
-    const bool resize = is_u8 && (rh != H || rw != W);
-    const int cy = is_u8 ? center_crop_offset(rh, npx) : 0, cx = is_u8 ? center_crop_offset(rw, npx) : 0;
+    FrameGeom g{npx, npx, 0, 0, false};
+    if (is_u8) VF_TRY(frame_geometry("clip_rn_encode", H, W, npx, npx, &g));
+    if (n == 0) return VF_OK;
     const size_t frame_elems = is_u8 ? size_t(H) * W * 3 : size_t(3) * npx * npx;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
-    VF_CUDA(cudaSetDevice(h->device));
-    if (resize) {
-        VF_TRY(grow(h, &h->resized, &h->resized_cap, size_t(h->max_frames) * rh * rw * 3));
-        VF_TRY(grow(h, &h->resize_tmp, &h->tmp_cap, size_t(h->max_frames) * H * rw * 3));
-    }
     VF_TRY(enter(h, user));
     for (int off = 0; off < n; off += h->max_frames) {      // calls beyond the workspace run in chunks
         const int m = std::min(h->max_frames, n - off);
-        const void* src = is_u8 ? static_cast<const void*>(static_cast<const uint8_t*>(frames) + off * frame_elems)
-                                : static_cast<const void*>(static_cast<const float*>(frames) + off * frame_elems);
-        if (resize) {
-            VF_TRY(resize_u8(static_cast<const uint8_t*>(src), m, H, W, h->resized, rh, rw, VF_FILTER_BICUBIC,
-                             h->resize_tmp, s));
-            h->launches += (rh != H) + (rw != W);
-            src = h->resized;
-        }
-        VF_TRY(clip_rn_input_pack(src, is_u8, m, rh, rw, cy, cx, npx, h->s0, s));
+        const uint8_t* u8 = nullptr;
+        if (is_u8)
+            VF_TRY(resize_frames(h, static_cast<const uint8_t*>(frames) + off * frame_elems, m, H, W, g, h->max_frames,
+                                 s, &u8));
+        const void* src = is_u8 ? static_cast<const void*>(u8) : static_cast<const float*>(frames) + off * frame_elems;
+        VF_TRY(clip_rn_input_pack(src, is_u8, m, g.rh, g.rw, g.cy, g.cx, npx, h->s0, s));
         VF_TRY(run_graphed(h, {m, 0, 0, 0}, [&] { return run_trunk(h, m, s); }));
         VF_TRY(run_cproj(h, m, out + size_t(off) * h->out_dim, s));
         h->launches += 1;       // the input pack
@@ -255,8 +220,6 @@ extern "C" {
 int vf_clip_rn_destroy(vf_clip_rn_t* h) {
     if (!h) return VF_OK;
     release(h);
-    if (h->resized) cudaFree(h->resized);
-    if (h->resize_tmp) cudaFree(h->resize_tmp);
     delete h;
     return VF_OK;
 }
@@ -266,7 +229,7 @@ int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_
     *out = nullptr;
     const ResTensors T{tensors, n_tensors, "clip_rn_create"};
     // clip.model.build_model: width from the stem, depths from the block keys, resolution from the positional embedding
-    const int64_t n_bn1 = numel_of(T, "visual.bn1.weight");
+    const int64_t n_bn1 = T.numel("visual.bn1.weight");
     if (n_bn1 <= 0) return fail(VF_ERR_INVALID, "clip_rn_create: missing tensor 'visual.bn1.weight'");
     const int width = int(2 * n_bn1), E = 32 * width;
     if (width % 16 || E % 64)
@@ -274,17 +237,17 @@ int vf_clip_rn_create(vf_clip_rn_t** out, const vf_named_tensor* tensors, int n_
     int layers[4];
     for (int L = 0; L < 4; ++L) {
         int b = 0;
-        while (numel_of(T, "visual.layer" + std::to_string(L + 1) + "." + std::to_string(b) + ".conv1.weight") > 0) ++b;
+        while (T.numel("visual.layer" + std::to_string(L + 1) + "." + std::to_string(b) + ".conv1.weight") > 0) ++b;
         if (b == 0) return fail(VF_ERR_INVALID, "clip_rn_create: missing tensor 'visual.layer%d.0.conv1.weight'", L + 1);
         layers[L] = b;
     }
-    const int64_t n_pos = numel_of(T, "visual.attnpool.positional_embedding");
+    const int64_t n_pos = T.numel("visual.attnpool.positional_embedding");
     if (n_pos <= 0) return fail(VF_ERR_INVALID, "clip_rn_create: missing tensor 'visual.attnpool.positional_embedding'");
     const int side = int(lround(sqrt(double(n_pos / E - 1))));
     if (side < 1 || n_pos != int64_t(side * side + 1) * E)
         return fail(VF_ERR_INVALID, "clip_rn_create: tensor 'visual.attnpool.positional_embedding' has %lld elements, "
                     "not (s^2 + 1) x %d", (long long)n_pos, E);
-    const int64_t n_cp = numel_of(T, "visual.attnpool.c_proj.weight");
+    const int64_t n_cp = T.numel("visual.attnpool.c_proj.weight");
     if (n_cp <= 0) return fail(VF_ERR_INVALID, "clip_rn_create: missing tensor 'visual.attnpool.c_proj.weight'");
     if (n_cp % E || n_cp / E % 8)
         return fail(VF_ERR_INVALID, "clip_rn_create: tensor 'visual.attnpool.c_proj.weight' has %lld elements, not a "

@@ -14,7 +14,6 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <map>
 #include <string>
 #include <vector>
 
@@ -46,50 +45,15 @@ struct vf_clip_vitl : vf::EngineCore {
     // workspace (max_frames frames)
     __half *patches = nullptr, *h = nullptr, *qkv = nullptr, *att = nullptr, *mlp = nullptr, *cls = nullptr;
     float *x = nullptr, *emb = nullptr, *feat = nullptr;
-    uint8_t *resized = nullptr, *resize_tmp = nullptr;        // grown on demand for the u8 entry's resize
-    size_t resized_cap = 0, tmp_cap = 0;
-    std::map<int, int> seen;                    // frames in chunk -> times run without a graph
 };
 
 namespace vf {
-
-constexpr size_t kVitlMaxGraphs = 16;
-
-static int vl_upload_f32(vf_clip_vitl* h, float** dst, const float* src, size_t count) {
-    VF_TRY(ralloc(h, dst, count));
-    VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-// fp32 host [rows, cols] -> fp16 device [rows, ld] (columns cols..ld-1 zero; transpose: src is [cols, rows]),
-// round-to-nearest-even
-static int vl_upload_f16(vf_clip_vitl* h, __half** dst, const float* src, size_t rows, size_t cols, size_t ld,
-                         bool transpose = false) {
-    std::vector<__half> tmp(rows * ld, __float2half_rn(0.f));
-    for (size_t r = 0; r < rows; ++r)
-        for (size_t c = 0; c < cols; ++c) tmp[r * ld + c] = __float2half_rn(transpose ? src[c * rows + r] : src[r * cols + c]);
-    VF_TRY(ralloc(h, dst, rows * ld));
-    VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    return VF_OK;
-}
-
-static int64_t vl_numel(const ResTensors& T, const std::string& name) {
-    for (int i = 0; i < T.n; ++i)
-        if (T.t[i].name && (name == T.t[i].name || ("module." + name) == T.t[i].name)) return T.t[i].numel;
-    return -1;
-}
-
-static GemmEpi vl_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate = 0) {
-    GemmEpi e;
-    memset(&e, 0, sizeof(e));
-    e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.bias = bias; e.act = act; e.accumulate = accumulate;
-    return e;
-}
 
 // h->patches (c frames) -> h->x: patch-embedding GEMM, then token assembly + ln_pre
 static int vl_embed(vf_clip_vitl* h, int c, cudaStream_t s) {
     const int P = h->patches_per_frame;
     VF_TRY(gemm_f16(h->patches, VITL_PK, h->w_patch, VITL_PK, c * P, VITL_W, VITL_PK,
-                    vl_epi(h->emb, VITL_W, 1, nullptr, VF_ACT_NONE), s));
+                    linear_epi(h->emb, VITL_W, 1, nullptr, VF_ACT_NONE), s));
     VF_TRY(vitl_embed_layernorm(h->emb, h->pos, h->cls_pos0, h->lnpre_w, h->lnpre_b, h->x, c, h->tokens, s));
     h->launches += 2;
     return VF_OK;
@@ -102,14 +66,14 @@ static int vl_blocks(vf_clip_vitl* h, int c, int l0, int l1, cudaStream_t s) {
     for (int l = l0; l < l1; ++l) {
         const VitlLayer& w = h->layer[l];
         VF_TRY(vitl_layernorm(h->x, W, w.ln1_w, w.ln1_b, h->h, W, M, s));
-        VF_TRY(gemm_f16(h->h, W, w.w_qkv, W, M, 3 * W, W, vl_epi(h->qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
+        VF_TRY(gemm_f16(h->h, W, w.w_qkv, W, M, 3 * W, W, linear_epi(h->qkv, 3 * W, 0, w.b_qkv, VF_ACT_NONE), s));
         VF_TRY(vitl_attention(h->qkv, h->att, c, T, VL_HEADS, s));
         const bool last = l + 1 == VL_LAYERS;
         const int rows = last ? c : M, a_ld = last ? T * W : W;
-        VF_TRY(gemm_f16(h->att, a_ld, w.w_o, W, rows, W, W, vl_epi(h->x, a_ld, 1, w.b_o, VF_ACT_NONE, 1), s));
+        VF_TRY(gemm_f16(h->att, a_ld, w.w_o, W, rows, W, W, linear_epi(h->x, a_ld, 1, w.b_o, VF_ACT_NONE, 1), s));
         VF_TRY(vitl_layernorm(h->x, a_ld, w.ln2_w, w.ln2_b, h->h, W, rows, s));
-        VF_TRY(gemm_f16(h->h, W, w.w_fc, W, rows, VL_MLP, W, vl_epi(h->mlp, VL_MLP, 0, w.b_fc, VF_ACT_QUICKGELU), s));
-        VF_TRY(gemm_f16(h->mlp, VL_MLP, w.w_proj, VL_MLP, rows, W, VL_MLP, vl_epi(h->x, a_ld, 1, w.b_proj, VF_ACT_NONE, 1), s));
+        VF_TRY(gemm_f16(h->h, W, w.w_fc, W, rows, VL_MLP, W, linear_epi(h->mlp, VL_MLP, 0, w.b_fc, VF_ACT_QUICKGELU), s));
+        VF_TRY(gemm_f16(h->mlp, VL_MLP, w.w_proj, VL_MLP, rows, W, VL_MLP, linear_epi(h->x, a_ld, 1, w.b_proj, VF_ACT_NONE, 1), s));
         h->launches += 6;
     }
     return VF_OK;
@@ -118,114 +82,43 @@ static int vl_blocks(vf_clip_vitl* h, int c, int l0, int l1, cudaStream_t s) {
 // class rows of h->x (row pitch T * 1024): ln_post, then the 1024 -> 768 projection -> out (c x 768 fp32)
 static int vl_head(vf_clip_vitl* h, int c, float* out, cudaStream_t s) {
     VF_TRY(vitl_layernorm(h->x, int64_t(h->tokens) * VITL_W, h->lnpost_w, h->lnpost_b, h->cls, VITL_W, c, s));
-    VF_TRY(gemm_f16(h->cls, VITL_W, h->w_proj, VITL_W, c, VL_EMBED, VITL_W, vl_epi(out, VL_EMBED, 1, nullptr, VF_ACT_NONE), s));
+    VF_TRY(gemm_f16(h->cls, VITL_W, h->w_proj, VITL_W, c, VL_EMBED, VITL_W, linear_epi(out, VL_EMBED, 1, nullptr, VF_ACT_NONE), s));
     h->launches += 2;
     return VF_OK;
 }
 
-static int vl_tower_eager(vf_clip_vitl* h, int c, float* out, cudaStream_t s) {
+static int vl_tower(vf_clip_vitl* h, int c, float* out, cudaStream_t s) {
     VF_TRY(vl_embed(h, c, s));
     VF_TRY(vl_blocks(h, c, 0, VL_LAYERS, s));
     return vl_head(h, c, out, s);
-}
-
-// the tower on one chunk whose patch matrix is in h->patches -> out (c x 768): replay the chunk size's graph, capturing
-// it the second time the size is seen (one-off sizes run eagerly); at most kVitlMaxGraphs graphs are kept
-static int vl_tower_chunk(vf_clip_vitl* h, int c, float* out, cudaStream_t s) {
-    if (!h->use_graph || gemm_profile_on()) return vl_tower_eager(h, c, out, s);
-    const GraphKey key{c, 0, 0, 0};
-    auto it = h->graphs.find(key);
-    if (it == h->graphs.end()) {
-        if (h->seen.size() > 4096) h->seen.clear();
-        if (++h->seen[c] < 2 || h->graphs.size() >= kVitlMaxGraphs) return vl_tower_eager(h, c, out, s);
-        CachedGraph g;
-        VF_TRY(capture_graph(h, s, [&] { return vl_tower_eager(h, c, h->feat, s); }, &g));
-        it = h->graphs.emplace(key, g).first;
-    }
-    VF_CUDA(cudaGraphLaunch(it->second.exec, s));
-    VF_CUDA(cudaMemcpyAsync(out, h->feat, size_t(c) * VL_EMBED * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    h->launches += it->second.launches;
-    return VF_OK;
-}
-
-// a resize buffer of at least `need` bytes; the engine stream is drained before an old one is freed
-static int vl_grow(vf_clip_vitl* h, uint8_t** p, size_t* cap, size_t need) {
-    if (need <= *cap) return VF_OK;
-    if (*p) {
-        VF_CUDA(cudaStreamSynchronize(h->cs));
-        VF_CUDA(cudaFree(*p));
-        *p = nullptr; *cap = 0;
-    }
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, need);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "clip_vitl: cudaMalloc(%zu bytes): %s", need, cudaGetErrorString(e));
-    *p = static_cast<uint8_t*>(q);
-    *cap = need;
-    return VF_OK;
-}
-
-// the CLIP transform of a (H, W) frame at n_px: short side resized to n_px (bicubic, Pillow-exact), centre crop
-struct VlGeom { int rh, rw, cy, cx; bool resize; };
-static int vl_geometry(const vf_clip_vitl* h, int H, int W, VlGeom* g) {
-    if (H <= 0 || W <= 0) return fail(VF_ERR_INVALID, "clip_vitl: bad frame geometry %dx%d", H, W);
-    VF_TRY(vf_resize_geometry(H, W, h->npx, 1, &g->rh, &g->rw));
-    g->resize = g->rh != H || g->rw != W;
-    g->cy = center_crop_offset(g->rh, h->npx);
-    g->cx = center_crop_offset(g->rw, h->npx);
-    return VF_OK;
-}
-
-// c device uint8 frames of geometry (H, W) -> h->patches
-static int vl_transform(vf_clip_vitl* h, const uint8_t* frames, int c, int H, int W, const VlGeom& g, cudaStream_t s) {
-    const uint8_t* cur = frames;
-    int ch = H, cw = W;
-    if (g.resize) {
-        VF_TRY(vl_grow(h, &h->resized, &h->resized_cap, size_t(h->max_frames) * g.rh * g.rw * 3));
-        VF_TRY(vl_grow(h, &h->resize_tmp, &h->tmp_cap, size_t(h->max_frames) * H * g.rw * 3));
-        VF_TRY(resize_u8(frames, c, H, W, h->resized, g.rh, g.rw, VF_FILTER_BICUBIC, h->resize_tmp, s));
-        h->launches += (g.rh != H) + (g.rw != W);
-        cur = h->resized; ch = g.rh; cw = g.rw;
-    }
-    VF_TRY(vitl_patchify_u8(cur, c, ch, cw, g.cy, g.cx, h->npx, h->patches, s));
-    h->launches += 1;
-    return VF_OK;
-}
-
-// frames per chunk for a call of n: as few chunks as the workspace allows, all (nearly) the same size
-static int vl_step(const vf_clip_vitl* h, int n) {
-    const int nchunks = (n + h->max_frames - 1) / h->max_frames;
-    return (n + nchunks - 1) / nchunks;
 }
 
 static int vl_encode(vf_clip_vitl* h, const void* frames, int is_u8, int n, int H, int W, float* out, void* stream) {
     if (!h || (n > 0 && (!frames || !out))) return fail(VF_ERR_INVALID, "clip_vitl_encode: null argument");
     if (n < 0) return fail(VF_ERR_INVALID, "clip_vitl_encode: %d frames", n);
     if (n == 0) return VF_OK;
-    VlGeom g{h->npx, h->npx, 0, 0, false};
-    if (is_u8) VF_TRY(vl_geometry(h, H, W, &g));
+    FrameGeom g{h->npx, h->npx, 0, 0, false};
+    if (is_u8) VF_TRY(frame_geometry("clip_vitl", H, W, h->npx, h->npx, &g));
     const size_t frame_elems = is_u8 ? size_t(H) * W * 3 : size_t(3) * h->npx * h->npx;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
     VF_TRY(enter(h, user));
-    const int step = vl_step(h, n);
+    const int step = balanced_step(n, h->max_frames);
     for (int off = 0; off < n; off += step) {
         const int c = n - off < step ? n - off : step;
         if (is_u8) {
-            VF_TRY(vl_transform(h, static_cast<const uint8_t*>(frames) + off * frame_elems, c, H, W, g, s));
+            const uint8_t* src;
+            VF_TRY(resize_frames(h, static_cast<const uint8_t*>(frames) + off * frame_elems, c, H, W, g, h->max_frames,
+                                 s, &src));
+            VF_TRY(vitl_patchify_u8(src, c, g.rh, g.rw, g.cy, g.cx, h->npx, h->patches, s));
         } else {
             VF_TRY(vitl_patchify_f32(static_cast<const float*>(frames) + off * frame_elems, c, h->npx, h->patches, s));
-            h->launches += 1;
         }
-        VF_TRY(vl_tower_chunk(h, c, out + size_t(off) * VL_EMBED, s));
+        h->launches += 1;
+        VF_TRY(run_graphed(h, {c, 0, 0, 0}, [&] { return vl_tower(h, c, h->feat, s); }));
+        VF_CUDA(cudaMemcpyAsync(out + size_t(off) * VL_EMBED, h->feat, size_t(c) * VL_EMBED * sizeof(float),
+                                cudaMemcpyDeviceToDevice, s));
     }
     return leave(h, user);
-}
-
-static int vl_debug_args(vf_clip_vitl* h, const void* a, const void* b, int n, const char* what) {
-    if (!h || !a || !b) return fail(VF_ERR_INVALID, "%s: null argument", what);
-    if (n <= 0 || n > h->max_frames)
-        return fail(VF_ERR_INVALID, "%s: %d frames (1 .. %d, the handle's max_frames)", what, n, h->max_frames);
-    VF_CUDA(cudaSetDevice(h->device));
-    return VF_OK;
 }
 
 }  // namespace vf
@@ -235,8 +128,6 @@ extern "C" {
 int vf_clip_vitl_destroy(vf_clip_vitl_t* h) {
     if (!h) return VF_OK;
     release(h);
-    if (h->resized) cudaFree(h->resized);
-    if (h->resize_tmp) cudaFree(h->resize_tmp);
     delete h;
     return VF_OK;
 }
@@ -249,9 +140,9 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
     // agree), patch from conv1's kernel, depth from the resblock keys, heads = width / 64, resolution from the
     // positional embedding, output width from proj
     const int W = VITL_W;
-    const int64_t n_cls = vl_numel(T, "visual.class_embedding");
+    const int64_t n_cls = T.numel("visual.class_embedding");
     if (n_cls <= 0) return fail(VF_ERR_INVALID, "clip_vitl_create: missing tensor 'visual.class_embedding'");
-    const int64_t n_conv = vl_numel(T, "visual.conv1.weight");
+    const int64_t n_conv = T.numel("visual.conv1.weight");
     if (n_conv <= 0) return fail(VF_ERR_INVALID, "clip_vitl_create: missing tensor 'visual.conv1.weight'");
     if (n_cls != W || n_conv % (3 * n_cls))
         return fail(VF_ERR_UNSUPPORTED, "clip_vitl_create: tensors 'visual.conv1.weight' (%lld elements) and "
@@ -263,13 +154,13 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
         return fail(VF_ERR_UNSUPPORTED, "clip_vitl_create: tensor 'visual.conv1.weight' has %lld elements, not "
                     "%d x 3 x 14 x 14 (patch 14 is built)", (long long)n_conv, W);
     int depth = 0;
-    while (vl_numel(T, "visual.transformer.resblocks." + std::to_string(depth) + ".attn.in_proj_weight") > 0) ++depth;
+    while (T.numel("visual.transformer.resblocks." + std::to_string(depth) + ".attn.in_proj_weight") > 0) ++depth;
     if (depth != VL_LAYERS)
         return fail(depth < VL_LAYERS ? VF_ERR_INVALID : VF_ERR_UNSUPPORTED,
                     "clip_vitl_create: tensor 'visual.transformer.resblocks.%d.attn.in_proj_weight' %s: %d resblocks "
                     "(24 are built)", depth < VL_LAYERS ? depth : VL_LAYERS, depth < VL_LAYERS ? "missing" : "present",
                     depth);
-    const int64_t n_pos = vl_numel(T, "visual.positional_embedding");
+    const int64_t n_pos = T.numel("visual.positional_embedding");
     if (n_pos <= 0) return fail(VF_ERR_INVALID, "clip_vitl_create: missing tensor 'visual.positional_embedding'");
     const int64_t cells = n_pos / W - 1;
     const int grid = int(lround(sqrt(double(cells > 0 ? cells : 0))));
@@ -280,7 +171,7 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
     if (npx != 224 && npx != 336)
         return fail(VF_ERR_UNSUPPORTED, "clip_vitl_create: tensor 'visual.positional_embedding' gives n_px %d "
                     "(224 and 336 are built)", npx);
-    const int64_t n_proj = vl_numel(T, "visual.proj");
+    const int64_t n_proj = T.numel("visual.proj");
     if (n_proj != int64_t(W) * VL_EMBED)
         return fail(n_proj <= 0 ? VF_ERR_INVALID : VF_ERR_UNSUPPORTED, "clip_vitl_create: tensor 'visual.proj' has %lld "
                     "elements, not %d x %d", (long long)n_proj, W, VL_EMBED);
@@ -294,23 +185,25 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
     h->who = "clip_vitl_create";
     h->device = device; h->max_frames = max_frames; h->npx = npx;
     h->patches_per_frame = grid * grid; h->tokens = grid * grid + 1;
+    h->capture_after = 2;            // one-off chunk sizes run eagerly
+    h->evict_when_full = false;
     auto body = [&]() -> int {
         const int Tk = h->tokens, P = h->patches_per_frame;
         const float *conv, *cls, *pos, *proj, *a, *b;
         VF_TRY(T.get("visual.conv1.weight", int64_t(W) * 588, &conv));
-        VF_TRY(vl_upload_f16(h, &h->w_patch, conv, W, 588, VITL_PK));
+        VF_TRY(upload_f16(h, &h->w_patch, conv, W, 588, VITL_PK));
         VF_TRY(T.get("visual.proj", int64_t(W) * VL_EMBED, &proj));
-        VF_TRY(vl_upload_f16(h, &h->w_proj, proj, VL_EMBED, W, W, true));
+        VF_TRY(upload_f16(h, &h->w_proj, proj, VL_EMBED, W, W, true));
         VF_TRY(T.get("visual.positional_embedding", int64_t(Tk) * W, &pos));
-        VF_TRY(vl_upload_f32(h, &h->pos, pos, size_t(Tk) * W));
+        VF_TRY(upload_f32(h, &h->pos, pos, size_t(Tk) * W));
         VF_TRY(T.get("visual.class_embedding", W, &cls));
         std::vector<float> c0(W);
         for (int i = 0; i < W; ++i) c0[i] = cls[i] + pos[i];
-        VF_TRY(vl_upload_f32(h, &h->cls_pos0, c0.data(), W));
-        VF_TRY(T.get("visual.ln_pre.weight", W, &a)); VF_TRY(vl_upload_f32(h, &h->lnpre_w, a, W));
-        VF_TRY(T.get("visual.ln_pre.bias", W, &a)); VF_TRY(vl_upload_f32(h, &h->lnpre_b, a, W));
-        VF_TRY(T.get("visual.ln_post.weight", W, &a)); VF_TRY(vl_upload_f32(h, &h->lnpost_w, a, W));
-        VF_TRY(T.get("visual.ln_post.bias", W, &a)); VF_TRY(vl_upload_f32(h, &h->lnpost_b, a, W));
+        VF_TRY(upload_f32(h, &h->cls_pos0, c0.data(), W));
+        VF_TRY(T.get("visual.ln_pre.weight", W, &a)); VF_TRY(upload_f32(h, &h->lnpre_w, a, W));
+        VF_TRY(T.get("visual.ln_pre.bias", W, &a)); VF_TRY(upload_f32(h, &h->lnpre_b, a, W));
+        VF_TRY(T.get("visual.ln_post.weight", W, &a)); VF_TRY(upload_f32(h, &h->lnpost_w, a, W));
+        VF_TRY(T.get("visual.ln_post.bias", W, &a)); VF_TRY(upload_f32(h, &h->lnpost_b, a, W));
         for (int l = 0; l < VL_LAYERS; ++l) {
             const std::string p = "visual.transformer.resblocks." + std::to_string(l) + ".";
             VitlLayer& d = h->layer[l];
@@ -320,14 +213,14 @@ int vf_clip_vitl_create(vf_clip_vitl_t** out, const vf_named_tensor* tensors, in
                 {"mlp.c_fc.bias", VL_MLP, &d.b_fc}, {"mlp.c_proj.bias", W, &d.b_proj}};
             for (const auto& v : vecs) {
                 VF_TRY(T.get(p + v.name, v.n, &a));
-                VF_TRY(vl_upload_f32(h, v.dst, a, size_t(v.n)));
+                VF_TRY(upload_f32(h, v.dst, a, size_t(v.n)));
             }
             const struct { const char* name; int rows, cols; __half** dst; } mats[] = {
                 {"attn.in_proj_weight", 3 * W, W, &d.w_qkv}, {"attn.out_proj.weight", W, W, &d.w_o},
                 {"mlp.c_fc.weight", VL_MLP, W, &d.w_fc}, {"mlp.c_proj.weight", W, VL_MLP, &d.w_proj}};
             for (const auto& m : mats) {
                 VF_TRY(T.get(p + m.name, int64_t(m.rows) * m.cols, &b));
-                VF_TRY(vl_upload_f16(h, m.dst, b, m.rows, m.cols, m.cols));
+                VF_TRY(upload_f16(h, m.dst, b, m.rows, m.cols));
             }
         }
         const size_t F = size_t(max_frames);
@@ -365,7 +258,7 @@ int vf_clip_vitl_encode_u8(vf_clip_vitl_t* h, const uint8_t* frames, int n, int 
 
 // The three pieces of the tower one at a time, eagerly, on the handle's workspace and the caller's stream.
 int vf_clip_vitl_debug_embed_f32(vf_clip_vitl_t* h, const float* frames, int n, float* x_out, void* stream) {
-    VF_TRY(vl_debug_args(h, frames, x_out, n, "clip_vitl_debug_embed_f32"));
+    VF_TRY(debug_frames(h, frames, x_out, n, h ? h->max_frames : 0, "max_frames", "clip_vitl_debug_embed_f32"));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     VF_TRY(vitl_patchify_f32(frames, n, h->npx, h->patches, s));
     h->launches += 1;
@@ -376,19 +269,22 @@ int vf_clip_vitl_debug_embed_f32(vf_clip_vitl_t* h, const float* frames, int n, 
 
 int vf_clip_vitl_debug_embed_u8(vf_clip_vitl_t* h, const uint8_t* frames, int n, int H, int W, float* x_out,
                                 void* stream) {
-    VF_TRY(vl_debug_args(h, frames, x_out, n, "clip_vitl_debug_embed_u8"));
-    VlGeom g;
-    VF_TRY(vl_geometry(h, H, W, &g));
+    VF_TRY(debug_frames(h, frames, x_out, n, h ? h->max_frames : 0, "max_frames", "clip_vitl_debug_embed_u8"));
+    FrameGeom g;
+    VF_TRY(frame_geometry("clip_vitl", H, W, h->npx, h->npx, &g));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     VF_CUDA(cudaStreamSynchronize(h->cs));       // a resize buffer may be re-allocated: the engine stream is idle
-    VF_TRY(vl_transform(h, frames, n, H, W, g, s));
+    const uint8_t* src;
+    VF_TRY(resize_frames(h, frames, n, H, W, g, h->max_frames, s, &src));
+    VF_TRY(vitl_patchify_u8(src, n, g.rh, g.rw, g.cy, g.cx, h->npx, h->patches, s));
+    h->launches += 1;
     VF_TRY(vl_embed(h, n, s));
     VF_CUDA(cudaMemcpyAsync(x_out, h->x, size_t(n) * h->tokens * VITL_W * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return VF_OK;
 }
 
 int vf_clip_vitl_debug_blocks(vf_clip_vitl_t* h, float* x, int n, int layer_begin, int layer_end, void* stream) {
-    VF_TRY(vl_debug_args(h, x, x, n, "clip_vitl_debug_blocks"));
+    VF_TRY(debug_frames(h, x, x, n, h ? h->max_frames : 0, "max_frames", "clip_vitl_debug_blocks"));
     if (layer_begin < 0 || layer_begin >= layer_end || layer_end > VL_LAYERS)
         return fail(VF_ERR_INVALID, "clip_vitl_debug_blocks: layers [%d, %d) are not a range within [0, %d)", layer_begin,
                     layer_end, VL_LAYERS);
@@ -401,7 +297,7 @@ int vf_clip_vitl_debug_blocks(vf_clip_vitl_t* h, float* x, int n, int layer_begi
 }
 
 int vf_clip_vitl_debug_head(vf_clip_vitl_t* h, const float* x, int n, float* out, void* stream) {
-    VF_TRY(vl_debug_args(h, x, out, n, "clip_vitl_debug_head"));
+    VF_TRY(debug_frames(h, x, out, n, h ? h->max_frames : 0, "max_frames", "clip_vitl_debug_head"));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     VF_CUDA(cudaMemcpyAsync(h->x, x, size_t(n) * h->tokens * VITL_W * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return vl_head(h, n, out, s);

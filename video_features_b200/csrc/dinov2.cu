@@ -48,8 +48,6 @@ struct vf_dinov2 : vf::EngineCore {
     // workspace (max_frames frames)
     __half *patches = nullptr, *hbuf = nullptr, *qkv = nullptr, *att = nullptr, *mlp = nullptr, *attc = nullptr;
     float *emb = nullptr, *x = nullptr, *ab = nullptr, *xc = nullptr, *feat = nullptr;
-    uint8_t *resized = nullptr, *resize_tmp = nullptr;        // grown on demand for the u8 entry's resize
-    size_t resized_cap = 0, tmp_cap = 0;
 };
 
 namespace vf {
@@ -135,89 +133,32 @@ static int dv_net(vf_dinov2* h, int c, cudaStream_t s) {
     return dv_head(h, c, h->feat, s);
 }
 
-// a resize buffer of at least `need` bytes; the engine stream is drained before an old one is freed
-static int dv_grow(vf_dinov2* h, uint8_t** p, size_t* cap, size_t need) {
-    if (need <= *cap) return VF_OK;
-    if (*p) {
-        VF_CUDA(cudaStreamSynchronize(h->cs));
-        VF_CUDA(cudaFree(*p));
-        *p = nullptr; *cap = 0;
-    }
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, need);
-    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "dinov2: cudaMalloc(%zu bytes): %s", need, cudaGetErrorString(e));
-    *p = static_cast<uint8_t*>(q);
-    *cap = need;
-    return VF_OK;
-}
-
-// Resize(256): the short side to 256 (bicubic, Pillow-exact), then the centre 224 crop
-struct DvGeom { int rh, rw, cy, cx; bool resize; };
-static int dv_geometry(int H, int W, DvGeom* g) {
-    if (H <= 0 || W <= 0) return fail(VF_ERR_INVALID, "dinov2: bad frame geometry %dx%d", H, W);
-    VF_TRY(vf_resize_geometry(H, W, DV_RESIZE, 1, &g->rh, &g->rw));
-    if (g->rh < DV_CROP || g->rw < DV_CROP)
-        return fail(VF_ERR_INVALID, "dinov2: a %dx%d frame resizes to %dx%d, smaller than the 224 crop", H, W, g->rh, g->rw);
-    g->resize = g->rh != H || g->rw != W;
-    g->cy = center_crop_offset(g->rh, DV_CROP);
-    g->cx = center_crop_offset(g->rw, DV_CROP);
-    return VF_OK;
-}
-
-// c device uint8 BGR frames of geometry (H, W) -> h->patches
-static int dv_transform(vf_dinov2* h, const uint8_t* frames, int c, int H, int W, const DvGeom& g, cudaStream_t s) {
-    const uint8_t* cur = frames;
-    int ch = H, cw = W;
-    if (g.resize) {
-        VF_TRY(dv_grow(h, &h->resized, &h->resized_cap, size_t(h->max_frames) * g.rh * g.rw * 3));
-        VF_TRY(dv_grow(h, &h->resize_tmp, &h->tmp_cap, size_t(h->max_frames) * H * g.rw * 3));
-        VF_TRY(resize_u8(frames, c, H, W, h->resized, g.rh, g.rw, VF_FILTER_BICUBIC, h->resize_tmp, s));
-        h->launches += (g.rh != H) + (g.rw != W);
-        cur = h->resized; ch = g.rh; cw = g.rw;
-    }
-    VF_TRY(dinov2_patchify_u8(cur, c, ch, cw, g.cy, g.cx, h->patches, s));
-    h->launches += 1;
-    return VF_OK;
-}
-
 static int dv_encode(vf_dinov2* h, const void* frames, int is_u8, int n, int H, int W, float* out, void* stream) {
     if (!h || (n > 0 && (!frames || !out))) return fail(VF_ERR_INVALID, "dinov2_encode: null argument");
     if (n < 0) return fail(VF_ERR_INVALID, "dinov2_encode: %d frames", n);
     if (n == 0) return VF_OK;
-    DvGeom g{DV_CROP, DV_CROP, 0, 0, false};
-    if (is_u8) VF_TRY(dv_geometry(H, W, &g));
+    FrameGeom g{DV_CROP, DV_CROP, 0, 0, false};
+    if (is_u8) VF_TRY(frame_geometry("dinov2", H, W, DV_RESIZE, DV_CROP, &g));
     const size_t frame_elems = is_u8 ? size_t(H) * W * 3 : size_t(3) * DV_CROP * DV_CROP;
     cudaStream_t user = static_cast<cudaStream_t>(stream), s = h->cs;
     VF_TRY(enter(h, user));
-    // as few chunks as the workspace allows, all (nearly) the same size
-    const int nchunks = (n + h->max_frames - 1) / h->max_frames, step = (n + nchunks - 1) / nchunks;
+    const int step = balanced_step(n, h->max_frames);
     for (int off = 0; off < n; off += step) {
         const int c = n - off < step ? n - off : step;
         if (is_u8) {
-            VF_TRY(dv_transform(h, static_cast<const uint8_t*>(frames) + off * frame_elems, c, H, W, g, s));
+            const uint8_t* src;
+            VF_TRY(resize_frames(h, static_cast<const uint8_t*>(frames) + off * frame_elems, c, H, W, g, h->max_frames,
+                                 s, &src));
+            VF_TRY(dinov2_patchify_u8(src, c, g.rh, g.rw, g.cy, g.cx, h->patches, s));
         } else {
             VF_TRY(dinov2_patchify_f32(static_cast<const float*>(frames) + off * frame_elems, c, h->patches, s));
-            h->launches += 1;
         }
+        h->launches += 1;
         VF_TRY(run_graphed(h, {c, 0, 0, 0}, [&] { return dv_net(h, c, s); }));
         VF_CUDA(cudaMemcpyAsync(out + size_t(off) * h->D, h->feat, size_t(c) * h->D * sizeof(float),
                                 cudaMemcpyDeviceToDevice, s));
     }
     return leave(h, user);
-}
-
-static int dv_debug_args(vf_dinov2* h, const void* a, const void* b, int n, const char* what) {
-    if (!h || !a || !b) return fail(VF_ERR_INVALID, "%s: null argument", what);
-    if (n <= 0 || n > h->max_frames)
-        return fail(VF_ERR_INVALID, "%s: %d frames (1 .. %d, the handle's max_frames)", what, n, h->max_frames);
-    VF_CUDA(cudaSetDevice(h->device));
-    return VF_OK;
-}
-
-static int dv_upload_f32(vf_dinov2* h, float** dst, const float* src, size_t count) {
-    VF_TRY(ralloc(h, dst, count));
-    VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
-    return VF_OK;
 }
 
 // the LayerScale fold of a residual-branch output linear: gamma and fp32(gamma * b)
@@ -228,8 +169,8 @@ static int dv_upload_ls(vf_dinov2* h, const ResTensors& T, const std::string& ga
     VF_TRY(T.get(bias, D, &b));
     std::vector<float> gb(D);
     for (int i = 0; i < D; ++i) gb[i] = g[i] * b[i];
-    VF_TRY(dv_upload_f32(h, g_dst, g, D));
-    return dv_upload_f32(h, b_dst, gb.data(), D);
+    VF_TRY(upload_f32(h, g_dst, g, D));
+    return upload_f32(h, b_dst, gb.data(), D);
 }
 
 }  // namespace vf
@@ -239,8 +180,6 @@ extern "C" {
 int vf_dinov2_destroy(vf_dinov2_t* h) {
     if (!h) return VF_OK;
     release(h);
-    if (h->resized) cudaFree(h->resized);
-    if (h->resize_tmp) cudaFree(h->resize_tmp);
     delete h;
     return VF_OK;
 }
@@ -304,11 +243,11 @@ int vf_dinov2_create(vf_dinov2_t** out, const vf_named_tensor* tensors, int n_te
         VF_TRY(upload_split_mat(h, T, "patch_embed.proj.weight", W, 3 * DV_PATCH * DV_PATCH, &h->w_patch, DV_PK));
         VF_TRY(upload_vec(h, T, "patch_embed.proj.bias", W, &h->b_patch));
         VF_TRY(T.get("pos_embed_224", int64_t(1 + DV_PATCHES) * W, &pos));
-        VF_TRY(dv_upload_f32(h, &h->pos, pos, size_t(1 + DV_PATCHES) * W));
+        VF_TRY(upload_f32(h, &h->pos, pos, size_t(1 + DV_PATCHES) * W));
         VF_TRY(T.get("cls_token", W, &a));
         std::vector<float> c0(W);
         for (int i = 0; i < W; ++i) c0[i] = a[i] + pos[i];
-        VF_TRY(dv_upload_f32(h, &h->cls_pos0, c0.data(), W));
+        VF_TRY(upload_f32(h, &h->cls_pos0, c0.data(), W));
         if (n_reg) VF_TRY(upload_vec(h, T, "register_tokens", int64_t(n_reg) * W, &h->reg));
         VF_TRY(upload_vec(h, T, "norm.weight", W, &h->norm_w));
         VF_TRY(upload_vec(h, T, "norm.bias", W, &h->norm_b));
@@ -367,7 +306,7 @@ int vf_dinov2_encode_u8(vf_dinov2_t* h, const uint8_t* frames, int n, int H, int
 }
 
 int vf_dinov2_debug_embed_f32(vf_dinov2_t* h, const float* frames, int n, float* x_out, void* stream) {
-    VF_TRY(dv_debug_args(h, frames, x_out, n, "dinov2_debug_embed_f32"));
+    VF_TRY(debug_frames(h, frames, x_out, n, h ? h->max_frames : 0, "max_frames", "dinov2_debug_embed_f32"));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     VF_TRY(dinov2_patchify_f32(frames, n, h->patches, s));
     h->launches += 1;
@@ -377,19 +316,22 @@ int vf_dinov2_debug_embed_f32(vf_dinov2_t* h, const float* frames, int n, float*
 }
 
 int vf_dinov2_debug_embed_u8(vf_dinov2_t* h, const uint8_t* frames, int n, int H, int W, float* x_out, void* stream) {
-    VF_TRY(dv_debug_args(h, frames, x_out, n, "dinov2_debug_embed_u8"));
-    DvGeom g;
-    VF_TRY(dv_geometry(H, W, &g));
+    VF_TRY(debug_frames(h, frames, x_out, n, h ? h->max_frames : 0, "max_frames", "dinov2_debug_embed_u8"));
+    FrameGeom g;
+    VF_TRY(frame_geometry("dinov2", H, W, DV_RESIZE, DV_CROP, &g));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     VF_CUDA(cudaStreamSynchronize(h->cs));       // a resize buffer may be re-allocated: the engine stream is idle
-    VF_TRY(dv_transform(h, frames, n, H, W, g, s));
+    const uint8_t* src;
+    VF_TRY(resize_frames(h, frames, n, H, W, g, h->max_frames, s, &src));
+    VF_TRY(dinov2_patchify_u8(src, n, g.rh, g.rw, g.cy, g.cx, h->patches, s));
+    h->launches += 1;
     VF_TRY(dv_embed(h, n, s));
     VF_CUDA(cudaMemcpyAsync(x_out, h->x, size_t(n) * h->S * h->D * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return VF_OK;
 }
 
 int vf_dinov2_debug_blocks(vf_dinov2_t* h, float* x, int n, int layer_begin, int layer_end, void* stream) {
-    VF_TRY(dv_debug_args(h, x, x, n, "dinov2_debug_blocks"));
+    VF_TRY(debug_frames(h, x, x, n, h ? h->max_frames : 0, "max_frames", "dinov2_debug_blocks"));
     if (layer_begin < 0 || layer_begin >= layer_end || layer_end > h->depth)
         return fail(VF_ERR_INVALID, "dinov2_debug_blocks: layers [%d, %d) are not a range within [0, %d)", layer_begin,
                     layer_end, h->depth);
@@ -402,7 +344,7 @@ int vf_dinov2_debug_blocks(vf_dinov2_t* h, float* x, int n, int layer_begin, int
 }
 
 int vf_dinov2_debug_head(vf_dinov2_t* h, const float* x, int n, float* out, void* stream) {
-    VF_TRY(dv_debug_args(h, x, out, n, "dinov2_debug_head"));
+    VF_TRY(debug_frames(h, x, out, n, h ? h->max_frames : 0, "max_frames", "dinov2_debug_head"));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     VF_CUDA(cudaMemcpyAsync(h->x, x, size_t(n) * h->S * h->D * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return dv_head(h, n, out, s);

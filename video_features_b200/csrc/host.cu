@@ -167,6 +167,11 @@ bool graphs_enabled() {
     return !(e && e[0] == '1');
 }
 
+bool graph_trace() {
+    const char* e = getenv("VF_GRAPH_TRACE");
+    return e && e[0] == '1';
+}
+
 int engine_alloc(EngineCore* h, void** p, size_t bytes) {
     void* q = nullptr;
     bytes += 65536;
@@ -203,9 +208,44 @@ void release(EngineCore* h) {
     cudaDeviceSynchronize();
     for (void* p : h->allocs) cudaFree(p);
     for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second.exec);
+    cudaFree(h->resized);
+    cudaFree(h->resize_tmp);
     if (h->cs) cudaStreamDestroy(h->cs);
     if (h->ev_in) cudaEventDestroy(h->ev_in);
     if (h->ev_out) cudaEventDestroy(h->ev_out);
+}
+
+int grow(EngineCore* h, uint8_t** p, size_t* cap, size_t need) {
+    if (need <= *cap) return VF_OK;
+    if (*p) {
+        VF_CUDA(cudaStreamSynchronize(h->cs));
+        VF_CUDA(cudaFree(*p));
+        *p = nullptr; *cap = 0;
+    }
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, need);
+    if (e != cudaSuccess) return fail(VF_ERR_NOMEM, "%s: cudaMalloc(%zu bytes): %s", h->who, need, cudaGetErrorString(e));
+    *p = static_cast<uint8_t*>(q);
+    *cap = need;
+    return VF_OK;
+}
+
+int upload_f32(EngineCore* h, float** dst, const float* src, size_t count) {
+    if (!src) return fail(VF_ERR_INVALID, "%s: missing weight tensor", h->who);
+    VF_TRY(ralloc(h, dst, count));
+    VF_CUDA(cudaMemcpy(*dst, src, count * sizeof(float), cudaMemcpyHostToDevice));
+    return VF_OK;
+}
+
+int upload_f16(EngineCore* h, __half** dst, const float* src, size_t rows, size_t cols, size_t ld, bool transpose) {
+    if (!src) return fail(VF_ERR_INVALID, "%s: missing weight tensor", h->who);
+    if (ld == 0) ld = cols;
+    std::vector<__half> tmp(rows * ld, __float2half_rn(0.f));
+    for (size_t r = 0; r < rows; ++r)
+        for (size_t c = 0; c < cols; ++c) tmp[r * ld + c] = __float2half_rn(transpose ? src[c * rows + r] : src[r * cols + c]);
+    VF_TRY(ralloc(h, dst, rows * ld));
+    VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    return VF_OK;
 }
 
 int capture_graph(EngineCore* h, cudaStream_t s, const std::function<int()>& run, CachedGraph* g) {
@@ -228,19 +268,70 @@ int run_graphed(EngineCore* h, const GraphKey& key, const std::function<int()>& 
     if (!h->use_graph || gemm_profile_on()) return run();
     auto it = h->graphs.find(key);
     if (it == h->graphs.end()) {
-        CachedGraph g;
-        VF_TRY(capture_graph(h, h->cs, run, &g));
         // bounded cache: ragged last chunks of many videos, or videos of many resolutions, must not pile up executable
         // graphs; an evicted graph that is still running is freed by the runtime when it completes
-        if (h->graphs.size() >= 16) {
+        const bool full = h->graphs.size() >= h->max_graphs;
+        if (h->seen.size() > 4096) h->seen.clear();
+        if (++h->seen[key] < h->capture_after || (full && !h->evict_when_full)) return run();
+        CachedGraph g;
+        VF_TRY(capture_graph(h, h->cs, run, &g));
+        if (full) {
             cudaGraphExecDestroy(h->graphs.begin()->second.exec);
             h->graphs.erase(h->graphs.begin());
         }
         it = h->graphs.emplace(key, g).first;
+        if (h->trace_graphs)
+            fprintf(stderr, "[vf] %s: graph captured for key (%d, %d, %d, %d), %zu cached\n", h->who, key[0], key[1], key[2],
+                    key[3], h->graphs.size());
     }
     VF_CUDA(cudaGraphLaunch(it->second.exec, h->cs));
     h->launches += it->second.launches;
     return VF_OK;
+}
+
+int frame_geometry(const char* who, int H, int W, int resize_to, int crop, FrameGeom* g) {
+    if (H <= 0 || W <= 0) return fail(VF_ERR_INVALID, "%s: bad frame geometry %dx%d", who, H, W);
+    VF_TRY(vf_resize_geometry(H, W, resize_to, 1, &g->rh, &g->rw));
+    if (g->rh < crop || g->rw < crop)
+        return fail(VF_ERR_INVALID, "%s: a %dx%d frame resizes to %dx%d, smaller than the %d crop", who, H, W, g->rh,
+                    g->rw, crop);
+    g->resize = g->rh != H || g->rw != W;
+    g->cy = center_crop_offset(g->rh, crop);
+    g->cx = center_crop_offset(g->rw, crop);
+    return VF_OK;
+}
+
+int resize_frames(EngineCore* h, const uint8_t* frames, int n, int H, int W, const FrameGeom& g, int max_frames,
+                  cudaStream_t s, const uint8_t** src) {
+    *src = frames;
+    if (!g.resize) return VF_OK;
+    VF_TRY(grow(h, &h->resized, &h->resized_cap, size_t(max_frames) * g.rh * g.rw * 3));
+    VF_TRY(grow(h, &h->resize_tmp, &h->tmp_cap, size_t(max_frames) * H * g.rw * 3));
+    VF_TRY(resize_u8(frames, n, H, W, h->resized, g.rh, g.rw, VF_FILTER_BICUBIC, h->resize_tmp, s));
+    h->launches += (g.rh != H) + (g.rw != W);
+    *src = h->resized;
+    return VF_OK;
+}
+
+int balanced_step(int n, int max_frames) {
+    const int nchunks = (n + max_frames - 1) / max_frames;
+    return nchunks > 0 ? (n + nchunks - 1) / nchunks : max_frames;
+}
+
+int debug_frames(const EngineCore* h, const void* a, const void* b, int n, int limit, const char* limit_name,
+                 const char* what) {
+    if (!h || !a || !b) return fail(VF_ERR_INVALID, "%s: null argument", what);
+    if (n <= 0 || n > limit)
+        return fail(VF_ERR_INVALID, "%s: %d frames (1 .. %d, the handle's %s)", what, n, limit, limit_name);
+    VF_CUDA(cudaSetDevice(h->device));
+    return VF_OK;
+}
+
+GemmEpi linear_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate) {
+    GemmEpi e;
+    memset(&e, 0, sizeof(e));
+    e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.bias = bias; e.act = act; e.accumulate = accumulate;
+    return e;
 }
 
 }  // namespace vf

@@ -37,6 +37,7 @@ int fail(int code, const char* fmt, ...);
 // cudaSetDevice(device), then VF_ERR_UNSUPPORTED unless the device is sm_90 (the library is built for sm_90a only)
 int check_device(int device);
 bool graphs_enabled();   // false under VF_NO_GRAPH=1: every call runs eagerly
+bool graph_trace();      // VF_GRAPH_TRACE=1: run_graphed reports every capture on stderr
 
 // graph-cache key: (frames), (clips, T), (F, Hp, Wp) or (F, H, W, iters), unused slots zero
 using GraphKey = std::array<int, 4>;
@@ -53,7 +54,16 @@ struct EngineCore {
     cudaStream_t cs = nullptr;                     // engine stream (open_stream), ordered against the caller's
     cudaEvent_t ev_in = nullptr, ev_out = nullptr; // stream by enter() / leave()
     bool use_graph = graphs_enabled();
+    bool trace_graphs = graph_trace();
     std::map<GraphKey, CachedGraph> graphs;        // run_graphed's cache
+    // run_graphed's admission policy: a key is captured on its capture_after-th sighting (earlier ones run eagerly); at
+    // most max_graphs are kept, and once that many are, a new key evicts the smallest (evict_when_full) or runs eagerly
+    int capture_after = 1;
+    size_t max_graphs = 16;
+    bool evict_when_full = true;
+    std::map<GraphKey, int> seen;                  // sightings of keys not in the cache
+    uint8_t *resized = nullptr, *resize_tmp = nullptr;   // the frame towers' resize scratch (resize_frames)
+    size_t resized_cap = 0, tmp_cap = 0;
 };
 
 // cudaMalloc'd, zero-filled, + 64 KB: the overlapping-row TMA view of a conv input extends up to (k_per_tap - C)
@@ -69,15 +79,40 @@ int ralloc(EngineCore* h, Tp** p, size_t count) {
 int open_stream(EngineCore* h);                    // the engine stream and its ev_in / ev_out pair
 int enter(EngineCore* h, cudaStream_t user);       // the engine stream waits for the work queued on `user`
 int leave(EngineCore* h, cudaStream_t user);       // `user` waits for the work queued on the engine stream
-// waits for the device, frees every allocation and graph, destroys the stream and events (the handle is not deleted)
+// waits for the device, frees every allocation, graph and the resize scratch, destroys the stream and events (the
+// handle is not deleted)
 void release(EngineCore* h);
+// a device buffer of at least `need` bytes; the engine stream is drained before an old one is freed
+int grow(EngineCore* h, uint8_t** p, size_t* cap, size_t need);
+// fp32 host -> device (a null source fails: a missing weight tensor)
+int upload_f32(EngineCore* h, float** dst, const float* src, size_t count);
+// fp32 host [rows, cols] -> fp16 device [rows, ld] (ld 0: cols; columns cols..ld-1 zero; transpose: src is
+// [cols, rows]), round-to-nearest-even
+int upload_f16(EngineCore* h, __half** dst, const float* src, size_t rows, size_t cols, size_t ld = 0,
+               bool transpose = false);
 // captures run() on stream s into an instantiated graph; h->launches is left as it was, g->launches gets what run()
 // counted
 int capture_graph(EngineCore* h, cudaStream_t s, const std::function<int()>& run, CachedGraph* g);
 // run() on the engine stream through the graph cache: eager under VF_NO_GRAPH=1 or GEMM profiling (event-bracketed
-// launches cannot be captured); otherwise the key's graph is captured on first use and replayed.  At most 16 graphs
-// are kept, the smallest key is evicted first.
+// launches cannot be captured); otherwise a key is captured as h's admission policy says and then replayed.  The
+// defaults capture on first use and keep 16 graphs, the smallest key evicted first.
 int run_graphed(EngineCore* h, const GraphKey& key, const std::function<int()>& run);
+
+// ---- the front end of the towers that take single frames (CLIP ViT-B / ViT-L / ResNet, DINOv2)
+// Resize(resize_to, bicubic) of the short side, then CenterCrop(crop): the resized size, the crop offset and whether the
+// frame is resized at all
+struct FrameGeom { int rh, rw, cy, cx; bool resize; };
+int frame_geometry(const char* who, int H, int W, int resize_to, int crop, FrameGeom* g);
+// n u8 frames of (H, W) -> *src, the frames the patchify kernel reads ((g.rh, g.rw) each): the frames themselves, or
+// their Pillow-exact bicubic resize into h->resized (grown for max_frames frames)
+int resize_frames(EngineCore* h, const uint8_t* frames, int n, int H, int W, const FrameGeom& g, int max_frames,
+                  cudaStream_t s, const uint8_t** src);
+// frames per chunk for a call of n: as few chunks as max_frames allows, all (nearly) the same size, so no ragged tail
+// chunk runs the whole tower on a handful of rows
+int balanced_step(int n, int max_frames);
+// the argument check of a debug entry: h, a and b set, 1 .. limit frames (limit_name: what the limit is called)
+int debug_frames(const EngineCore* h, const void* a, const void* b, int n, int limit, const char* limit_name,
+                 const char* what);
 
 // ---- tensor maps (driver entry point fetched at run time; the library does not link libcuda).
 // 2-D row-major tensor of 2- or 4-byte elements, 128-byte-swizzled boxes of box_rows x (128 / elem_bytes) columns.
@@ -97,6 +132,7 @@ struct GemmEpi {
     int accumulate;         // fp32 out only: 1 = out += result (fp32 TMA reduce-adds from the epilogue; every element
                             // is added exactly once, so the sum is deterministic) -- the residual-stream update of the ViT blocks
 };
+GemmEpi linear_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate = 0);
 int gemm_f16(const __half* A, int lda, const __half* B, int ldb, int M, int N, int K, const GemmEpi& ep,
              cudaStream_t stream);
 

@@ -294,16 +294,14 @@ static int mv_forward(vf_mvit* h, const void* src, int is_u8, int n_frames, int 
         return fail(VF_ERR_INVALID, "mvit_forward: %d clips of %d frames (the position tables fix 16 frames)", n, T);
     if (n > 0 && (!src || !out || (is_u8 && !starts))) return fail(VF_ERR_INVALID, "mvit_forward: null argument");
     const int per_chunk = std::min(h->max_clips, R21D_MAX_CHUNK);
-    int rh = MV_CROP, rw = MV_CROP, cy = 0, cx = 0;
+    FrameGeom g{MV_CROP, MV_CROP, 0, 0, false};
     if (is_u8) {
         if (H < 1 || W < 1) return fail(VF_ERR_INVALID, "mvit_forward: frame size %dx%d", H, W);
         for (int i = 0; i < n; ++i)
             if (starts[i] < 0 || int64_t(starts[i]) + T > n_frames)
                 return fail(VF_ERR_INVALID, "mvit_forward: clip %d (frames %d..%d) outside the %d frames", i, starts[i],
                             starts[i] + T - 1, n_frames);
-        VF_TRY(vf_resize_geometry(H, W, MV_RESIZE, 1, &rh, &rw));     // Resize([256]): the short side to 256
-        cy = center_crop_offset(rh, MV_CROP);
-        cx = center_crop_offset(rw, MV_CROP);
+        VF_TRY(frame_geometry("mvit_forward", H, W, MV_RESIZE, MV_CROP, &g));     // Resize([256]), CenterCrop(224)
     }
     if (n == 0) return VF_OK;
     const int64_t per_clip = rows_of(7) * 768;
@@ -317,7 +315,7 @@ static int mv_forward(vf_mvit* h, const void* src, int is_u8, int n_frames, int 
             // the patch kernel reads the caller's frames in place: any frame span fits
             VF_TRY(clip_window("mvit_forward", starts + off, n - off, T, per_chunk, INT_MAX, &m, &lo, &hi, &st));
             const uint8_t* f0 = static_cast<const uint8_t*>(src) + int64_t(lo) * H * W * 3;
-            VF_TRY(mvit_patch_u8(f0, st, m, H, W, rh, rw, cy, cx, h->patches, s));
+            VF_TRY(mvit_patch_u8(f0, st, m, H, W, g.rh, g.rw, g.cy, g.cx, h->patches, s));
         } else {
             m = std::min(per_chunk, n - off);
             VF_TRY(mvit_patch_f32(static_cast<const float*>(src) + int64_t(off) * 3 * T * MV_CROP * MV_CROP, m,

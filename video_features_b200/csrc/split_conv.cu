@@ -16,6 +16,11 @@ const vf_named_tensor* ResTensors::find(const std::string& name) const {
     return nullptr;
 }
 
+int64_t ResTensors::numel(const std::string& name) const {
+    const vf_named_tensor* e = find(name);
+    return e ? e->numel : -1;
+}
+
 int ResTensors::get(const std::string& name, int64_t numel, const float** out) const {
     const vf_named_tensor* e = find(name);
     if (!e) return fail(VF_ERR_INVALID, "%s: missing tensor '%s'", who, name.c_str());
@@ -220,13 +225,6 @@ int upload_split_mat(EngineCore* h, const ResTensors& T, const std::string& name
     VF_TRY(ralloc(h, dst, tmp.size()));
     VF_CUDA(cudaMemcpy(*dst, tmp.data(), tmp.size() * sizeof(__half), cudaMemcpyHostToDevice));
     return VF_OK;
-}
-
-GemmEpi linear_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate) {
-    GemmEpi e;
-    memset(&e, 0, sizeof(e));
-    e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.bias = bias; e.act = act; e.accumulate = accumulate;
-    return e;
 }
 
 int split_linear(const __half* A, int M, int N, int K, const __half* W2, const GemmEpi& ep, cudaStream_t s) {

@@ -26,6 +26,7 @@ struct ResConv {
 struct ResTensors {
     const vf_named_tensor* t; int n; const char* who;
     const vf_named_tensor* find(const std::string& name) const;     // null when absent
+    int64_t numel(const std::string& name) const;                   // -1 when absent
     int get(const std::string& name, int64_t numel, const float** out) const;
     // output channels of the (1,3,3) conv `name` over ci input channels: its weight is [co][ci][1][3][3]
     int spatial_width(const std::string& name, int ci, int* co) const;
@@ -83,7 +84,6 @@ int upload_vec(EngineCore* h, const ResTensors& T, const std::string& name, int6
 // lo = fp16(w - hi), round-to-nearest-even
 int upload_split_mat(EngineCore* h, const ResTensors& T, const std::string& name, int64_t rows, int64_t cols,
                      __half** dst, int64_t cols_pad = 0);
-GemmEpi linear_epi(void* out, int ldo, int out_f32, const float* bias, int act, int accumulate = 0);
 // out = A[M, K] . (W_hi + W_lo)^T with the epilogue `ep`: a 1-tap split-weight linear on the conv-mode GEMM (A rows of
 // pitch K, no row mask), as clip_resnet.cu's linears
 int split_linear(const __half* A, int M, int N, int K, const __half* W2, const GemmEpi& ep, cudaStream_t s);

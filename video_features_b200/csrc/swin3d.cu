@@ -238,16 +238,14 @@ static int sw_forward(vf_swin3d* h, const void* src, int is_u8, int n_frames, in
     if (per_chunk < 1)
         return fail(VF_ERR_INVALID, "swin3d_forward: a %d-frame clip exceeds the workspace (%d clips x %d frames)", T,
                     h->max_clips, h->max_T);
-    int rh = SW_CROP, rw = SW_CROP, cy = 0, cx = 0;
+    FrameGeom g{SW_CROP, SW_CROP, 0, 0, false};
     if (is_u8) {
         if (H < 1 || W < 1) return fail(VF_ERR_INVALID, "swin3d_forward: frame size %dx%d", H, W);
         for (int i = 0; i < n; ++i)
             if (starts[i] < 0 || int64_t(starts[i]) + T > n_frames)
                 return fail(VF_ERR_INVALID, "swin3d_forward: clip %d (frames %d..%d) outside the %d frames", i, starts[i],
                             starts[i] + T - 1, n_frames);
-        VF_TRY(vf_resize_geometry(H, W, SW_RESIZE, 1, &rh, &rw));     // Resize([256]): the short side to 256
-        cy = center_crop_offset(rh, SW_CROP);
-        cx = center_crop_offset(rw, SW_CROP);
+        VF_TRY(frame_geometry("swin3d_forward", H, W, SW_RESIZE, SW_CROP, &g));     // Resize([256]), CenterCrop(224)
     }
     if (n == 0) return VF_OK;
     const int C8 = 8 * h->dim;
@@ -261,7 +259,7 @@ static int sw_forward(vf_swin3d* h, const void* src, int is_u8, int n_frames, in
             // the patch kernel reads the caller's frames in place: any frame span fits
             VF_TRY(clip_window("swin3d_forward", starts + off, n - off, T, per_chunk, INT_MAX, &m, &lo, &hi, &st));
             const uint8_t* f0 = static_cast<const uint8_t*>(src) + int64_t(lo) * H * W * 3;
-            VF_TRY(swin3d_patch_u8(f0, st, m, T, H, W, rh, rw, cy, cx, h->patches, s));
+            VF_TRY(swin3d_patch_u8(f0, st, m, T, H, W, g.rh, g.rw, g.cy, g.cx, h->patches, s));
         } else {
             m = std::min(per_chunk, n - off);
             VF_TRY(swin3d_patch_f32(static_cast<const float*>(src) + int64_t(off) * 3 * T * SW_CROP * SW_CROP, m, T,
