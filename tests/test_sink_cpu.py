@@ -115,10 +115,12 @@ def _ns(tmp_path, **kw):
 
 
 @pytest.mark.parametrize("mode", ["default", "async", "resume"])
-def test_extractor_forward_loops_with_stubbed_engines(tmp_path, monkeypatch, mode):
+def test_extractor_forward_loops_with_stubbed_engines(tmp_path, monkeypatch, capsys, mode):
     from video_features_b200.extract.extract_clip import ExtractCLIP
     from video_features_b200.extract.extract_i3d import ExtractI3D
     from video_features_b200.extract.extract_raft import ExtractRAFT
+    from video_features_b200.extract.extract_s3d import ExtractS3D
+    from video_features_b200.extract.extract_vggish import ExtractVGGish
     monkeypatch.delenv("VF_ASYNC_SINK", raising=False)
     monkeypatch.delenv("VF_RESUME", raising=False)
     if mode == "async":
@@ -130,7 +132,7 @@ def test_extractor_forward_loops_with_stubbed_engines(tmp_path, monkeypatch, mod
             video = a[-1] if a else k.get('video_path')
             video = k.get('video_path', video)
             calls.append((key, os.path.basename(str(video))))
-            if os.path.basename(str(video)) == "b.mp4":
+            if os.path.splitext(os.path.basename(str(video)))[0] == "b":
                 raise RuntimeError("decoder says no")                  # per-video catch-print-continue
             return _feats(key)
         return f
@@ -170,6 +172,35 @@ def test_extractor_forward_loops_with_stubbed_engines(tmp_path, monkeypatch, mod
     monkeypatch.setattr(ExtractRAFT, "extract", fake_extract('raft'))
     assert er(_FakeIndices([0, 1, 2])) is None
     assert sorted(os.listdir(out / "raft")) == ["a_raft.npy", "c_raft.npy"] and len(calls) == 3
+
+    # a stack extractor (S3D): files under <output_path>/s3d, and the kept feature dicts are returned
+    calls.clear()
+    es = ExtractS3D(_ns(tmp_path, feature_type='s3d'))
+    monkeypatch.setattr(ExtractS3D, "extract", fake_extract('s3d'))
+    es.keep_features = True
+    capsys.readouterr()
+    got = es(_FakeIndices([0, 1, 2]))
+    assert sorted(os.listdir(out / "s3d")) == ["a_s3d.npy", "c_s3d.npy"] and len(calls) == 3
+    assert len(got) == 2 and set(got[0]) == {'s3d', 'fps', 'timestamps_ms'}
+    b = str(tmp_path / "b.mp4")
+    assert f"Extraction failed at: {b} with error (↑). Continuing extraction" in capsys.readouterr().out
+
+    # VGGish (output_direct: <output_path>/vggish_torch/<stem>.npy, for the resume check too)
+    calls.clear()
+    wavs = []
+    for n in ("a.wav", "b.wav", "c.wav"):
+        (tmp_path / n).write_bytes(b"x")
+        wavs.append(str(tmp_path / n))
+    ev = ExtractVGGish(_ns(tmp_path, feature_type='vggish_torch', video_paths=wavs, output_direct=True))
+    monkeypatch.setattr(ExtractVGGish, "extract", fake_extract('vggish_torch'))
+    if mode == "resume":
+        (out / "vggish_torch").mkdir()
+        np.save(out / "vggish_torch" / "a.npy", np.zeros((1, 3), np.float32))
+        monkeypatch.setenv("VF_RESUME", "1")
+    assert ev(_FakeIndices([0, 1, 2])) == []
+    assert sorted(os.listdir(out / "vggish_torch")) == ["a.npy", "c.npy"]
+    assert [c[1] for c in calls] == (["b.wav", "c.wav"] if mode == "resume" else ["a.wav", "b.wav", "c.wav"])
+    assert f"Extraction failed at: {wavs[1]}. Continuing extraction" in capsys.readouterr().out
 
 
 class _FakeClipEngine:

@@ -10,18 +10,16 @@ Normalize(0.45, 0.225)).  The output key is the feature type; rows are float32 `
 ``{output_path}/{feature_type}``.
 
 Decoding, pinned staging, the asynchronous engine calls (vf_mvit_forward_u8), the one device->host copy per video and
-``--show_pred`` (``head.1`` through class_head.py, Kinetics top-5 per stack) are ExtractSwin3D's.
+``--show_pred`` (``head.1`` through class_head.py, Kinetics top-5 per stack) are base.StackExtractor's.
 """
 from __future__ import annotations
 
-import glob
-import os
 from typing import Dict
 
 import torch
 
 from ..mvit_engine import MViTEngine
-from .extract_resnet import checkpoint_dirs
+from .base import load_first
 from .extract_swin3d import CLIPS_PER_CALL, ExtractSwin3D
 
 MVIT_KEYS = ("head.1.weight", "head.1.bias")      # torchvision MViT.head: Sequential(Dropout, Linear(768, 400))
@@ -32,22 +30,15 @@ _STATE_DICTS: Dict[str, Dict[str, torch.Tensor]] = {}
 
 
 def load_mvit_weights(feature_type: str) -> Dict[str, torch.Tensor]:
-    """The first checkpoint matching PATTERNS[feature_type] in checkpoint_dirs() ($VF_CKPT_DIR, then
+    """The first checkpoint matching PATTERNS[feature_type] in base.checkpoint_dirs() ($VF_CKPT_DIR, then
     $TORCH_HOME/hub/checkpoints, where torchvision stores it); read from disk once per process."""
     if feature_type not in _STATE_DICTS:
-        dirs, pattern = checkpoint_dirs(), PATTERNS[feature_type]
-        for d in dirs:
-            found = sorted(glob.glob(os.path.join(d, pattern)))
-            if found:
-                _STATE_DICTS[feature_type] = torch.load(found[0], map_location="cpu")
-                break
-        else:
-            raise FileNotFoundError(f"{pattern} not found in {dirs} (set VF_CKPT_DIR or TORCH_HOME)")
+        _STATE_DICTS[feature_type] = load_first(PATTERNS[feature_type])
     return _STATE_DICTS[feature_type]
 
 
 class ExtractMViT(ExtractSwin3D):
-    patterns = PATTERNS
+    feature_types = tuple(PATTERNS)
     head_keys = MVIT_KEYS
     default_stack = MVIT_STACK_SIZE
     default_step = MVIT_STACK_SIZE

@@ -13,69 +13,37 @@ from typing import Dict
 
 import numpy as np
 import torch
-from tqdm import tqdm
 
 from .. import ops
 from .._lib import VF_FILTER_BILINEAR
 from ..raft_engine import RAFTEngine
-from ..utils import AsyncSink, action_on_extraction, already_extracted, form_list_from_user_input
+from .base import Extractor, device_index
 from .extract_i3d import load_checkpoint
 
 
-# attributes the reference's constructor copies from `args` unchanged (extract_raft.py:24-36)
-_ARG_ATTRS = ('feature_type', 'batch_size', 'extraction_fps', 'resize_to_smaller_edge', 'side_size', 'show_pred',
-              'keep_tmp_files', 'on_extraction')
-
-
-class ExtractRAFT(torch.nn.Module):
+class ExtractRAFT(Extractor):
 
     def __init__(self, args):
-        super().__init__()
-        for name in _ARG_ATTRS:
-            setattr(self, name, getattr(args, name))
-        self.path_list = form_list_from_user_input(args)
-        # per-feature sub-folders of the scratch and output roots, as the reference lays them out
-        self.tmp_path, self.output_path = (os.path.join(root, self.feature_type) for root in (args.tmp_path, args.output_path))
-        self.progress = tqdm(total=len(self.path_list))
-        if self.extraction_fps is not None:
-            raise NotImplementedError("extraction_fps re-encodes with ffmpeg (outside the rebuilt path, SURVEY.md §2)")
+        super().__init__(args)
+        # attributes the reference's constructor copies from `args` unchanged (extract_raft.py:24-36)
+        self.batch_size = args.batch_size
+        self.resize_to_smaller_edge = args.resize_to_smaller_edge
+        self.side_size = args.side_size
         self._engines: Dict[int, tuple] = {}              # device index -> (engine, (frames, h, w) capacity)
         # pairs per engine call: frame pairs are independent, so how many share a call does not change any value; the
         # reference's default of one pair per call (--batch_size 1) would leave the GPU idle between launches
         self.pairs_per_call = max(self.batch_size, int(os.environ.get("VF_RAFT_PAIRS", "16")))
 
     def forward(self, indices: torch.LongTensor):
-        device = indices.device
-        if device.type != 'cuda':
-            raise RuntimeError("the H100 engine has no CPU path: pass indices on a CUDA device")
-        sink = AsyncSink() if os.environ.get("VF_ASYNC_SINK") == "1" else None     # opt-in extras, see ExtractCLIP.forward
-        resume = os.environ.get("VF_RESUME") == "1"
-        try:
-            for idx in indices:
-                video = self.path_list[idx]
-                try:                                      # per-video catch-print-continue (extract_raft.py:60-75)
-                    if resume and already_extracted([self.feature_type], video, self.output_path, self.on_extraction):
-                        self.progress.update()
-                        continue
-                    feats = self.extract(device, None, video)
-                    if sink is not None:
-                        sink.submit(feats, video, self.output_path, self.on_extraction)
-                    else:
-                        action_on_extraction(feats, video, self.output_path, self.on_extraction)
-                except KeyboardInterrupt:
-                    raise
-                except Exception as err:
-                    print(err)
-                    print(f'Extraction failed at: {video} with error (↑). Continuing extraction')
-                self.progress.update()
-        finally:
-            if sink is not None:
-                sink.close()
+        self._run(indices, keep=False)                    # returns None and keeps no features, as the reference's
+
+    def extract_video(self, device, video_path):
+        return self.extract(device, None, video_path)
 
     def _engine(self, device: torch.device, h: int, w: int) -> RAFTEngine:
         """One engine per device.  Its workspace is sized for the largest frame seen so far; a larger frame closes it
         and creates a bigger one (a list of many resolutions must not accumulate engines until cudaMalloc fails)."""
-        idx = device.index if device.index is not None else torch.cuda.current_device()
+        idx = device_index(device)
         eng, cap = self._engines.get(idx, (None, (0, 0, 0)))
         if eng is None or h > cap[1] or w > cap[2]:
             if eng is not None:
