@@ -11,7 +11,13 @@ holds the residual update of one block run alone on the oracle's stream: those f
 tight enough that weights rounded to fp16 exceed it (BLOCK_SEPARATION, rel-L2).  A lost lo half must exceed the
 embedding bar by SEPARATION."""
 FEATURES = {384: (7e-4, 9e-4), 768: (7e-4, 9e-4), 1024: (7e-4, 9e-4), 1536: (1e-3, 1e-3)}
-BARS = {"embed": (3e-6, 4e-6), "blocks": (1.1e-3, 1.3e-3), "block": (2.6e-4, 5e-4), "head": (3e-7, 4e-7)}
+BARS = {"embed": (3e-6, 4e-6), "blocks": (1.1e-3, 1.3e-3), "block": (2.6e-4, 5e-4), "head": (3e-7, 4e-7),
+        "attention": (6e-5, 1e-3), "attention hard": (4e-5, 1e-3)}
+# the attention kernel alone (vitl_attention, tests/test_attention_hard_gpu.py) against the float64 reference of its
+# declared rounding (tests/attention_ref.py) at 257 / 261 tokens and 6 / 12 / 16 / 24 heads.  Measured on the H100 80GB
+# HBM3 (700 W): random frames 3.1e-5 / 4.8e-4, hard ones (scores in the hundreds) 1.9e-5 / 5.0e-4; the max-abs part is
+# one fp16 ulp of the output, so its bar is two.  The kernel built without the rescale of its output measured
+# 1.0 / 1.8 or more.
 PROJECT = (1e-3, 1e-3)
 SEPARATION = 3.0
 # "block" is 1.14-1.6x the engine's measured worst (1.7-2.3e-4 rel-L2), not 2x, so that it works as a control: fp16

@@ -5,8 +5,8 @@ replay against eager, the window-attention kernel alone against float64, and the
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
+import attention_ref as A
 from oracle import swin3d_net as S
 from swin3d_bars import BARS, SEPARATION
 
@@ -89,34 +89,7 @@ def test_graph_replay_equals_eager(cuda_device, monkeypatch):
 def attention_ref(qkv, bias, table, shifted):
     """float64 window attention from a qkv matrix (n, T', H, W, 3C): the oracle's windowing, padded positions taking the
     qkv bias as their q / k / v (a zero row after norm1), q scaled by 32^-0.5, bias, -100 mask, softmax."""
-    n, t, h, w, c3 = qkv.shape
-    c, heads = c3 // 3, c3 // 96
-    win, sh = S.window_and_shift((t, h, w), shifted)
-    pad = [(win[i] - (t, h, w)[i] % win[i]) % win[i] for i in range(3)]
-    x = qkv.double() - bias.double()
-    x = F.pad(x, (0, 0, 0, pad[2], 0, pad[1], 0, pad[0])) + bias.double()
-    tp, hp, wp = x.shape[1:4]
-    if sum(sh):
-        x = torch.roll(x, shifts=(-sh[0], -sh[1], -sh[2]), dims=(1, 2, 3))
-    nw = (tp // win[0]) * (hp // win[1]) * (wp // win[2])
-    vol = win[0] * win[1] * win[2]
-    x = x.view(n, tp // win[0], win[0], hp // win[1], win[1], wp // win[2], win[2], c3)
-    x = x.permute(0, 1, 3, 5, 2, 4, 6, 7).reshape(n * nw, vol, 3, heads, 32)
-    q, k, v = x.permute(2, 0, 3, 1, 4)
-    attn = (q * 32 ** -0.5) @ k.transpose(-2, -1)
-    attn = attn + table.double()[S.bias_index(win).reshape(-1).to(qkv.device)].view(vol, vol, heads).permute(2, 0, 1)
-    if sum(sh):
-        reg = S.region_ids((tp, hp, wp), win, sh).to(qkv.device)
-        reg = reg.view(tp // win[0], win[0], hp // win[1], win[1], wp // win[2], win[2]).permute(0, 2, 4, 1, 3, 5)
-        reg = reg.reshape(nw, vol)
-        mask = torch.where(reg[:, None, :] != reg[:, :, None], -100.0, 0.0).double()
-        attn = (attn.view(n, nw, heads, vol, vol) + mask[None, :, None]).view(n * nw, heads, vol, vol)
-    y = (attn.softmax(-1) @ v).transpose(1, 2).reshape(n, tp // win[0], hp // win[1], wp // win[2], win[0], win[1],
-                                                       win[2], c)
-    y = y.permute(0, 1, 4, 2, 5, 3, 6, 7).reshape(n, tp, hp, wp, c)
-    if sum(sh):
-        y = torch.roll(y, shifts=(sh[0], sh[1], sh[2]), dims=(1, 2, 3))
-    return y[:, :t, :h, :w]
+    return A.swin3d(qkv, bias, table, shifted, rounding=False, key_block=None)
 
 
 # (C, T', H = W): every stage's (heads, spatial extent) at an unpadded, a padded and a clamped T'
