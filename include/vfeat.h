@@ -654,6 +654,46 @@ int vf_dinov2_swiglu(const float* ab, int rows, int hidden, void* out, void* str
 int vf_dinov2_attention(const void* qkv, int n, int S, int heads, void* out, void* stream);
 int64_t vf_dinov2_launch_count(const vf_dinov2_t* h);
 
+/* ---- VideoMAE clip features: Hugging Face `VideoMAEForVideoClassification` (Kinetics-400 fine-tuned ViT-S / B / L,
+ * 16 frames at 224 px, 2-frame tubelets of 16 x 16 patches: 1568 tokens), the classifier's input
+ * fc_norm(mean over tokens of the last hidden state).  Weights: the checkpoint's tensors by key (videomae.*, fc_norm.*),
+ * HOST fp32, plus "position_embeddings", the (1568, D) fp32 sinusoid table, and "image_mean" / "image_std" (3 each), the
+ * processor's Normalize constants.  config: 6 floats, hidden size, depth, heads, MLP width, LayerNorm eps, qkv_bias
+ * (1: q_bias / v_bias required, 0: refused when present).  Hidden size
+ * 384, 768 or 1024 with head dim 64 is built; anything else, a missing key or a wrong size is refused naming it. */
+typedef struct vf_videomae vf_videomae_t;
+
+/* Workspace of max_clips clips (0 = 16; at most 64), about 31 MB per clip at ViT-B; a call runs in chunks. */
+int vf_videomae_create(vf_videomae_t** out, const vf_named_tensor* tensors, int n_tensors, const float* config,
+                       int device, int max_clips);
+int vf_videomae_destroy(vf_videomae_t* h);
+/* info receives 5 ints: D, depth, heads, MLP width, max_clips. */
+int vf_videomae_info(const vf_videomae_t* h, int* info);
+/* clips: n x 16 x 3 x 224 x 224 fp32 on the device (the processor's pixel_values), T == 16 -> out: n x D fp32. */
+int vf_videomae_forward_f32(vf_videomae_t* h, const float* clips, int n, int T, float* out, void* stream);
+/* transform fused: frames n_frames x H x W x 3 uint8 BGR on the device, any size; clip i is frames starts[i] ..
+ * starts[i] + 15 (host starts) -> Resize(shortest_edge 224, Pillow bilinear), center crop 224 at the floor of half the
+ * margin, BGR->RGB, rescale 1 / 255, Normalize.  Bit-identical to vf_videomae_forward_f32 on the same transformed
+ * clips. */
+int vf_videomae_forward_u8(vf_videomae_t* h, const uint8_t* frames, int n_frames, int H, int W, const int* starts, int n,
+                           int T, float* out, void* stream);
+/* Diagnostics, eagerly on the caller's stream, n <= max_clips: the tubelet rows (n x 1568 x 1536 fp16) of the u8 or
+ * f32 entry; the embedding of tubelet rows -> x_out n x 1568 x D fp32; blocks [layer_begin, layer_end) in place on x;
+ * fc_norm of the token mean of x -> out n x D. */
+int vf_videomae_debug_tubelets_u8(vf_videomae_t* h, const uint8_t* frames, int n_frames, int H, int W,
+                                  const int* starts, int n, void* tubelets, void* stream);
+int vf_videomae_debug_tubelets_f32(vf_videomae_t* h, const float* clips, int n, void* tubelets, void* stream);
+int vf_videomae_debug_embed(vf_videomae_t* h, const void* tubelets, int n, float* x_out, void* stream);
+int vf_videomae_debug_blocks(vf_videomae_t* h, float* x, int n, int layer_begin, int layer_end, void* stream);
+int vf_videomae_debug_head(vf_videomae_t* h, const float* x, int n, float* out, void* stream);
+/* Precision control: zero the lo half of every split-fp16 weight, so the engine runs plain fp16 weights (the tests show
+ * that their bars catch it).  Irreversible for the handle. */
+int vf_videomae_debug_drop_lo(vf_videomae_t* h);
+/* The attention the blocks use alone (wgmma): qkv n x S rows [q | k | v] of 3 x heads*64 fp16 -> out n x S x heads*64
+ * fp16, scale 1/8, no mask, 1 <= S <= 2048. */
+int vf_videomae_attention(const void* qkv, int n, int S, int heads, void* out, void* stream);
+int64_t vf_videomae_launch_count(const vf_videomae_t* h);
+
 /* ---- classifier head (--show_pred): replaces `model.fc(feats)` of models/resnet/extract_resnet.py:105-114 and
  * models/r21d/extract_r21d.py:113-121, I3D's conv3d_0c_1x1 + mean over time (models/i3d/i3d_src/i3d_net.py:266-274),
  * and the softmax + sort of utils/utils.py:19-47.  weight: n_classes x n_features, bias: n_classes, HOST fp32. */

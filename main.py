@@ -8,7 +8,8 @@ released ViT, 768-d features), which the reference does not offer either; ``--mo
 R(2+1)D-34 models for ``r21d_rgb``; ``swin3d_t`` / ``swin3d_s`` / ``swin3d_b`` are torchvision's Swin3D video
 transformers and ``mvit_v1_b`` / ``mvit_v2_s`` its Multiscale Vision Transformers (Kinetics-400 clip features);
 ``dinov2_vit{s,b,l,g}14`` and their ``_reg`` variants are DINOv2's self-supervised ViTs (per-frame features, the hub
-model's class token after its final norm).
+model's class token after its final norm); ``videomae_vit{s,b,l}16`` are the Kinetics-400 fine-tuned VideoMAE models in
+Hugging Face's layout (clip features, the classifier's input).
 ``--show_pred`` on the CLIP feature types is upstream video_features' zero-shot prediction: every frame's image feature
 against the text features of ``--pred_texts`` (default: "a photo of {name}" for the Kinetics-400 classes).
 """
@@ -24,7 +25,7 @@ SUPPORTED = ['i3d', 'raft', 'pwc', 'CLIP-ViT-B/32', 'CLIP-ViT-B/16', 'CLIP4CLIP-
              'resnet101', 'resnet152', 'r21d_rgb', 'vggish_torch', 's3d', 'CLIP-ViT-L/14', 'CLIP-ViT-L/14@336px',
              'swin3d_t', 'swin3d_s', 'swin3d_b', 'mvit_v1_b', 'mvit_v2_s', 'dinov2_vits14', 'dinov2_vitb14',
              'dinov2_vitl14', 'dinov2_vitg14', 'dinov2_vits14_reg', 'dinov2_vitb14_reg', 'dinov2_vitl14_reg',
-             'dinov2_vitg14_reg']
+             'dinov2_vitg14_reg', 'videomae_vits16', 'videomae_vitb16', 'videomae_vitl16']
 
 
 def build_extractor(args):
@@ -59,6 +60,9 @@ def build_extractor(args):
     if args.feature_type.startswith('dinov2_'):
         from video_features_b200.extract.extract_dinov2 import ExtractDINOv2
         return ExtractDINOv2(args)
+    if args.feature_type in ['videomae_vits16', 'videomae_vitb16', 'videomae_vitl16']:
+        from video_features_b200.extract.extract_videomae import ExtractVideoMAE
+        return ExtractVideoMAE(args)
     if args.feature_type == 'vggish_torch':
         from video_features_b200.extract.extract_vggish import ExtractVGGish
         return ExtractVGGish(args)
@@ -100,7 +104,7 @@ def parallel_feature_extraction(args):
 _FEATURE_TYPES = ('i3d vggish r21d_rgb resnet18 resnet34 resnet50 resnet101 resnet152 raft pwc CLIP-ViT-B/32 CLIP-ViT-B/16 '
                   'CLIP4CLIP-ViT-B-32 vggish_torch s3d CLIP-ViT-L/14 CLIP-ViT-L/14@336px swin3d_t swin3d_s swin3d_b mvit_v1_b mvit_v2_s '
                   'dinov2_vits14 dinov2_vitb14 dinov2_vitl14 dinov2_vitg14 dinov2_vits14_reg dinov2_vitb14_reg '
-                  'dinov2_vitl14_reg dinov2_vitg14_reg').split()
+                  'dinov2_vitl14_reg dinov2_vitg14_reg videomae_vits16 videomae_vitb16 videomae_vitl16').split()
 
 # (flag, argparse keywords): names, types, defaults, choices and dests are the reference's (main.py:93-149)
 _FLAGS = [

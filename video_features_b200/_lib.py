@@ -261,6 +261,22 @@ SIGNATURES = {
     "vf_dinov2_swiglu": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_dinov2_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "vf_dinov2_launch_count": (C.c_int64, [C.c_void_p]),
+    "vf_videomae_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(NamedTensor), C.c_int, C.POINTER(C.c_float),
+                                     C.c_int, C.c_int]),
+    "vf_videomae_destroy": (C.c_int, [C.c_void_p]),
+    "vf_videomae_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
+    "vf_videomae_forward_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_forward_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_int,
+                                         C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_debug_tubelets_u8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                                C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_debug_tubelets_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_debug_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_debug_blocks": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vf_videomae_debug_head": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_debug_drop_lo": (C.c_int, [C.c_void_p]),
+    "vf_videomae_attention": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vf_videomae_launch_count": (C.c_int64, [C.c_void_p]),
     "vf_head_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "vf_head_destroy": (C.c_int, [C.c_void_p]),
     "vf_head_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -307,7 +307,7 @@ int resize_frames(EngineCore* h, const uint8_t* frames, int n, int H, int W, con
     if (!g.resize) return VF_OK;
     VF_TRY(grow(h, &h->resized, &h->resized_cap, size_t(max_frames) * g.rh * g.rw * 3));
     VF_TRY(grow(h, &h->resize_tmp, &h->tmp_cap, size_t(max_frames) * H * g.rw * 3));
-    VF_TRY(resize_u8(frames, n, H, W, h->resized, g.rh, g.rw, VF_FILTER_BICUBIC, h->resize_tmp, s));
+    VF_TRY(resize_u8(frames, n, H, W, h->resized, g.rh, g.rw, g.filter, h->resize_tmp, s));
     h->launches += (g.rh != H) + (g.rw != W);
     *src = h->resized;
     return VF_OK;

@@ -100,8 +100,8 @@ int run_graphed(EngineCore* h, const GraphKey& key, const std::function<int()>& 
 
 // ---- the front end of the towers that take single frames (CLIP ViT-B / ViT-L / ResNet, DINOv2)
 // Resize(resize_to, bicubic) of the short side, then CenterCrop(crop): the resized size, the crop offset and whether the
-// frame is resized at all
-struct FrameGeom { int rh, rw, cy, cx; bool resize; };
+// frame is resized at all; filter: the Pillow filter resize_frames applies
+struct FrameGeom { int rh, rw, cy, cx; bool resize; int filter = VF_FILTER_BICUBIC; };
 int frame_geometry(const char* who, int H, int W, int resize_to, int crop, FrameGeom* g);
 // n u8 frames of (H, W) -> *src, the frames the patchify kernel reads ((g.rh, g.rw) each): the frames themselves, or
 // their Pillow-exact bicubic resize into h->resized (grown for max_frames frames)

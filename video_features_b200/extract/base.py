@@ -20,7 +20,7 @@ from __future__ import annotations
 import glob
 import os
 from collections import deque
-from typing import Callable, Dict, Iterable, Iterator, List, Sequence, Tuple
+from typing import Callable, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -270,6 +270,10 @@ class StackExtractor(Extractor):
     def new_engine(self, idx: int):
         raise NotImplementedError
 
+    def class_names(self) -> Optional[List[str]]:
+        """The --show_pred class names; None: the Kinetics-400 names."""
+        return None
+
     def new_head(self, idx: int) -> ClassHead:
         return ClassHead.from_state_dict(self.load_weights(), self.head_keys, idx, f"{self.feature_type} checkpoint")
 
@@ -308,7 +312,7 @@ class StackExtractor(Extractor):
                     def emit(tops, stacks=range(first, first + len(starts))):
                         for j, i in enumerate(stacks):
                             print(f'{video_path} @ frames ({i * step}, {i * step + T})')
-                            print_top_predictions(*(t[j:j + 1] for t in tops[0]), 'kinetics')
+                            print_top_predictions(*(t[j:j + 1] for t in tops[0]), 'kinetics', self.class_names())
                     preds.submit([(head, outs[-1])], emit)
             s ^= 1
         if preds is not None:

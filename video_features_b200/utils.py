@@ -274,6 +274,9 @@ def sanity_check(args: argparse.Namespace):
             raise AssertionError(f'--show_pred: the {args.feature_type} checkpoint is a backbone without a classifier')
         if args.stack_size is not None:
             raise AssertionError(f'--stack_size: {args.feature_type} gives one feature per frame; stacks do not apply')
+    if args.feature_type.startswith('videomae_') and args.stack_size is not None and args.stack_size != 16:
+        raise AssertionError(f'--stack_size: {args.feature_type} takes stacks of 16 frames (its positional table is '
+                             f'built for 16 frames); got {args.stack_size}')
     if args.show_pred:
         print('--show_pred: only the first of the listed GPUs is used')
         args.device_ids = args.device_ids[:1]
